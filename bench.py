@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""Benchmark of the TD-MPC2 planning hot path on B200 (contract: see DESIGN.md 'Measurement').
+"""Benchmark of the TD-MPC2 planning hot path on H100 (contract: see DESIGN.md 'Measurement').
 
     python bench.py --gpus 1 --steps 10 --warmup 3                    # this build, workload c2 (BASELINE configs[1])
     python bench.py --workload c3|c4|c5 ...                           # the other BASELINE configs (per-GPU share)
     python bench.py --impl reference --steps 5 --warmup 3             # the reference's plan() on the host cores
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
+    python bench.py --steps 10 --dump-outputs DIR                     # also write the last timed step's outputs as .npy
 
 A "step" is one full plan() over the batch of environments: noise draws, prologue (encode + policy-prior rollouts),
 I CEM iterations, epilogue -- and the action all-gather when the environment axis is sharded (N > 1).
@@ -19,7 +20,7 @@ Weak scaling: every rank plans its own share, so `--gpus 8` runs c4 / c5 exactly
 
 After the timed regions (never inside them) rank 0 adds: `parity_check` (environments OF THE TIMED BATCH re-planned
 with explicit noise and compared with the CPU oracle), `cpu_baseline`, and `gpu_baseline` (the same algorithm as
-batched eager PyTorch / cuBLAS on this GPU, and the reference's own `_plan` on this GPU when baseline/_ref exists).
+batched eager PyTorch / cuBLAS on this GPU, and the reference's own `_plan` on this GPU when oracle/_ref exists).
 """
 from __future__ import annotations
 
@@ -66,7 +67,7 @@ def load_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback: H100 SXM data sheet, dense, 700 W"
 
 
 class ClockSampler:
@@ -131,7 +132,7 @@ def _ref_available() -> bool:
 
 def _cpu_worker(args):
     """One host process: plans `envs` environments one after another (the reference has no env axis) with `threads`
-    intra-op threads; returns (seconds per env-plan, kind)."""
+    intra-op threads; returns (seconds per env-plan, kind, timed steps).  Stops early once `budget_s` is spent."""
     wl, envs, steps, warmup, threads, budget_s, use_ref, seed = args
     import torch as th
     th.set_num_threads(threads)
@@ -171,7 +172,7 @@ def _cpu_worker(args):
             if s >= warmup:
                 times.append(dt / envs)
         kind = "port"
-    return sum(times) / len(times), kind
+    return sum(times) / len(times), kind, len(times)
 
 
 def _cpu_layout_run(wl, steps, warmup, budget_s, procs, threads, use_ref):
@@ -185,7 +186,7 @@ def _cpu_layout_run(wl, steps, warmup, budget_s, procs, threads, use_ref):
             res = pool.map(_cpu_worker, jobs)
     t_env = statistics.mean(r[0] for r in res)
     value = sum(cfg.num_samples * cfg.horizon / r[0] for r in res)
-    return value, t_env, res[0][1]
+    return value, t_env, res[0][1], min(r[2] for r in res)
 
 
 def cpu_reference_run(wl: str, steps: int, warmup: int, budget_s: float):
@@ -194,7 +195,8 @@ def cpu_reference_run(wl: str, steps: int, warmup: int, budget_s: float):
     environments are independent, so the host layouts tried are processes x intra-op threads -- one process with
     16 threads, and process-parallel with 8 threads each over all cores -- and the BEST aggregate is reported.
     Every process plans its environments one after another (evaluate.py's loop; the reference has no env axis).
-    Returns (steps/s aggregate, seconds per env-plan of one process, cores used, kind, procs, all layouts tried)."""
+    Returns (steps/s aggregate, seconds per env-plan of one process, cores used, kind, procs, timed steps of that layout,
+    all layouts tried)."""
     host = os.cpu_count() or 1
     use_ref = _ref_available()
     layouts = [(1, min(16, host))]
@@ -205,11 +207,12 @@ def cpu_reference_run(wl: str, steps: int, warmup: int, budget_s: float):
         if t_first is not None and 12.0 * t_first * (warmup + 1) > 2.0 * budget_s and procs > 1:
             tried.append({"procs": procs, "threads": threads, "skipped": "would exceed the time budget"})
             continue
-        value, t_env, kind = _cpu_layout_run(wl, steps, warmup, budget_s, procs, threads, use_ref)
+        value, t_env, kind, n_steps = _cpu_layout_run(wl, steps, warmup, budget_s, procs, threads, use_ref)
         t_first = t_env if t_first is None else t_first
-        tried.append({"procs": procs, "threads": threads, "steps_per_s": round(value, 1), "s_per_env_plan": round(t_env, 3)})
+        tried.append({"procs": procs, "threads": threads, "steps_per_s": round(value, 1), "s_per_env_plan": round(t_env, 3),
+                      "timed_steps": n_steps})
         if best is None or value > best[0]:
-            best = (value, t_env, procs * threads, kind, procs)
+            best = (value, t_env, procs * threads, kind, procs, n_steps)
     return best + (tried,)
 
 
@@ -224,14 +227,15 @@ def run_reference(args):
     per_env_gflop = flops_per_env(cfg, heads_used=cfg.num_q) / 1e9
     budget = 150.0 if per_env_gflop < 200 else 240.0
     heavy = per_env_gflop > 1000                 # 317M presets: one env-plan is tens of seconds of host time
-    steps = 1 if heavy else max(1, min(args.steps, 20))
-    value, t_env, cores, kind, procs, tried = cpu_reference_run(wl, steps, 0 if heavy else min(args.warmup, 1), budget_s=budget)
-    src = ("the reference's own unmodified TDMPC2._plan (baseline/_ref via oracle/ref_harness.py)" if kind == "reference"
+    # --steps timed steps per process, unless the time budget runs out first; the line reports the count actually timed
+    value, t_env, cores, kind, procs, n_steps, tried = cpu_reference_run(wl, max(1, args.steps), 0 if heavy else min(args.warmup, 1),
+                                                                         budget_s=budget)
+    src = ("the reference's own unmodified TDMPC2._plan (oracle/_ref via oracle/ref_harness.py)" if kind == "reference"
            else "oracle port of the reference algorithm (reference sources not on this box)")
     sample = (f"{procs} processes x {cores // procs} threads, each planning 1 environment of the workload per step, "
               f"sequentially inside a process (the reference has no env axis); {src}")
     line = {
-        "impl": "reference", "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": args.gpus, "steps": args.steps,
+        "impl": "reference", "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": args.gpus, "steps": n_steps,
         "warmup": args.warmup, "ms_per_step": 1e3 * t_env, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": describe(wl, cfg, cfg.num_envs) + " (reference algorithm, host CPU, eager PyTorch fp32)",
@@ -319,7 +323,7 @@ def parity_check(cfg, sd, obs_host, task_host, E_local, dev, engine, envs, budge
 
 # ------------------------------------------------------------------------------------------------ GPU baselines (same box)
 def gpu_baselines(wl, cfg, dev, budget_s=40.0):
-    """SURVEY.md section 8(d)(ii)/(iii): what the library path does on the same B200 (never the product path)."""
+    """SURVEY.md section 8(d)(ii)/(iii): what the library path does on the same GPU (never the product path)."""
     out = {}
     try:
         import importlib.util
@@ -356,12 +360,12 @@ def gpu_baselines(wl, cfg, dev, budget_s=40.0):
             ms = statistics.median(times)
             out["reference_plan_eager_gpu"] = {"value": rcfg.num_samples * rcfg.horizon / (ms * 1e-3), "unit": UNIT,
                                                "ms_per_env_plan": ms, "calls": len(times),
-                                               "impl": "the reference's own unmodified TDMPC2._plan (baseline/_ref), eager, "
+                                               "impl": "the reference's own unmodified TDMPC2._plan (oracle/_ref), eager, "
                                                        "one environment per call (it has no env axis), fp32"}
             del agent
             torch.cuda.empty_cache()
         else:
-            out["reference_plan_eager_gpu"] = {"unavailable": "baseline/_ref (copy of the reference's planning files) not on this box"}
+            out["reference_plan_eager_gpu"] = {"unavailable": "oracle/_ref (copy of the reference's planning files) not on this box"}
     except Exception as e:
         out["reference_plan_error"] = repr(e)[:300]
     return out
@@ -411,6 +415,8 @@ def main():
     ap.add_argument("--rng", default="torch", choices=["torch", "philox"],
                     help="torch = the reference's noise draws (parity; the headline); philox = the DECLARED NON-PARITY throughput "
                          "mode: the two large noise tensors are generated inside the kernels (its own line; no oracle comparison)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (the actions, float32) as DIR/<name>.npy")
     ap.add_argument("--passes", type=int, default=3, choices=[1, 3],
                     help="3 = fp32-parity arithmetic (the headline); 1 = the DECLARED NON-PARITY fast mode (one fp16 MMA per "
                          "product): its own line, dtype f16, parity_check reports the elite-flip rate instead of gating")
@@ -477,12 +483,14 @@ def main():
         torch.cuda.synchronize()
 
     def timed(fn, steps):
-        """K steps between CUDA events, barrier + synchronize on both sides, max over ranks."""
+        """K steps between CUDA events, barrier + synchronize on both sides, max over ranks; also returns the last
+        step's result."""
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         barrier()
         e0.record()
+        out = None
         for _ in range(steps):
-            fn(False)
+            out = fn(False)
         e1.record()
         barrier()
         ms = e0.elapsed_time(e1)
@@ -490,7 +498,7 @@ def main():
             t = torch.tensor([ms], device=dev)
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
             ms = float(t.item())
-        return ms / steps
+        return ms / steps, out
 
     # ---- warm-up (first call t0=True, then steady-state warm starts; the first steady call captures the graph)
     step_device(True)
@@ -501,9 +509,14 @@ def main():
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    ms_step = timed(step_device, args.steps)
+    ms_step, last_actions = timed(step_device, args.steps)
     launches = agent.planner.launches - launches0
-    ms_e2e = timed(step_e2e, args.steps)
+    if args.dump_outputs and rank == 0:
+        # the actions of the last timed step, all environments (gathered when sharded): [E_total, action_dim] float32
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "actions.npy"), last_actions.float().cpu().numpy())
+    ms_e2e, _ = timed(step_e2e, args.steps)
     clocks = sampler.stop() if rank == 0 else {}
 
     # ---- dominant kernel: one CEM-iteration launch, timed alone with events on its stream
@@ -536,18 +549,6 @@ def main():
             dist.destroy_process_group()
         return
     peaks, peak_src = load_peaks()
-    traffic, traffic_src = None, None
-    try:   # DRAM bytes per launch of the dominant kernel, from the committed ncu --set full capture of this workload
-        sfx = "_pp" if agent.planner.iter_engine == "tcgen05pp" else ""       # one capture per engine
-        with open(os.path.join(ROOT, "profiles", f"r02_traffic_{wl}{sfx}.json")) as f:
-            tj = json.load(f)
-        if int(tj.get("envs", -1)) == E_local and args.passes == 3:
-            from tdmpc2_b200 import build as _b
-            traffic = tj["dram_bytes_per_launch"]
-            traffic_src = {"file": f"profiles/r02_traffic_{wl}{sfx}.json", "kernel_sources_unchanged_since_capture":
-                           tj.get("lib_digest") == _b._digest()}
-    except Exception:
-        traffic = None
     L, M, A_, T, B = cfg.latent_dim, cfg.mlp_dim, cfg.action_dim, cfg.task_dim, cfg.num_bins
     D = L + T + A_
     w = lambda i, h, o: i * h + h * h + h * o
@@ -564,8 +565,8 @@ def main():
         "dtype": "f32" if args.passes == 3 else "f16", "data": "synthetic",
         "config": {"workload": describe(wl, cfg, E_local),
                    "global_envs": E_total, "parallelism": f"env-shard x{world}", "engine": agent.planner.iter_engine,
-                   "arithmetic": "3-pass fp16-split operands on tcgen05 kind::f16, fp32 accumulate (fp32-parity mode)" if args.passes == 3
-                                 else "DECLARED NON-PARITY fast mode: single-pass fp16 operands on tcgen05 kind::f16, fp32 accumulate",
+                   "arithmetic": "3-pass fp16-split operands on wgmma f16, fp32 accumulate (fp32-parity mode)" if args.passes == 3
+                                 else "DECLARED NON-PARITY fast mode: single-pass fp16 operands on wgmma f16, fp32 accumulate",
                    "rng": "torch CUDA generator (reference draw semantics)" if args.rng == "torch"
                           else "DECLARED NON-PARITY: in-kernel Philox4x32-10 + Box-Muller for noise_r / noise_pi",
                    "launch": "CUDA-graph replay of prologue -> I x iter -> epilogue" if agent._use_graph and not args.no_graph
@@ -579,10 +580,8 @@ def main():
                 "h2d_bytes_per_step": int(E_local * obs_dim * 4), "d2h_bytes_per_step": int(E_total * A_ * 4)},
         "gpu_launches": int(launches),
         "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                     "frac_vs_sustained": achieved / float(peaks.get("bf16_tflops_sustained", peak)),
-                     "traffic": traffic, "traffic_source": traffic_src,
-                     "kernel": ("plan_pp_kernel" if agent.planner.iter_engine == "tcgen05pp" else "plan_kernel<tcgen05, pair>") + " (one CEM iteration)",
-                     "ms_per_launch": ms_iter, "peak_source": f"MEASURED_PEAKS.json bf16_tflops ({peak_src}, burst)",
+                     "kernel": f"plan_kernel<{agent.planner.iter_engine}> (one CEM iteration)",
+                     "ms_per_launch": ms_iter, "peak_source": f"MEASURED_PEAKS.json bf16_tflops ({peak_src})",
                      "flop_per_launch": flops_iter,
                      "note": ("achieved counts ALGORITHMIC flops (2 Q heads, 1x); the fp32-parity path issues 3 fp16 MMAs "
                               "per product, so its ceiling is peak/3") if args.passes == 3 else
@@ -614,7 +613,7 @@ def main():
             line["gpu_baseline"] = gpu_baselines(wl, cfg, dev)
         if not args.no_cpu_baseline:
             heavy = flops_per_env(cfg, heads_used=cfg.num_q) > 1e12
-            v, t_env, cores, kind, procs, tried = cpu_reference_run(wl, steps=1 if heavy else 3, warmup=0 if heavy else 1, budget_s=15.0)
+            v, t_env, cores, kind, procs, _, tried = cpu_reference_run(wl, steps=1 if heavy else 3, warmup=0 if heavy else 1, budget_s=15.0)
             line["cpu_baseline"] = {"value": v, "unit": UNIT, "cores": cores, "kind": kind, "host_cores": os.cpu_count(), "layouts_tried": tried,
                                     "sample": f"{procs} processes x {cores // procs} threads, each planning 1 environment of the workload "
                                               f"per step (best of the host layouts tried), sequential inside a process (reference has no env axis), eager PyTorch fp32; "

@@ -6,7 +6,7 @@
  * (packed weights, workspace).  A real host then allocates them (cudaMalloc), calls tdmpc2_planner_bind(),
  * fills a tdmpc2_weights with device pointers to the checkpoint tensors, tdmpc2_pack_weights(), and per environment
  * step runs tdmpc2_plan_prologue() -> iterations x tdmpc2_plan_iter() -> tdmpc2_plan_epilogue() on its stream
- * (INTEGRATION.md section 2).  Without an sm_100 device tdmpc2_planner_create() fails with TDMPC2_ERR_NO_DEVICE:
+ * (INTEGRATION.md section 2).  Without an sm_90 device tdmpc2_planner_create() fails with TDMPC2_ERR_NO_DEVICE:
  * there is no CPU fallback. */
 #include <stdio.h>
 #include <string.h>
@@ -28,7 +28,7 @@ int main(void) {
   int rc = tdmpc2_planner_create(&d, &p);
   if (rc != TDMPC2_OK) {
     printf("tdmpc2_planner_create: %d (%s)\n", rc, tdmpc2_last_error());
-    return rc == TDMPC2_ERR_NO_DEVICE ? 0 : 1;   /* expected on a machine without a B200 */
+    return rc == TDMPC2_ERR_NO_DEVICE ? 0 : 1;   /* expected on a machine without a H100 */
   }
   size_t packed = 0, ws = 0;
   tdmpc2_planner_packed_bytes(p, &packed);

@@ -1,5 +1,5 @@
 /*
- * tdmpc2_b200.h -- C ABI of the B200-native TD-MPC2 planning hot path.
+ * tdmpc2_b200.h -- C ABI of the H100-native TD-MPC2 planning hot path.
  *
  * The reference (nicklashansen/tdmpc2) has no FFI / plugin API: its planner is
  * the Python method TDMPC2._plan (tdmpc2/tdmpc2.py:138-206) calling
@@ -19,7 +19,7 @@
  *   - fp32 tensors, int32 task / q-head indices, uint8 flags, int64 elite
  *     indices (torch.topk's dtype);
  *   - there is NO CPU fallback: every call fails with TDMPC2_ERR_NO_DEVICE
- *     unless the current device is sm_100 (B200).
+ *     unless the current device is sm_90 (H100).
  *
  * Batched semantics (new in this build): a leading environment axis E.  Each
  * environment is one independent reference _plan call (own obs, task, t0,
@@ -44,7 +44,7 @@ extern "C" {
 typedef enum tdmpc2_status {
   TDMPC2_OK = 0,
   TDMPC2_ERR_INVALID = -1,     /* bad dims / null pointer / unsupported config */
-  TDMPC2_ERR_NO_DEVICE = -2,   /* no CUDA device, or device is not sm_100      */
+  TDMPC2_ERR_NO_DEVICE = -2,   /* no CUDA device, or device is not sm_90      */
   TDMPC2_ERR_CUDA = -3,        /* a CUDA runtime / driver call failed          */
   TDMPC2_ERR_STATE = -4,       /* call order violated (e.g. plan before bind)  */
   TDMPC2_ERR_UNSUPPORTED = -5  /* config outside what the reference's planner itself accepts (multi-task episodic) */
@@ -52,19 +52,13 @@ typedef enum tdmpc2_status {
 
 /* GEMM engine used by the fused MLP kernels. */
 typedef enum tdmpc2_engine {
-  TDMPC2_ENGINE_TCGEN05 = 0,   /* TMA + tcgen05.mma (3x fp16-split, fp32 TMEM accumulate): the product path */
+  TDMPC2_ENGINE_TCGEN05 = 0,   /* TMA + wgmma (3x fp16-split, fp32 register accumulate): the product path */
   TDMPC2_ENGINE_SIMT = 1,      /* CUDA-core fp32 FFMA over the same packed operands: bring-up / diagnostics  */
-  TDMPC2_ENGINE_TCGEN05_2SM = 2, /* as 0, but CEM iterations run on CTA pairs (tcgen05 cta_group::2, M = 256):
-                                  each CTA streams half of every weight tile.  Falls back to 0 when a model has
-                                  layers wider than TMEM or an odd number of 128-row tiles per environment */
-  TDMPC2_ENGINE_TCGEN05_PP = 3, /* as 2, but every CTA splits its tile into two 64-row halves (cta_group::2, M = 128)
-                                  whose accumulators sit side by side in TMEM: the GEMM of one half overlaps the
-                                  LayerNorm / head epilogue of the other.  Trunk layers must be 256 or 512 wide and
-                                  heads at most 128 (the 5M preset); anything else runs as engine 2 */
-  TDMPC2_ENGINE_TCGEN05_2SM_PF = 4 /* as 2 (bit-identical results), but the TMA producer prefetches the next layer's first
-                                  weight chunks into the idle W ring during the epilogue, which then stages its output
-                                  in the A ring.  Episodic models or LayerNorm widths that are not multiples of 32
-                                  run as engine 2 */
+  /* Engines 2 - 4 (CTA pairs, ping-pong halves, weight prefetch) were designed around cta_group::2 MMAs, which sm_90a
+     does not have.  They are accepted and run as engine 0 (tdmpc2_planner_iter_engine reports 0). */
+  TDMPC2_ENGINE_TCGEN05_2SM = 2,
+  TDMPC2_ENGINE_TCGEN05_PP = 3,
+  TDMPC2_ENGINE_TCGEN05_2SM_PF = 4
 } tdmpc2_engine;
 
 /* Planner + model dimensions.  Mirrors the keys the reference reads from cfg:
@@ -128,7 +122,7 @@ int tdmpc2_abi_version(void);
 const char* tdmpc2_last_error(void);
 
 /* Validates dims, lays out the packed-weight blob and the workspace.  Needs a
- * current sm_100 device (queries SM count).  No device memory is allocated. */
+ * current sm_90 device (queries SM count).  No device memory is allocated. */
 int tdmpc2_planner_create(const tdmpc2_dims* dims, tdmpc2_planner** out);
 void tdmpc2_planner_destroy(tdmpc2_planner* p);
 int tdmpc2_planner_packed_bytes(const tdmpc2_planner* p, size_t* out);
@@ -144,19 +138,16 @@ int tdmpc2_planner_iter_engine(const tdmpc2_planner* p);
  * persisting part of L2 (sets the DEVICE-wide cudaLimitPersistingL2CacheSize, hence opt-in); 0 switches it off.
  * No reference counterpart (the reference's activations are ordinary torch tensors). */
 int tdmpc2_planner_set_l2_persist(tdmpc2_planner* p, int enable);
-/* Accuracy knob of layers wider than 512 outputs (48M / 317M presets).  The tensor core's fp32 accumulator rounds toward
- * zero on every K = 16 step, so its error grows with the reduction length K; with k_elems > 0 the partial sums are
- * flushed to fp32 every k_elems elements of K and added with round-to-nearest (one extra accumulator drain per
- * segment).  Default 2048; 0 = whole K in one accumulation.  No reference counterpart. */
+/* Reduction-segment knobs (k_elems >= 0) of the wide layers and of the head layers.  The wgmma engine already adds the
+ * partial sum of every 64-element K-chunk with round-to-nearest, so on this build they validate their argument and
+ * change nothing.  No reference counterpart. */
 int tdmpc2_planner_set_kseg(tdmpc2_planner* p, int k_elems);
-/* The same for the head layers (reward / Q / pi / termination outputs, which have no LayerNorm behind them to absorb
- * the accumulator's toward-zero drift): default 512, 0 = whole K in one accumulation. */
 int tdmpc2_planner_set_head_kseg(tdmpc2_planner* p, int k_elems);
-/* Arithmetic of the tcgen05 engines 0 / 2 / 4.  passes = 3 (default): every product is three fp16 MMAs over the hi / lo
+/* Arithmetic of the tensor-core engine 0.  passes = 3 (default): every product is three fp16 MMAs over the hi / lo
  * operand planes -- the mode whose results match the reference's fp32 plan() (tdmpc2.py:138-206) within 1e-4.
  * passes = 1: DECLARED NON-PARITY fast mode -- hi planes only (one fp16 MMA per product, fp32 accumulate; ~1e-3
  * value error, elite sets differ from the reference's): for throughput studies, never the headline number.
- * Engines 1 (SIMT) and 3 (ping-pong) ignore it. */
+ * Engine 1 (SIMT) ignores it. */
 int tdmpc2_planner_set_passes(tdmpc2_planner* p, int passes);
 /* Replaces: agent.load()/WorldModel.to(device) weight placement (tdmpc2.py:81-95).
  * Packs the state-dict tensors into the kernel layout: per Linear two fp16

@@ -1,9 +1,9 @@
 """Harness that executes the REFERENCE's own planner code on CPU -- TEST INFRASTRUCTURE ONLY.
 
-Works only where the reference checkout exists (default /root/reference, i.e. in
-the build container; never on the GPU box).  Nothing from the reference is
-copied: its modules are imported from where they lie.  The recipe is the one
-verified in SURVEY.md section 8(c) / Appendix A:
+Works where the reference checkout exists (TDMPC2_REFERENCE_DIR, or a `reference`
+checkout next to this repository), or where `make_ref_build()` has left its
+byte-compiled planning modules under the git-ignored oracle/_ref/.  The recipe is
+the one verified in SURVEY.md section 8(c) / Appendix A:
 
   1. import-only stubs for `tensordict` (not installable here) so that
      common/layers.py, common/world_model.py and tdmpc2.py import;
@@ -30,31 +30,30 @@ import torch
 import torch.nn as nn
 
 _ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-# Where the reference's modules lie: the read-only checkout in the build container, or -- on the GPU box, where
-# /root/reference does not exist -- the git-ignored verbatim copy `baseline/_ref/tdmpc2` that `make_ref_copy()` (run by
-# __graft_entry__.build()) places next to the repo so that the unmodified reference can be timed beside the kernels.
-_CANDIDATES = [os.environ.get("TDMPC2_REFERENCE_DIR", ""), "/root/reference/tdmpc2",
-               os.path.join(_ROOT, "baseline", "_ref", "tdmpc2")]
-REF_DIR = next((d for d in _CANDIDATES if d and os.path.isfile(os.path.join(d, "tdmpc2.py"))), _CANDIDATES[1])
+# Where the reference's modules lie: its checkout, or the byte-compiled planning modules that `make_ref_build()` (run
+# by __graft_entry__.build()) leaves in the git-ignored oracle/_ref/tdmpc2, so that the unmodified reference can be timed
+# beside the kernels on a machine without the checkout.
+_SRC_CANDIDATES = [os.environ.get("TDMPC2_REFERENCE_DIR", ""), os.path.join(os.path.dirname(_ROOT), "reference", "tdmpc2")]
+SRC_DIR = next((d for d in _SRC_CANDIDATES if d and os.path.isfile(os.path.join(d, "tdmpc2.py"))), None)
+BUILD_DIR = os.path.join(_ROOT, "oracle", "_ref", "tdmpc2")
+REF_DIR = SRC_DIR or BUILD_DIR
 
 
-def make_ref_copy(src: str = "/root/reference/tdmpc2") -> bool:
-    """Copy the files of the reference's planning path (tdmpc2.py + common/*.py, unmodified) to baseline/_ref/tdmpc2
-    (git-ignored, travels to the GPU box with the snapshot).  No-op where the checkout does not exist."""
-    import shutil
-    if not os.path.isfile(os.path.join(src, "tdmpc2.py")):
+def make_ref_build() -> bool:
+    """Byte-compile the reference's planning path (tdmpc2.py + common/*.py, unmodified) into sourceless modules under
+    oracle/_ref/tdmpc2 (git-ignored).  No-op where the checkout does not exist."""
+    import py_compile
+    if SRC_DIR is None:
         return False
-    dst = os.path.join(_ROOT, "baseline", "_ref", "tdmpc2")
-    os.makedirs(os.path.join(dst, "common"), exist_ok=True)
-    shutil.copy2(os.path.join(src, "tdmpc2.py"), os.path.join(dst, "tdmpc2.py"))
-    for f in os.listdir(os.path.join(src, "common")):
-        if f.endswith(".py"):
-            shutil.copy2(os.path.join(src, "common", f), os.path.join(dst, "common", f))
+    os.makedirs(os.path.join(BUILD_DIR, "common"), exist_ok=True)
+    files = ["tdmpc2.py"] + [os.path.join("common", f) for f in sorted(os.listdir(os.path.join(SRC_DIR, "common"))) if f.endswith(".py")]
+    for f in files:
+        py_compile.compile(os.path.join(SRC_DIR, f), cfile=os.path.join(BUILD_DIR, f + "c"), doraise=True)
     return True
 
 
 def available() -> bool:
-    return os.path.isfile(os.path.join(REF_DIR, "tdmpc2.py"))
+    return any(os.path.isfile(os.path.join(REF_DIR, "tdmpc2" + ext)) for ext in (".py", ".pyc"))
 
 
 _mods = None

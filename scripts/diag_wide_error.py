@@ -11,7 +11,7 @@ from tdmpc2_b200.planner import Planner
 from oracle.plan_oracle import plan_oracle
 from helpers import mixed_noise
 wl = sys.argv[1] if len(sys.argv) > 1 else "c4"
-engines = sys.argv[2:] or ["tcgen05x2", "tcgen05", "simt"]
+engines = sys.argv[2:] or ["tcgen05", "simt"]
 E = 3
 cfg = workload(wl, num_envs=E, iterations=2)
 sd = synth_state_dict(cfg, seed=9)

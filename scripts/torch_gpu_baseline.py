@@ -1,6 +1,6 @@
 """Strong baseline for SURVEY.md section 8(d)(iii): the planner restated as BATCHED eager PyTorch (rows = E x N
 through the same torch ops the reference uses: F.linear / layer_norm / mish / softmax / topk), runnable on the
-same B200 as the fused kernels.  Measurement aid, not product code and not the parity oracle (that is
+same H100 as the fused kernels.  Measurement aid, not product code and not the parity oracle (that is
 oracle/plan_oracle.py; tests/test_torch_batched_baseline.py holds this file to it on CPU).
 
     python scripts/torch_gpu_baseline.py [--workload c2] [--envs 256] [--steps 5] [--device cuda:0]

@@ -1,4 +1,4 @@
-"""Builds the sm_100a C-ABI library in-tree (tdmpc2_b200/libtdmpc2_b200.so).
+"""Builds the sm_90a C-ABI library in-tree (tdmpc2_b200/libtdmpc2_b200.so).
 
 nvcc cross-compiles without a GPU; the .so is git-ignored but travels with the
 repo snapshot to the GPU box.  `python -m tdmpc2_b200.build` or
@@ -16,8 +16,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libtdmpc2_b200.so")
 STAMP = LIB + ".stamp"
-SOURCES = ["api.cu", "plan_kernels.cuh", "plan_pp.cuh", "ptx.cuh", os.path.join("..", "..", "include", "tdmpc2_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+SOURCES = ["api.cu", "plan_kernels.cuh", "pixel_encoder.cuh", "ptx.cuh", "rng.cuh",
+           os.path.join("..", "..", "include", "tdmpc2_b200.h")]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 
 

@@ -1,4 +1,4 @@
-"""Planning configuration for the B200 planner.
+"""Planning configuration for the H100 planner.
 
 Restates the planning / architecture keys of the reference's Hydra config as a
 plain attribute bag (hydra/omegaconf are not needed on the hot path):
@@ -158,7 +158,7 @@ def workload(name: str, **overrides: Any) -> Config:
                   enc_dim=64, mlp_dim=64, latent_dim=64, num_enc_layers=2, num_q=3,
                   num_envs=2, num_samples=128, num_elites=16, num_pi_trajs=8,
                   horizon=3, iterations=3)
-    elif name == "tiny-wide":  # test-sized model whose hidden layers exceed the 512 TMEM columns (wide path)
+    elif name == "tiny-wide":  # test-sized model whose hidden layers are wider than 512 (640 columns)
         kw = dict(obs_dim=19, action_dim=7, model_size=None, task="tiny-wide",
                   enc_dim=96, mlp_dim=640, latent_dim=64, num_enc_layers=2, num_q=3,
                   num_envs=2, num_samples=128, num_elites=16, num_pi_trajs=8,

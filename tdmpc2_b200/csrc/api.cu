@@ -15,7 +15,6 @@
 
 #include "../../include/tdmpc2_b200.h"
 #include "plan_kernels.cuh"
-#include "plan_pp.cuh"
 #include "pixel_encoder.cuh"
 
 using namespace tdmpc2;
@@ -59,7 +58,7 @@ __global__ void absmax_kernel(const float* __restrict__ w, size_t n, unsigned* s
 // W[N, K] fp32 row-major -> two fp16 planes [Npad, Kpad] of W * 2^k, zero padded.
 // 2^k puts max|W| in [128, 256): fp16 hi keeps 11 bits, lo the next 11, both in the normal range.
 // Output row n takes source row n (n < split_at) or split_at + (n - split_to) (n >= split_to): the pi head's
-// log_std rows are moved to a 32-aligned column so the fused epilogue reads them with aligned tcgen05.ld.
+// log_std rows are moved to a 32-aligned column (column Apad of the head's output row).
 __device__ __forceinline__ int src_index(int n, int src_n, int split_at, int split_to) {
   if (n < split_at) return n;
   if (n >= split_to && n - split_to + split_at < src_n) return n - split_to + split_at;
@@ -134,17 +133,11 @@ struct tdmpc2_planner {
   uint8_t* ws = nullptr;
   PlanParams base;
   int engine = TDMPC2_ENGINE_TCGEN05;
-  bool bound = false, weights_ok = false, smem_attr_pp = false, all_fused = true;
-  bool attr_done[16] = {};          // dynamic-smem opt-in done, per plan_kernel instantiation
+  bool bound = false, weights_ok = false;
+  bool attr_done[4] = {};           // dynamic-smem opt-in done, per plan_kernel instantiation
   int64_t launches = 0;
-  unsigned wide_sleep_ns = 0;
-  int head_kseg = 8;                // heads: 512 elements of K per TMEM accumulation (the 5M preset's whole K)
-  int kseg = 32;                    // wide layers: K-chunks per TMEM accumulation segment (2048 elements; 0 = whole K)
   size_t l2_window_bytes = 0;       // > 0: launches carry a persisting-L2 access-policy window over the activation scratch
   float l2_hit_ratio = 1.f;
-  bool pair_ok = true;              // every layer of the CEM iteration can run as cta_group::2
-  int l2hint = 2;                   // PlanParams::l2hint (TDMPC2_B200_L2HINT): 2 = evict-last on fused activation stores (default), 1 = operand-load hints (experiment)
-  unsigned stagger = 0;             // PlanParams::stagger (TDMPC2_B200_STAGGER, clock cycles; experiment knob)
   int passes = 3;                   // 3 = fp32-parity arithmetic, 1 = declared non-parity fast mode (PlanParams::passes)
   int zb_kc0 = 0, zb_pitch = 0;     // shared-latent fold (PlanParams::zbias): K-chunks of [z | emb] folded into a per-env bias
   const int32_t* cur_task = nullptr;
@@ -177,13 +170,13 @@ static int check_device(int* num_sms) {
   int dev = 0, ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     cudaGetLastError();
-    return fail(TDMPC2_ERR_NO_DEVICE, "no CUDA device: the B200 planner has no CPU fallback");
+    return fail(TDMPC2_ERR_NO_DEVICE, "no CUDA device: the planner has no CPU fallback");
   }
   CUDA_TRY(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10)
-    return fail(TDMPC2_ERR_NO_DEVICE, "device %d (%s) is sm_%d%d; this library is built for sm_100a only", dev, prop.name,
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(TDMPC2_ERR_NO_DEVICE, "device %d (%s) is sm_%d%d; this library is built for sm_90a only", dev, prop.name,
                 prop.major, prop.minor);
   *num_sms = prop.multiProcessorCount;
   return 0;
@@ -249,14 +242,10 @@ extern "C" int tdmpc2_planner_create(const tdmpc2_dims* dims, tdmpc2_planner** o
   p->KpadX = std::max(pad_to(D, kKch), pad_to(d.obs_dim + T, kKch));
   p->KpadH = std::max(pad_to(M, kKch), pad_to(d.enc_dim, kKch));
   p->NpadMax = 0;
-  for (auto& l : p->layers) { p->NpadMax = std::max(p->NpadMax, l.Npad); if (l.Npad > kFusedMaxN) p->all_fused = false; }
+  for (auto& l : p->layers) p->NpadMax = std::max(p->NpadMax, l.Npad);
   p->Ppad = 1;
   while (p->Ppad < d.num_pi_trajs) p->Ppad <<= 1;
   p->tiles_per_env = (d.num_samples + kTileM - 1) / kTileM;
-  p->wide_sleep_ns = env_uint("TDMPC2_B200_WIDE_SLEEP_NS", 0);   // experiment knob (see DESIGN.md)
-  p->stagger = env_uint("TDMPC2_B200_STAGGER", 0);
-  p->l2hint = static_cast<int>(env_uint("TDMPC2_B200_L2HINT", 2));   // bit 1 (value 2) on by default: see PlanParams::l2hint
-  p->pair_ok = true;   // fused layers and the super-chunked wide layers both run as cta_group::2
 
   // ---- packed blob layout
   size_t off = 0;
@@ -331,19 +320,14 @@ extern "C" int tdmpc2_planner_set_engine(tdmpc2_planner* p, int engine) {
   return 0;
 }
 
-// Wide layers (output wider than the 512 TMEM columns): flush the TMEM partial sums to fp32 every `k_elems` elements of
-// the reduction dimension (rounded to 64-element chunks) and add the segments with round-to-nearest.  0 = accumulate the
-// whole reduction in TMEM (fastest).
+// The tensor-core engine adds every 64-element K-chunk's partial sum with round-to-nearest, which is finer than any
+// segment length these calls can ask for: they validate their argument and change nothing on this build.
 extern "C" int tdmpc2_planner_set_kseg(tdmpc2_planner* p, int k_elems) {
   if (!p || k_elems < 0) return fail(TDMPC2_ERR_INVALID, "bad kseg");
-  p->kseg = (k_elems + kKch - 1) / kKch;
   return 0;
 }
-// The same for the head layers (reward / Q / pi / termination outputs): their partial sums alternate between two TMEM
-// buffers and are added in registers, at no measurable cost.  Default 512; 0 = whole K in one accumulation.
 extern "C" int tdmpc2_planner_set_head_kseg(tdmpc2_planner* p, int k_elems) {
   if (!p || k_elems < 0) return fail(TDMPC2_ERR_INVALID, "bad head kseg");
-  p->head_kseg = (k_elems + kKch - 1) / kKch;
   return 0;
 }
 
@@ -357,16 +341,14 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-static int make_map(EncodeTiledFn enc, CUtensorMap* m, void* base, uint64_t kpad, uint64_t rows, int box_cols = kKch,
-                    int box_rows = 128) {
+static int make_map(EncodeTiledFn enc, CUtensorMap* m, void* base, uint64_t kpad, uint64_t rows) {
   cuuint64_t dims[2] = {kpad, rows};
   cuuint64_t strides[1] = {kpad * 2};
-  cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
+  cuuint32_t box[2] = {static_cast<cuuint32_t>(kKch), static_cast<cuuint32_t>(kTileM)};
   cuuint32_t estr[2] = {1, 1};
-  // 64-column boxes (operand loads): 128-byte rows, 128B swizzle; 32-column boxes (epilogue stores): 64B swizzle;
-  // 16-column boxes (ping-pong epilogue stores): 32-byte rows, no swizzle
+  // 64-column boxes (operand loads): 128-byte rows, 128B swizzle (the wgmma operand layout)
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   box_cols == kKch ? CU_TENSOR_MAP_SWIZZLE_128B : box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(TDMPC2_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) kpad=%llu rows=%llu", (int)r,
                                      (unsigned long long)kpad, (unsigned long long)rows);
@@ -392,15 +374,6 @@ extern "C" int tdmpc2_planner_bind(tdmpc2_planner* p, void* packed, void* worksp
   int rc;
   if ((rc = make_map(enc, &B.tmX, p->ws + p->off_X, p->KpadX, static_cast<uint64_t>(p->nslots) * 2 * kTileM))) return rc;
   if ((rc = make_map(enc, &B.tmH, p->ws + p->off_H, p->KpadH, static_cast<uint64_t>(p->nslots) * 2 * kTileM))) return rc;
-  if ((rc = make_map(enc, &B.tmXs, p->ws + p->off_X, p->KpadX, static_cast<uint64_t>(p->nslots) * 2 * kTileM, 32))) return rc;
-  if ((rc = make_map(enc, &B.tmHs, p->ws + p->off_H, p->KpadH, static_cast<uint64_t>(p->nslots) * 2 * kTileM, 32))) return rc;
-  {
-    const uint64_t rows = static_cast<uint64_t>(p->nslots) * 2 * kTileM;
-    if ((rc = make_map(enc, &B.tmX64, p->ws + p->off_X, p->KpadX, rows, kKch, kPPHalf))) return rc;
-    if ((rc = make_map(enc, &B.tmH64, p->ws + p->off_H, p->KpadH, rows, kKch, kPPHalf))) return rc;
-    if ((rc = make_map(enc, &B.tmXs64, p->ws + p->off_X, p->KpadX, rows, kPPStgCols, kPPHalf))) return rc;
-    if ((rc = make_map(enc, &B.tmHs64, p->ws + p->off_H, p->KpadH, rows, kPPStgCols, kPPHalf))) return rc;
-  }
   for (int m = 0; m < p->nmaps; ++m)
     if ((rc = make_map(enc, &B.tmW[m], p->packed + p->map_off[m], p->map_kpad[m], p->map_rows[m]))) return rc;
 
@@ -510,135 +483,55 @@ extern "C" int tdmpc2_pack_weights(tdmpc2_planner* p, const tdmpc2_weights* w, v
 }
 
 // ------------------------------------------------------------------------------------ launches
-// plan_pp.cuh covers models whose trunk layers are 256 / 512 wide and whose heads fit one 128-column chunk
-static bool pp_eligible(const tdmpc2_planner* p) {
-  const tdmpc2_dims& d = p->d;
-  if (d.episodic || !p->all_fused || d.action_dim > 64 || d.num_bins > 128 || d.num_bins < 1 || 6 * d.horizon + 9 > kPPMaxSteps) return false;
-  if (d.num_samples % kTileM != 0 || (d.latent_dim + d.task_dim) % 8 != 0 || (d.latent_dim + d.task_dim) / 8 > kEpiThreads) return false;
-  if (d.simnorm_dim != 8) return false;
-  for (size_t i = static_cast<size_t>(p->li_dyn); i < p->layers.size(); ++i) {
-    const LayerHost& l = p->layers[i];
-    if (l.has_ln) { if (l.N != l.Npad || (l.Npad != 256 && l.Npad != 512)) return false; }
-    else if (l.Npad != 128) return false;
-  }
-  return true;
-}
-
-// The engine the CEM-iteration launches of this planner actually run (the requested one falls back when a model or
-// shape does not fit it: ping-pong -> CTA pairs -> single CTAs).
+// The engine the CEM-iteration launches of this planner actually run.  The CTA-pair and ping-pong engines (2, 3, 4) are
+// built on Blackwell's cta_group::2 MMAs; on sm_90a they run as the single-CTA tensor-core engine 0.
 extern "C" int tdmpc2_planner_iter_engine(const tdmpc2_planner* p) {
   if (!p) return -1;
-  if (p->engine == TDMPC2_ENGINE_SIMT || p->engine == TDMPC2_ENGINE_TCGEN05) return p->engine;
-  const bool pairs = (p->tiles_per_env % 2 == 0) && p->pair_ok;
-  if (!pairs) return TDMPC2_ENGINE_TCGEN05;
-  if (p->engine == TDMPC2_ENGINE_TCGEN05_PP) return (p->passes == 3 && pp_eligible(p)) ? TDMPC2_ENGINE_TCGEN05_PP : TDMPC2_ENGINE_TCGEN05_2SM;
-  return p->engine;
+  return p->engine == TDMPC2_ENGINE_SIMT ? TDMPC2_ENGINE_SIMT : TDMPC2_ENGINE_TCGEN05;
 }
 
-// W prefetch (plan_kernel<..., WPF>): every LayerNorm layer of the CEM iteration must take the epilogue's fast path
-// (whole 32-column blocks out through TMA stores), which is the only one that stages in the A ring
-static bool wpf_eligible(const tdmpc2_planner* p) {
-  if (p->d.episodic || !p->all_fused) return false;
-  for (size_t i = static_cast<size_t>(p->li_dyn); i < p->layers.size(); ++i)
-    if (p->layers[i].has_ln && p->layers[i].N % 32 != 0) return false;
-  return true;
-}
-
-// Launch attributes shared by every plan_kernel launch: the cluster dimension of the CTA-pair engines and -- when
-// enabled (tdmpc2_planner_set_l2_persist) -- an access-policy window that keeps the per-CTA activation scratch
-// (X + H planes, contiguous in the workspace) resident in the persisting part of L2, so that its dirty lines are not
-// written back to HBM while noise and weights stream through.
+// Launch attributes shared by every plan_kernel launch: when enabled (tdmpc2_planner_set_l2_persist), an access-policy
+// window that keeps the per-CTA activation scratch (X + H planes, contiguous in the workspace) resident in the
+// persisting part of L2, so that its dirty lines are not written back to HBM while noise and weights stream through.
 struct LaunchCfg {
   cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[2];
-  LaunchCfg(tdmpc2_planner* p, int grid, size_t smem, cudaStream_t st, bool cluster2);
+  cudaLaunchAttribute attr[1];
+  LaunchCfg(tdmpc2_planner* p, int grid, size_t smem, cudaStream_t st);
 };
 
 template <class K>
-static int launch_one(tdmpc2_planner* p, K kernel, int grid, size_t smem, cudaStream_t st, bool cluster2, const PlanParams& prm,
-                      int threads = kThreads) {
-  LaunchCfg lc(p, grid, smem, st, cluster2);
-  lc.cfg.blockDim = dim3(threads);
+static int launch_big(tdmpc2_planner* p, K kernel, bool* attr_done, int grid, cudaStream_t st, const PlanParams& prm) {
+  if (!*attr_done) {     // > 48 KiB of dynamic shared memory needs the opt-in, once per kernel instantiation
+    CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+    *attr_done = true;
+  }
+  LaunchCfg lc(p, grid, kSmemBytes, st);
   CUDA_TRY(cudaLaunchKernelEx(&lc.cfg, kernel, prm));
   CUDA_TRY(cudaGetLastError());
   p->launches += 1;
   return 0;
 }
 
-template <class K>
-static int launch_big(tdmpc2_planner* p, K kernel, bool* attr_done, int grid, cudaStream_t st, bool cluster2, const PlanParams& prm) {
-  if (!*attr_done) {     // > 48 KiB of dynamic shared memory needs the opt-in, once per kernel instantiation
-    CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    *attr_done = true;
-  }
-  return launch_one(p, kernel, grid, kSmemBytes, st, cluster2, prm);
-}
-
 static int launch_plan(tdmpc2_planner* p, const PlanParams& prm, int ntiles, cudaStream_t st) {
-  const bool simt = p->engine == TDMPC2_ENGINE_SIMT;
   // episodic models: the rollout modes run the instantiations that carry the termination head
   const bool epi = p->d.episodic && (prm.mode == MODE_ITER || prm.mode == MODE_VALUE);
-  // models with layers wider than TMEM (and the one-layer diagnostic mode, whose raw output may be) take the WIDE kernels
-  const bool wide = !p->all_fused || prm.mode == MODE_LAYER;
-  int grid = std::min(ntiles, p->nslots);
+  const int grid = std::min(ntiles, p->nslots);
   PlanParams prm2 = prm;
   prm2.prof = p->prof;
   prm2.prof_slots = p->nslots;
-  prm2.kseg = p->kseg;
-  prm2.head_kseg = p->head_kseg;
-  prm2.wide_sleep_ns = p->wide_sleep_ns;
   prm2.passes = p->passes;
-  prm2.stagger = p->stagger;
-  prm2.l2hint = p->l2hint;
-  static_assert(sizeof(p->attr_done) / sizeof(bool) >= 16, "attr_done slots");
-  // CTA-pair (cta_group::2) launch: CEM iterations only, whole pairs of tiles of one environment
-  const bool pair_engine = (p->engine == TDMPC2_ENGINE_TCGEN05_2SM || p->engine == TDMPC2_ENGINE_TCGEN05_PP ||
-                            p->engine == TDMPC2_ENGINE_TCGEN05_2SM_PF);
-  if (p->engine == TDMPC2_ENGINE_TCGEN05_PP && prm.mode == MODE_ITER && (p->tiles_per_env % 2 == 0) && (ntiles % 2 == 0) &&
-      p->passes == 3 && pp_eligible(p)) {
-    // ping-pong kernel (plan_pp.cuh): GEMM of one 64-row half overlaps the epilogue of the other
-    if (!p->smem_attr_pp) {
-      CUDA_TRY(cudaFuncSetAttribute(plan_pp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPPSmemBytes));
-      p->smem_attr_pp = true;
-    }
-    return launch_one(p, plan_pp_kernel, grid & ~1, kPPSmemBytes, st, true, prm2, kPPThreads);
-  }
   bool* ad = p->attr_done;
-  if (simt) {
-    if (epi) return launch_big(p, plan_kernel<ENGINE_SIMT, false, true>, &ad[0], grid, st, false, prm2);
-    return launch_big(p, plan_kernel<ENGINE_SIMT>, &ad[1], grid, st, false, prm2);
+  if (p->engine == TDMPC2_ENGINE_SIMT) {
+    if (epi) return launch_big(p, plan_kernel<ENGINE_SIMT, true>, &ad[0], grid, st, prm2);
+    return launch_big(p, plan_kernel<ENGINE_SIMT>, &ad[1], grid, st, prm2);
   }
-  // CTA pairs take tiles (2p, 2p + 1): CEM iterations with an even number of tiles per environment (so that a pair never
-  // straddles the refit hand-off asymmetrically), and the policy-prior rollouts whenever the tile count is even
-  const bool pair = pair_engine && p->pair_ok && (ntiles % 2 == 0) &&
-                    ((prm.mode == MODE_ITER && p->tiles_per_env % 2 == 0) || prm.mode == MODE_PRIOR);
-  if (pair) {
-    grid &= ~1;
-    if (wide) {
-      if (epi) return launch_big(p, plan_kernel<ENGINE_TC, true, true, false, true>, &ad[2], grid, st, true, prm2);
-      return launch_big(p, plan_kernel<ENGINE_TC, true, false, false, true>, &ad[3], grid, st, true, prm2);
-    }
-    if (epi) return launch_big(p, plan_kernel<ENGINE_TC, true, true>, &ad[4], grid, st, true, prm2);
-    if (p->engine == TDMPC2_ENGINE_TCGEN05_2SM_PF && wpf_eligible(p))
-      return launch_big(p, plan_kernel<ENGINE_TC, true, false, true>, &ad[5], grid, st, true, prm2);
-    return launch_big(p, plan_kernel<ENGINE_TC, true>, &ad[6], grid, st, true, prm2);
-  }
-  if (wide) {
-    if (epi) return launch_big(p, plan_kernel<ENGINE_TC, false, true, false, true>, &ad[7], grid, st, false, prm2);
-    return launch_big(p, plan_kernel<ENGINE_TC, false, false, false, true>, &ad[8], grid, st, false, prm2);
-  }
-  if (epi) return launch_big(p, plan_kernel<ENGINE_TC, false, true>, &ad[9], grid, st, false, prm2);
-  return launch_big(p, plan_kernel<ENGINE_TC>, &ad[10], grid, st, false, prm2);
+  if (epi) return launch_big(p, plan_kernel<ENGINE_TC, true>, &ad[2], grid, st, prm2);
+  return launch_big(p, plan_kernel<ENGINE_TC>, &ad[3], grid, st, prm2);
 }
 
-LaunchCfg::LaunchCfg(tdmpc2_planner* p, int grid, size_t smem, cudaStream_t st, bool cluster2) {
+LaunchCfg::LaunchCfg(tdmpc2_planner* p, int grid, size_t smem, cudaStream_t st) {
   cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
   int n = 0;
-  if (cluster2) {
-    attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = 2; attr[n].val.clusterDim.y = 1; attr[n].val.clusterDim.z = 1;
-    ++n;
-  }
   if (p->l2_window_bytes > 0) {
     attr[n].id = cudaLaunchAttributeAccessPolicyWindow;
     attr[n].val.accessPolicyWindow.base_ptr = p->ws + p->off_X;
@@ -806,7 +699,7 @@ extern "C" int tdmpc2_plan_iter_rng(tdmpc2_planner* p, const uint64_t* rng_state
   if (rc) return rc;
   const tdmpc2_dims& d = p->d;
   if (!rng_state || !qidx || iteration < 0) return fail(TDMPC2_ERR_INVALID, "null argument");
-  if (p->engine == TDMPC2_ENGINE_SIMT) return fail(TDMPC2_ERR_UNSUPPORTED, "in-kernel noise needs a tcgen05 engine");
+  if (p->engine == TDMPC2_ENGINE_SIMT) return fail(TDMPC2_ERR_UNSUPPORTED, "in-kernel noise needs a tensor-core engine");
   PlanParams prm = p->base;
   prm.task = p->cur_task;
   prm.mode = MODE_ITER;

@@ -1,9 +1,8 @@
-// Fused planning kernels for sm_100a (B200).
+// Fused planning kernels for sm_90a (H100).
 //
-// One persistent kernel template, `plan_kernel<ENGINE, PAIR, EPISODIC, WPF>`, runs the MLP chains of
-// the TD-MPC2 planner on 128-row tiles (the flags are compile-time so that an unused feature costs no code:
-// PAIR = CTA pairs / cta_group::2, EPISODIC = termination head in the rollout, WPF = weight prefetch during the
-// epilogue).  All modes share the device code:
+// One persistent kernel template, `plan_kernel<ENGINE, EPISODIC>`, runs the MLP chains of the TD-MPC2 planner on
+// 128-row tiles (EPISODIC = termination head in the rollout; compile-time so that an unused feature costs no code).
+// All modes share the device code:
 //
 //   MODE_ENCODE : rows = environments.      z = encode(obs, task)        (reference world_model.py:103-112)
 //   MODE_PRIOR  : rows = (env, pi-traj).    the P policy-prior rollouts  (reference tdmpc2.py:154-160)
@@ -13,26 +12,16 @@
 //   MODE_VALUE  : MODE_ITER's rollout on caller-given z / actions, no refit (reference tdmpc2.py:122-136)
 //   MODE_LAYER  : one layer, for diagnostics.
 //
-// Every dense layer is `acc = A[128, Kpad] * W[Npad, Kpad]^T` with both operands
-// stored as two fp16 planes (hi, lo; x ~= hi + lo to ~22 bits).  The tcgen05
-// engine accumulates A_lo*W_hi + A_hi*W_lo + A_hi*W_hi in fp32 in TMEM
-// (kind::f16, K=16), operands staged by TMA (128-byte swizzle) through two
-// mbarrier rings (A: 2 x 32 KiB, W: 2 x 64 KiB | 4 x 32 KiB) so that an A K-chunk
-// is streamed once per layer: warp 0 = TMA producer, warp 1 = MMA issuer,
-// warps 4-19 = epilogue (4 TMEM lane quarters x 4 column groups).
+// Every dense layer is `acc = A[128, Kpad] * W[Npad, Kpad]^T` with both operands stored as two fp16 planes (hi, lo;
+// x ~= hi + lo to ~22 bits).  The tensor-core engine (ENGINE_TC) streams 64-element K-chunks of both operands with TMA
+// (128-byte swizzle) through a 3-stage mbarrier ring (warp 16 = producer) into four consumer warpgroups, each of which
+// owns a 64 x 64 block of every 128 x 128 output block and runs wgmma (m64n64k16) A_lo*W_hi + A_hi*W_lo + A_hi*W_hi
+// per K-chunk into fresh fp32 registers; the K-chunk partials are added with round-to-nearest and the block goes to
+// an fp32 scratch row buffer in global memory.  The SIMT engine computes the same sums with FFMA on CUDA cores.  Both
+// engines then run the same row phases (warp per row): bias + LayerNorm + Mish / SimNorm, two-hot-inverse,
+// tanh-Gaussian sampling, and emit the next layer's fp16 planes.
 //
-//   * PAIR mode (CEM iterations): clusters of two CTAs issue cta_group::2 MMAs with
-//     M = 256 (each CTA's own 128-row tile); each CTA streams half of every W tile.
-//     plan_pp.cuh holds the ping-pong variant of this mode (two 64-row halves per CTA).
-//   * Layers with Npad <= 512 (the whole accumulator fits TMEM) use the FUSED
-//     epilogue: one thread per row reads its accumulator row straight from TMEM
-//     (tcgen05.ld), applies bias + LayerNorm + Mish / SimNorm / two-hot-inverse /
-//     tanh-Gaussian sampling in packed fp32x2 math, and emits the next layer's fp16
-//     planes as swizzled smem tiles that leave through TMA stores.
-//   * Wider layers (48M / 317M presets) drain N-chunks of 256 columns to an fp32
-//     scratch row buffer and run the same math warp-per-row afterwards.
-//
-// Activations live in a per-CTA scratch slot (global memory, L2-resident: X planes +
+// Activations live in a per-CTA scratch slot (global memory: X planes +
 // one in-place hidden buffer, 0.56 MB per slot for the 5M model).
 #pragma once
 #include <cuda.h>
@@ -46,40 +35,26 @@
 
 namespace tdmpc2 {
 
-constexpr int kTileM = 128;       // rows per tile (UMMA M)
+constexpr int kTileM = 128;       // rows per tile
 constexpr int kKch = 64;          // K elements per pipeline stage (128 B of fp16: one swizzle row)
-constexpr int kNch = 256;         // N columns per accumulator chunk (UMMA N max)
 constexpr int kStages = 2;
-constexpr int kAPlane = kTileM * 128;           // 16 KiB: one A plane of a stage
-constexpr int kWPlane = kNch * 128;             // 32 KiB: one W plane of a stage
-constexpr int kStageBytes = 2 * kAPlane + 2 * kWPlane;   // 96 KiB (the operand smem is kStages * kStageBytes = 192 KiB)
-// The 192 KiB are split into two independent rings so that an A K-chunk is loaded ONCE per layer and re-used by
-// every N-chunk of weights: A ring = 2 x (hi 16 KiB | lo 16 KiB), W ring = 2 x (hi 32 KiB | lo 32 KiB).
-constexpr int kASlotBytes = 2 * kAPlane;                  // 32 KiB
-constexpr int kWSlotBytes = 2 * kWPlane;                  // 64 KiB
-constexpr int kARing = 2, kWRing = 2;
-constexpr int kWRingPair = 4;                            // pair mode: 4 half-size W slots (hi 16 KiB | lo 16 KiB) in the same 128 KiB
-constexpr int kWRingOff = kARing * kASlotBytes;           // 64 KiB
-static_assert(kARing * kASlotBytes + kWRing * kWSlotBytes == kStages * kStageBytes, "operand smem layout");
-// Fused-epilogue staging for TMA stores: per column group 2 buffers x (hi 8 KiB | lo 8 KiB) = one 32-column block
-// each, 64-byte-swizzled; the 128 KiB alias the W ring (idle once every MMA of the layer has retired).
-constexpr int kStgPlane = kTileM * 64;                    // 8 KiB
-constexpr int kStgBuf = 2 * kStgPlane;                    // 16 KiB
-constexpr int kThreads = 576;                   // 18 warps: 65536 / 576 = 113 -> 112 registers per thread
+constexpr int kAPlane = kTileM * 128;           // 16 KiB: one 128-row plane of a K-chunk
+constexpr int kStageBytes = 6 * kAPlane;        // 96 KiB (the operand smem is kStages * kStageBytes = 192 KiB)
+// Tensor-core engine: 3 ring stages of (A hi | A lo | W hi | W lo), 16 KiB each, inside the same 192 KiB.
+constexpr int kGStages = 3;
+constexpr int kGStageBytes = 4 * kAPlane;
+constexpr int kGNb = 128;                        // output columns per block (W rows per stage)
+constexpr int kGWarpGroups = 4;                  // consumer warps 0..15: warpgroup g owns rows 64 (g & 1).., columns 64 (g >> 1)..
+constexpr int kGProducerWarp = 4 * kGWarpGroups; // warp 16 issues the TMA loads
+static_assert(kGStages * kGStageBytes <= kStages * kStageBytes, "operand smem layout");
+constexpr int kThreads = 576;                   // 18 warps; ptxas assigns 96 registers per thread (small spills)
 constexpr int kWarps = kThreads / 32;
-constexpr int kEpiWarp0 = 2;                    // warps 2..17 are the epilogue warps: 4 column groups x 4 lane quarters
-constexpr int kEpiGroups = 4;
-constexpr int kEpiThreads = kEpiGroups * 128;
 constexpr int kMaxWMaps = 8;
 constexpr int kMaxHeadCols = 256;  // widest head output (2A or num_bins)
-constexpr int kFusedMaxN = 512;    // TMEM columns
-constexpr int kSmemCtrl = 2048;    // barriers, tmem ptr, flags (128 B) + G[128] + q1[128]
-constexpr int kSmemRowBuf = kWarps * kMaxHeadCols * 4;  // one head-output row per warp (wide path)
+constexpr int kSmemCtrl = 2048;    // barriers, flags (256 B) + G[128] + q1[128] + term[128]
+constexpr int kSmemRowBuf = kWarps * kMaxHeadCols * 4;  // one head-output row per warp
 constexpr int kSmemRowEnv = kTileM * 4;                 // env index of each tile row
-constexpr int kSmemVec = 3 * kFusedMaxN * 4;            // bias / ln_g / ln_b of the current layer
-constexpr int kSmemPart = 2 * kEpiGroups * kTileM * 4;  // LayerNorm partials [mean | M2][group][128]
-constexpr int kSmemBytes = kStages * kStageBytes + kSmemCtrl + kSmemRowBuf + kSmemRowEnv + kSmemVec + kSmemPart +
-                           1024 /*align slack*/;
+constexpr int kSmemBytes = kStages * kStageBytes + kSmemCtrl + kSmemRowBuf + kSmemRowEnv;
 
 enum Mode { MODE_ENCODE = 0, MODE_PRIOR = 1, MODE_ITER = 2, MODE_VALUE = 3, MODE_LAYER = 4 };
 enum Engine { ENGINE_TC = 0, ENGINE_SIMT = 1 };
@@ -105,9 +80,6 @@ struct LayerDev {
 struct PlanParams {
   CUtensorMap tmX;                 // [slots*2*128, KpadX] fp16, box 64 x 128
   CUtensorMap tmH;                 // [slots*2*128, KpadH]
-  CUtensorMap tmXs, tmHs;          // same tensors, box 32 x 128, 64-byte swizzle: the epilogue's TMA stores
-  CUtensorMap tmX64, tmH64;        // 64-row boxes (ping-pong engine, plan_pp.cuh): loads 64 x 64, 128-byte swizzle
-  CUtensorMap tmXs64, tmHs64;      //                                             : stores 16 x 64, 32-byte rows, no swizzle
   CUtensorMap tmW[kMaxWMaps];      // weights, one map per Kpad class, box 64 x 128
   const LayerDev* layers;
   int E, N, P, Ppad, K, H, obs_dim, A, Apad, L, M, T, B, num_q, simnorm, num_enc;   // Apad = pad32(A): the pi head's
@@ -130,10 +102,6 @@ struct PlanParams {
   long long* prof;   // optional [prof_slots][4][12] cycle counters + [32][16] trace stamps of CTA 0 (diagnostics), or nullptr
   int prof_slots;    // = number of scratch slots (SM count)
   int li_term;       // first of the 3 termination-head layers (cfg.episodic, world_model.py:28), or -1
-  int head_kseg;     // head layers: K-chunks per accumulator hand-off (0 = whole K in one accumulation)
-  unsigned wide_sleep_ns;   // wide layers: nanosleep between polls of the 16 epilogue warps' accumulator wait (0 = spin)
-  int kseg;          // wide layers: K-chunks (of 64) accumulated in TMEM before the partial sum is flushed to the fp32 raw
-                     // scratch and added there with round-to-nearest (0 = the whole K in one go); see epi_wide
   // Shared-latent fold (MODE_ITER, rollout step t = 0): every sample row of an environment carries the SAME [z | emb]
   // (z.repeat(N), tdmpc2.py:163), so the [z | emb] part of reward.0 / dynamics.0 is a per-environment vector.  The
   // prologue computes zbias[mlp][e][n] = bias[n] + sum_{k < 64 zb_kc0} [z | emb]_e[k] W[n][k] once per plan()
@@ -142,16 +110,8 @@ struct PlanParams {
   const float* zbias;   // [2 (0 reward, 1 dynamics)][E][zb_pitch]
   int zb_kc0, zb_pitch;
   // 3 = fp32-parity arithmetic (A_lo W_hi + A_hi W_lo + A_hi W_hi); 1 = the DECLARED NON-PARITY fast mode: hi planes only
-  // (one fp16 MMA per product, fp32 accumulate), half the operand bytes, no lo planes written.  tdmpc2_planner_set_passes.
+  // (one fp16 MMA per product, fp32 accumulate), half the operand bytes.  tdmpc2_planner_set_passes.
   int passes;
-  // MODE_ITER: every second CTA (pair) starts this many clock cycles late, so that neighbouring SMs are not all in their
-  // GEMM phase (L2 -> SM ingest, tensor-pipe power) and all in their epilogue at the same instants.  0 = off.
-  unsigned stagger;
-  // Wide models (activation planes + weights exceed L2): 1 = operand loads carry L2 eviction hints -- the per-CTA activation
-  // planes, re-read once per 512-column super-chunk with a reuse distance far beyond L2, are loaded evict-first so that
-  // they stop displacing the weight chunks that all 148 CTAs read within a short window (evict-last).  Bit 1 (value 2):
-  // evict-last on the fused epilogues' activation-plane stores (default on).  0 = evict-normal everywhere.
-  int l2hint;
   // Declared non-parity throughput mode (rng.cuh): non-null = the CEM iteration generates noise_r / noise_pi itself
   // (noise_r / noise_pi are null then); rng_iter = index of this iteration within the plan (selects the Philox stream)
   const unsigned long long* rng_state;
@@ -238,13 +198,6 @@ __device__ __forceinline__ float4 lds128(const float* p) {   // p must point int
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];\n" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "r"(ptx::smem_u32(p)));
   return r;
 }
-__device__ __forceinline__ void group_bar_sync(int grp) {   // named barrier among the 4 warps of one column group
-  asm volatile("bar.sync %0, 128;\n" ::"r"(2 + grp) : "memory");
-}
-__device__ __forceinline__ void epi_bar_sync() {   // named barrier among the 8 epilogue warps
-  asm volatile("bar.sync 1, %0;\n" ::"n"(kEpiThreads) : "memory");
-}
-
 // Diagnostics (cycle counters per role, clock stamps per layer of CTA 0) exist only in builds with -DTDMPC2_PROF
 // (tdmpc2_b200.build.build_variant("prof", ["TDMPC2_PROF=1"]), loaded through TDMPC2_B200_LIB): in the product build
 // they compile to nothing -- the 8 per-thread 64-bit counters alone cost 16 registers of a 96-register budget.
@@ -264,33 +217,17 @@ __device__ __forceinline__ long long prof_clock() { return kProf ? clock64() : 0
 // ------------------------------------------------------------------------------------ CTA context
 struct Ctx {
   uint8_t* stage_base;      // kStages * kStageBytes, 1024-aligned
-  uint64_t* a_full;         // [kARing]
-  uint64_t* a_empty;        // [kARing]
-  uint64_t* w_full;         // [kWRing]
-  uint64_t* w_empty;        // [kWRing]
-  uint64_t* acc_full;       // [2]  wide path: accumulator slot ready
-  uint64_t* acc_empty;      // [2]  wide path: accumulator slot drained
-  uint64_t* facc;           // [2]  fused path: accumulator chunk ready
-  uint64_t* rawb;           // [4 groups][2] wide layers, normalise pass: raw block landed in the group's input buffer
-  uint32_t* tmem_ptr;
+  uint64_t* g_full;         // [kGStages]  tensor-core engine: operand stage landed (TMA transaction bytes)
+  uint64_t* g_empty;        // [kGStages]  tensor-core engine: operand stage consumed (one arrival per consumer warp)
   float* rowbuf;            // [kWarps][kMaxHeadCols]
-  float* vec;               // [3][kFusedMaxN]  bias, ln_g, ln_b (fused path)
-  float* part;              // [2][2][128]      LayerNorm partials (fused path)
   float* G;                 // [128] discounted reward sum
   float* q1;                // [128] first Q head
   float* term;              // [128] sticky termination flag of the row (episodic models, tdmpc2.py:126-134)
   int* flags;               // small ints
   int* rowenv;              // [128]
-  uint32_t tmem_base;
   int slot, warp, lane;
-  int cg2, rank;             // CTA-pair mode (tcgen05 cta_group::2): pair rank 0 = leader issues the MMAs
-  int wpf;                   // W prefetch: the producer streams the NEXT layer's first weight chunks during the epilogue
-  uint32_t w_pref;           // (producer thread) weight chunks of the coming layer that are already in flight
-  uint32_t w_ring, w_stride, w_lo_off;   // W ring geometry: 2 x 64 KiB (lo plane at +32 KiB) or, in pair mode, 4 x 32 KiB (+16 KiB)
   // pipeline counters (each role keeps its own; persist across layers / tiles)
-  uint32_t pa_it, pw_it, ma_it, mw_it, a_it, d_it;
-  uint32_t rb_it;           // wide layers: raw blocks consumed so far by this thread's column group (buffer = it & 1)
-  uint32_t fph0, fph1;      // fused path: phase parity of facc[0|1] (tracked identically by every thread)
+  uint32_t pa_it, ma_it;
   long long pf0, pf1, pf2, pf3, pf4, pf5, pf6, pf7;   // per-thread cycle accumulators (diagnostics)
   int trace_step;
 };
@@ -398,221 +335,86 @@ __device__ __forceinline__ float pi_action(const PlanParams& P, float mu, float 
   return tanhf(__fadd_rn(mu, __fmul_rn(eps, expf(ls))));
 }
 
-// ------------------------------------------------------------------------------------ TMA producer / MMA issuer
-// FUSED == true : the whole accumulator (Npad <= 512) lives in TMEM: K-chunks outermost, each A chunk is loaded
-//                 once and multiplied with every N-chunk of weights; facc[0] fires when all chunks are complete.
-// FUSED == false: wide path, N-chunks outermost, accumulator chunks alternate between two 256-column TMEM slots
-//                 (acc_full / acc_empty) and A is re-streamed per chunk.
-__device__ __forceinline__ void prod_load_a(const PlanParams& P, Ctx& c, const CUtensorMap* tmA, int kc, int arow_hi, int arow_lo) {
-  const uint32_t s = c.pa_it % kARing, ph = (c.pa_it / kARing) & 1;
-  const long long tw = prof_clock();
-  ptx::mbar_wait(&c.a_empty[s], ph ^ 1);
-  c.pf0 += prof_clock() - tw;
-  uint8_t* st = c.stage_base + s * kASlotBytes;
-  const bool lo = P.passes != 1;                 // fast mode streams the hi planes only
-  if (ptx::elect_one()) {                        // the whole warp runs the role loop, one lane issues (see tc_producer)
-    if (c.cg2) {
-      // both CTAs of the pair stream their own 128 rows; the bytes of both land on the leader's barrier
-      if (c.rank == 0) ptx::mbar_expect_tx(&c.a_full[s], lo ? 2 * kASlotBytes : 2 * kAPlane);
-      const uint64_t pol = (P.l2hint & 1) ? ptx::kL2EvictFirst : ptx::kL2EvictNormal;
-      ptx::tma_load_2d_2sm(tmA, &c.a_full[s], st, kc * kKch, arow_hi, pol);
-      if (lo) ptx::tma_load_2d_2sm(tmA, &c.a_full[s], st + kAPlane, kc * kKch, arow_lo, pol);
-    } else {
-      ptx::mbar_expect_tx(&c.a_full[s], lo ? kASlotBytes : kAPlane);
-      ptx::tma_load_2d(tmA, &c.a_full[s], st, kc * kKch, arow_hi);
-      if (lo) ptx::tma_load_2d(tmA, &c.a_full[s], st + kAPlane, kc * kKch, arow_lo);
-    }
-  }
-  ++c.pa_it;
-}
-__device__ __forceinline__ void prod_load_w(Ctx& c, const CUtensorMap* tmW, int Npad, int wrow, int kc, int nc, bool lo = true,
-                                            bool l2hint = false) {
-  const int ncols = min(kNch, Npad - nc * kNch);   // 128 or 256
-  const uint32_t s = c.pw_it % c.w_ring, ph = (c.pw_it / c.w_ring) & 1;
-  const long long tw = prof_clock();
-  ptx::mbar_wait(&c.w_empty[s], ph ^ 1);
-  c.pf0 += prof_clock() - tw;
-  uint8_t* st = c.stage_base + kWRingOff + s * c.w_stride;
-  if (!ptx::elect_one()) { ++c.pw_it; return; }
-  if (c.cg2) {
-    // each CTA streams HALF of the N-chunk's weight rows (one 128-row box per plane; for a 128-column chunk only
-    // its first 64 rows are consumed): the pair MMA reads B rows [0, N/2) from the leader and [N/2, N) from the peer
-    if (c.rank == 0) ptx::mbar_expect_tx(&c.w_full[s], (lo ? 2 : 1) * (2 * 128 * 128));
-    const int wr = wrow + nc * kNch + c.rank * (ncols / 2);
-    const uint64_t pol = l2hint ? ptx::kL2EvictLast : ptx::kL2EvictNormal;
-    ptx::tma_load_2d_2sm(tmW, &c.w_full[s], st, kc * kKch, wr, pol);
-    if (lo) ptx::tma_load_2d_2sm(tmW, &c.w_full[s], st + c.w_lo_off, kc * kKch, wr + Npad, pol);
-  } else {
-    ptx::mbar_expect_tx(&c.w_full[s], (lo ? 2 : 1) * ncols * 128);
-    for (int b = 0; b < ncols / 128; ++b) {
-      const int wr = wrow + nc * kNch + b * 128;
-      ptx::tma_load_2d(tmW, &c.w_full[s], st + b * (128 * 128), kc * kKch, wr);
-      if (lo) ptx::tma_load_2d(tmW, &c.w_full[s], st + kWPlane + b * (128 * 128), kc * kKch, wr + Npad);
-    }
-  }
-  ++c.pw_it;
-}
-
-// N-chunks [nc0, nc0 + nnc_lim) of the layer (default: all of them): K-chunks outermost, each A chunk is loaded once
-// and multiplied with every N-chunk of the range; layers wider than TMEM call this once per 512-column super-chunk.
-// Role loops (TMA producer, MMA issuer) are run by the WHOLE warp, with one elected lane issuing the asynchronous
-// instructions: in warp-convergent code the compiler keeps ring counters, coordinates and operand descriptors in uniform
-// registers (12 UTCHMMA back to back), whereas inside an `if (lane == 0)` branch every cp.async.bulk.tensor / tcgen05.mma
-// gets a ~13-instruction "elect + R2UR + retry" waterfall (~120 cycles per MMA: more than an N = 128 MMA takes).
-__device__ __forceinline__ void tc_producer(const PlanParams& P, Ctx& c, const LayerRec& ly, int srcbuf, const LayerDev* next,
-                                            int nc0 = 0, int nnc_lim = 1 << 30, int kc0 = 0, int kc_lim = 1 << 30, int next_kc0 = 0) {
-  const int nkc = min(ly.Kpad / kKch, kc0 + kc_lim);
-  const int nnc = min((ly.Npad + kNch - 1) / kNch - nc0, nnc_lim);
-  const CUtensorMap* tmA = (srcbuf == BUF_X) ? &P.tmX : &P.tmH;
-  const CUtensorMap* tmW = &P.tmW[ly.wmap];
-  const int arow_hi = plane_row0(P, c.slot, srcbuf, 0), arow_lo = plane_row0(P, c.slot, srcbuf, 1);
-  TDMPC2_TRACE(P, c, 1);
-  uint32_t skip = c.wpf ? c.w_pref : 0u;     // chunks the previous layer's producer pass already requested
-  for (int kc = kc0; kc < nkc; ++kc) {
-    prod_load_a(P, c, tmA, kc, arow_hi, arow_lo);
-    for (int nc = nc0; nc < nc0 + nnc; ++nc) {
-      if (skip) --skip;
-      else prod_load_w(c, tmW, ly.Npad, ly.wrow, kc, nc, P.passes != 1, (P.l2hint & 1) != 0);
-    }
-  }
-  if (c.wpf) {
-    // The W ring drains while this layer's last MMAs retire and then idles through the whole epilogue (which
-    // stages its output in the A ring in this mode): fill it with the head of the next layer's weight stream.
-    uint32_t n = 0;
-    if (next) {
-      const CUtensorMap* tmW2 = &P.tmW[next->wmap];
-      const int nkc2 = next->Kpad / kKch, nnc2 = (next->Npad + kNch - 1) / kNch;
-      for (int kc = next_kc0; kc < nkc2 && n < c.w_ring; ++kc)      // next_kc0: the next layer's first K-chunk (shared-latent fold)
-        for (int nc = 0; nc < nnc2 && n < c.w_ring; ++nc) { prod_load_w(c, tmW2, next->Npad, next->wrow, kc, nc, P.passes != 1); ++n; }
-    }
-    c.w_pref = n;
-  }
-}
-
-// 12 MMAs of one (A K-chunk, W K-chunk x N-chunk) pair: A_lo*W_hi + A_hi*W_lo + A_hi*W_hi, 4 K-steps of 16.
-__device__ __forceinline__ void mma_stage(uint32_t d, uint32_t sa, uint32_t sw, uint32_t w_lo_off, uint32_t idesc, bool first, bool cg2,
-                                          bool one_pass = false) {
-#ifdef TDMPC2_EXP_NOMMA   // measurement build: no MMAs are issued, the commits release the operand slots at once -> the GEMM
-  return;                 // phases last exactly as long as the operand ingest (results are garbage; scripts/gpu_r2l.sh)
-#endif
-  if (!ptx::elect_one()) return;   // whole-warp role loop, one lane issues (tcgen05.commit must come from the same lane:
-                                   // elect.sync with a full mask always picks the same one)
-  if (one_pass) {                                   // declared non-parity fast mode: A_hi * W_hi only
-#pragma unroll
-    for (int ks = 0; ks < kKch / 16; ++ks) {
-      const uint64_t a_hi = ptx::make_sw128_kmajor_desc(sa + ks * 32);
-      const uint64_t w_hi = ptx::make_sw128_kmajor_desc(sw + ks * 32);
-      if (cg2) ptx::umma_f16_2sm(d, a_hi, w_hi, idesc, !(first && ks == 0));
-      else ptx::umma_f16(d, a_hi, w_hi, idesc, !(first && ks == 0));
-    }
-    return;
-  }
-#pragma unroll
-  for (int ks = 0; ks < kKch / 16; ++ks) {
-    const uint64_t a_hi = ptx::make_sw128_kmajor_desc(sa + ks * 32);
-    const uint64_t a_lo = ptx::make_sw128_kmajor_desc(sa + kAPlane + ks * 32);
-    const uint64_t w_hi = ptx::make_sw128_kmajor_desc(sw + ks * 32);
-    const uint64_t w_lo = ptx::make_sw128_kmajor_desc(sw + w_lo_off + ks * 32);
-    if (cg2) {
-      ptx::umma_f16_2sm(d, a_lo, w_hi, idesc, !(first && ks == 0));
-      ptx::umma_f16_2sm(d, a_hi, w_lo, idesc, 1);
-      ptx::umma_f16_2sm(d, a_hi, w_hi, idesc, 1);
-    } else {
-      ptx::umma_f16(d, a_lo, w_hi, idesc, !(first && ks == 0));   // small terms first
-      ptx::umma_f16(d, a_hi, w_lo, idesc, 1);
-      ptx::umma_f16(d, a_hi, w_hi, idesc, 1);
-    }
-  }
-}
-__device__ __forceinline__ uint32_t mma_wait_a(Ctx& c) {
-  const uint32_t s = c.ma_it % kARing, ph = (c.ma_it / kARing) & 1;
-  const long long tw = prof_clock();
-  ptx::mbar_wait(&c.a_full[s], ph);
-  c.pf0 += prof_clock() - tw;
-  return s;
-}
-__device__ __forceinline__ uint32_t mma_wait_w(Ctx& c) {
-  const uint32_t s = c.mw_it % c.w_ring, ph = (c.mw_it / c.w_ring) & 1;
-  const long long tw = prof_clock();
-  ptx::mbar_wait(&c.w_full[s], ph);
-  c.pf0 += prof_clock() - tw;
-  return s;
-}
-
-// Accumulates N-chunks [nc0, nc0 + nnc_lim) of the layer into TMEM columns [0, 256 * nnc); facc[0] fires when all of
-// them are complete.
-__device__ __forceinline__ void tc_mma(const PlanParams& P, Ctx& c, const LayerRec& ly, int nc0 = 0, int nnc_lim = 1 << 30,
-                                       int kc0 = 0, int kc_lim = 1 << 30) {
-  const int nkc = min(ly.Kpad / kKch, kc0 + kc_lim);
-  const int nnc = min((ly.Npad + kNch - 1) / kNch - nc0, nnc_lim);
-  const uint32_t sbase = ptx::smem_u32(c.stage_base);
-  for (int kc = kc0; kc < nkc; ++kc) {
-    const uint32_t as = mma_wait_a(c);
-    if (kc == kc0) TDMPC2_TRACE(P, c, 2);
-    for (int nc = nc0; nc < nc0 + nnc; ++nc) {
-      const uint32_t ws = mma_wait_w(c);
-      ptx::tc_fence_after();
-      const int ncols = min(kNch, ly.Npad - nc * kNch);
-      mma_stage(c.tmem_base + (nc - nc0) * kNch, sbase + as * kASlotBytes, sbase + kWRingOff + ws * c.w_stride, c.w_lo_off,
-                ptx::make_idesc_f16(c.cg2 ? 2 * kTileM : kTileM, ncols), kc == kc0, c.cg2 != 0, P.passes == 1);
-      if (ptx::elect_one()) {
-        if (c.cg2) ptx::umma_commit_2sm(&c.w_empty[ws]);
-        else ptx::umma_commit(&c.w_empty[ws]);     // frees the W slot when these MMAs retire
+// ------------------------------------------------------------------------------------ tensor-core engine: GEMM -> raw scratch
+// raw[128, Npad] = A[128, Kpad] * W[Npad, Kpad]^T over K-chunks [kc0, Kpad / 64), through TMA and wgmma (see the top of
+// this file).  Each K-chunk (12 wgmma: A_lo*W_hi + A_hi*W_lo + A_hi*W_hi, small terms first, 4 K-steps of 16) is
+// accumulated into zeroed registers and then added to the running sum with round-to-nearest, so that a long reduction
+// does not inherit the tensor core's internal accumulation rounding.  passes == 1: A_hi*W_hi only, hi planes only.
+__device__ __forceinline__ void gemm_tc(const PlanParams& P, Ctx& c, const LayerRec& ly, int srcbuf, int kc0 = 0) {
+  const int kc1 = ly.Kpad / kKch;
+  const int nnb = ly.Npad / kGNb;
+  const bool lo = P.passes != 1;
+  if (c.warp == kGProducerWarp) {
+    const CUtensorMap* tmA = (srcbuf == BUF_X) ? &P.tmX : &P.tmH;
+    const CUtensorMap* tmW = &P.tmW[ly.wmap];
+    const int arow_hi = plane_row0(P, c.slot, srcbuf, 0), arow_lo = plane_row0(P, c.slot, srcbuf, 1);
+    for (int nb = 0; nb < nnb; ++nb) {
+      const int wr = ly.wrow + nb * kGNb;
+      for (int kc = kc0; kc < kc1; ++kc) {
+        const uint32_t s = c.pa_it % kGStages, ph = (c.pa_it / kGStages) & 1;
+        const long long tw = prof_clock();
+        ptx::mbar_wait(&c.g_empty[s], ph ^ 1);
+        c.pf0 += prof_clock() - tw;
+        if (ptx::elect_one()) {
+          uint8_t* st = c.stage_base + s * kGStageBytes;
+          ptx::mbar_expect_tx(&c.g_full[s], (lo ? 4 : 2) * kAPlane);
+          ptx::tma_load_2d(tmA, &c.g_full[s], st, kc * kKch, arow_hi);
+          ptx::tma_load_2d(tmW, &c.g_full[s], st + 2 * kAPlane, kc * kKch, wr);
+          if (lo) {
+            ptx::tma_load_2d(tmA, &c.g_full[s], st + kAPlane, kc * kKch, arow_lo);
+            ptx::tma_load_2d(tmW, &c.g_full[s], st + 3 * kAPlane, kc * kKch, wr + ly.Npad);
+          }
+        }
+        __syncwarp();
+        ++c.pa_it;
       }
-      ++c.mw_it;
     }
-    if (ptx::elect_one()) {
-      if (c.cg2) ptx::umma_commit_2sm(&c.a_empty[as]);
-      else ptx::umma_commit(&c.a_empty[as]);
-    }
-    ++c.ma_it;
-  }
-  if (ptx::elect_one()) {
-    if (c.cg2) ptx::umma_commit_2sm(&c.facc[0]);
-    else ptx::umma_commit(&c.facc[0]);
-  }
-  TDMPC2_TRACE(P, c, 3);
-}
-
-// Head layers (plain Linear outputs, Npad <= 256) with a long reduction: the accumulator is handed to the epilogue every
-// `kseg` K-chunks, alternating between two TMEM buffers (columns [0,256) and [256,512)), and the epilogue adds the
-// segments in fp32 registers with round-to-nearest.  Why: tcgen05's accumulate step rounds TOWARD ZERO (measured:
-// scripts/micro/mma_rounding.py), which shrinks a long accumulation by ~n_MMA * 2^-25 relative; LayerNorm removes a
-// uniform shrink from the hidden layers, but the heads' logits have no LayerNorm behind them.
-__device__ __forceinline__ int head_segments(const PlanParams& P, const LayerRec& ly) {
-  const int nkc = ly.Kpad / kKch;
-  return (P.head_kseg > 0 && nkc > P.head_kseg) ? (nkc + P.head_kseg - 1) / P.head_kseg : 1;
-}
-__device__ __forceinline__ void tc_mma_head_seg(const PlanParams& P, Ctx& c, const LayerRec& ly, int nseg) {
-  const int nkc = ly.Kpad / kKch;
-  const uint32_t sbase = ptx::smem_u32(c.stage_base);
-  const uint32_t idesc = ptx::make_idesc_f16(c.cg2 ? 2 * kTileM : kTileM, ly.Npad);
-  for (int seg = 0; seg < nseg; ++seg) {
-    const int b = seg & 1;
-    if (seg >= 2) {                                    // buffer b was drained (segment seg - 2)
-      uint32_t& it = b ? c.d_it : c.a_it;
-      ptx::mbar_wait(&c.acc_empty[b], it & 1);
-      ++it;
-      ptx::tc_fence_after();
-    }
-    const int kc0 = seg * P.head_kseg, kc1 = min(nkc, kc0 + P.head_kseg);
-    for (int kc = kc0; kc < kc1; ++kc) {
-      const uint32_t as = mma_wait_a(c);
-      const uint32_t ws = mma_wait_w(c);
-      ptx::tc_fence_after();
-      mma_stage(c.tmem_base + b * kNch, sbase + as * kASlotBytes, sbase + kWRingOff + ws * c.w_stride, c.w_lo_off, idesc,
-                kc == kc0, c.cg2 != 0, P.passes == 1);
-      if (ptx::elect_one()) {
-        if (c.cg2) { ptx::umma_commit_2sm(&c.w_empty[ws]); ptx::umma_commit_2sm(&c.a_empty[as]); }
-        else { ptx::umma_commit(&c.w_empty[ws]); ptx::umma_commit(&c.a_empty[as]); }
+  } else if (c.warp < kGProducerWarp) {
+    const int wg = c.warp >> 2, t = threadIdx.x & 127;
+    const int r0 = (wg & 1) * 64, n0 = (wg >> 1) * 64;
+    const int row = r0 + (t >> 5) * 16 + ((t & 31) >> 2), col = n0 + 2 * (t & 3);
+    float* rawbase = raw_ptr(P, c.slot);
+    const uint32_t sbase = ptx::smem_u32(c.stage_base);
+    for (int nb = 0; nb < nnb; ++nb) {
+      float sum[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) sum[i] = 0.f;
+      for (int kc = kc0; kc < kc1; ++kc) {
+        const uint32_t s = c.ma_it % kGStages, ph = (c.ma_it / kGStages) & 1;
+        const long long tw = prof_clock();
+        ptx::mbar_wait(&c.g_full[s], ph);
+        c.pf2 += prof_clock() - tw;
+        const uint32_t sa = sbase + s * kGStageBytes + r0 * 128, sw = sbase + s * kGStageBytes + 2 * kAPlane + n0 * 128;
+        float acc[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < kKch / 16; ++ks) {
+          const uint64_t a_hi = ptx::make_sw128_kmajor_desc(sa + ks * 32), w_hi = ptx::make_sw128_kmajor_desc(sw + ks * 32);
+          if (lo) {
+            ptx::wgmma_m64n64k16(acc, ptx::make_sw128_kmajor_desc(sa + kAPlane + ks * 32), w_hi);
+            ptx::wgmma_m64n64k16(acc, a_hi, ptx::make_sw128_kmajor_desc(sw + kAPlane + ks * 32));
+          }
+          ptx::wgmma_m64n64k16(acc, a_hi, w_hi);
+        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        __syncwarp();
+        if (c.lane == 0) ptx::mbar_arrive(&c.g_empty[s]);     // this warp's reads of the stage are complete
+#pragma unroll
+        for (int i = 0; i < 32; ++i) sum[i] = __fadd_rn(sum[i], acc[i]);
+        ++c.ma_it;
       }
-      ++c.mw_it; ++c.ma_it;
-    }
-    if (ptx::elect_one()) {
-      if (c.cg2) ptx::umma_commit_2sm(&c.facc[b]);
-      else ptx::umma_commit(&c.facc[b]);
+      float* o = rawbase + static_cast<size_t>(row) * P.NpadMax + nb * kGNb + col;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        __stcg(reinterpret_cast<float2*>(o + 8 * j), make_float2(sum[4 * j], sum[4 * j + 1]));
+        __stcg(reinterpret_cast<float2*>(o + 8 * static_cast<size_t>(P.NpadMax) + 8 * j), make_float2(sum[4 * j + 2], sum[4 * j + 3]));
+      }
     }
   }
+  __syncthreads();
 }
 
 // ------------------------------------------------------------------------------------ SIMT engine: GEMM -> raw scratch
@@ -672,7 +474,7 @@ __device__ __forceinline__ void gemm_simt(const PlanParams& P, Ctx& c, const Lay
   __syncthreads();
 }
 
-// ------------------------------------------------------------------------------------ wide path: row phases (warp per row)
+// ------------------------------------------------------------------------------------ row phases (warp per row)
 __device__ __forceinline__ float ln_act_lane(float y, bool valid, int act) {
   if (act == EPI_LN_MISH) return mish_f(y);
   // SimNorm (layers.py:74-88): softmax over groups of 8 consecutive columns = 8 adjacent lanes.
@@ -786,963 +588,6 @@ __device__ __forceinline__ void rows_head(const PlanParams& P, Ctx& c, const Lay
   }
 }
 
-// ------------------------------------------------------------------------------------ fused path: TMEM epilogues
-// Thread-per-row: epilogue warp e (0..15) owns TMEM lanes 32*(e&3).. and the column group (e>>2).
-struct EpiThread {
-  int q, grp, row;
-  uint32_t taddr;     // TMEM address of this thread's lane, column 0
-};
-__device__ __forceinline__ EpiThread epi_thread(const Ctx& c) {
-  EpiThread t;
-  const int e = c.warp - kEpiWarp0;
-  t.q = c.warp & 3;                   // a warp may only touch the TMEM lane quarter (warp id % 4)
-  t.grp = e >> 2; t.row = t.q * 32 + c.lane;
-  t.taddr = c.tmem_base + (static_cast<uint32_t>(t.q * 32) << 16);
-  return t;
-}
-__device__ __forceinline__ void epi_stage_vectors(Ctx& c, const LayerRec& ly, bool with_ln) {
-  const int t = threadIdx.x - kEpiWarp0 * 32;
-  for (int i = t; i < ly.Npad; i += kEpiThreads) {
-    c.vec[i] = ly.bias[i];
-    if (with_ln) { c.vec[kFusedMaxN + i] = ly.ln_g[i]; c.vec[2 * kFusedMaxN + i] = ly.ln_b[i]; }
-  }
-  epi_bar_sync();
-}
-
-// Fast-path activation math for the fused epilogue.  __expf = ex2.approx(x*log2e) (rel. error ~2^-22 + |x|*6e-8),
-// __fdividef = rcp.approx * n (~1.5 ulp): Mish stays within ~1e-6 relative of the exact value.
-__device__ __forceinline__ float ex2_ftz(float x) {   // single MUFU.EX2
-  float r;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-__device__ __forceinline__ float rcp_ftz(float x) {   // single MUFU.RCP
-  float r;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-__device__ __forceinline__ float exp_fast(float x) { return ex2_ftz(x * 1.4426950408889634f); }
-// Packed fp32x2 arithmetic (FFMA2 / FADD2 / FMUL2 on sm_100): two elements per instruction on the FP32 pipe,
-// which is what bounds the fused epilogue.
-__device__ __forceinline__ float2 f2(float a, float b) { return make_float2(a, b); }
-__device__ __forceinline__ float2 f2s(float a) { return make_float2(a, a); }
-// Two Mish values; the two divisions share one reciprocal, 1/d.x = d.y / (d.x d.y) (halves the MUFU.RCP count; it
-// measured neutral, the epilogue is latency-bound).  x is clamped at 10: n/(n+2) already rounds to 1 there, and
-// d.x * d.y stays below 2.4e17.
-__device__ __forceinline__ float2 mish_fast2(float2 x) {
-  const float2 a = f2(fminf(x.x, 10.f), fminf(x.y, 10.f));
-  const float2 z = __fmul2_rn(a, f2s(1.4426950408889634f));
-  const float2 e = f2(ex2_ftz(z.x), ex2_ftz(z.y));
-  const float2 n = __fmul2_rn(e, __fadd2_rn(e, f2s(2.f)));
-  const float2 d = __fadd2_rn(n, f2s(2.f));
-  const float2 r = __fmul2_rn(f2s(rcp_ftz(d.x * d.y)), f2(d.y, d.x));
-  return __fmul2_rn(x, __fmul2_rn(n, r));
-}
-__device__ __forceinline__ float mish_fast(float x) {
-  const float e = exp_fast(fminf(x, 30.f));        // x > 30: n/(n+2) == 1 in fp32 already; keeps e*e finite
-  const float n = e * (e + 2.f);
-  return x * (n * rcp_ftz(n + 2.f));
-}
-
-// Pass 2 of the fused LayerNorm epilogue, specialised for the common case (whole 32-column blocks, planes out
-// through TMA stores, no fp32 side output): one block = two x16 TMEM loads, packed fp32x2 math, four 16-byte
-// swizzled smem stores per plane, then the block is handed to the TMA unit.
-template <int KIND, bool FAST = false>   // FAST: single-pass mode (PlanParams::passes == 1), the lo plane is neither computed nor stored
-__device__ __forceinline__ void epi_pass2_fast(const PlanParams& P, Ctx& c, const EpiThread& et, const EpiArgs& ea, int cb,
-                                               int nvalid, float inv_scale, float rstd, float nmr) {
-  const float* sb = c.vec; const float* sg = c.vec + kFusedMaxN; const float* sbe = c.vec + 2 * kFusedMaxN;
-  // staging tiles: two per group aliasing the idle W ring -- or, when the W ring is busy prefetching the next layer
-  // (c.wpf), ONE per group in the idle A ring, re-used once the previous store has read it
-  uint8_t* stg = c.wpf ? c.stage_base + et.grp * kStgBuf : c.stage_base + kWRingOff + et.grp * (2 * kStgBuf);
-  const bool lead_warp = (et.q == 0);   // one elected lane of the group's first warp issues, commits and waits (cheap in SASS: no waterfall)
-  const CUtensorMap* tmD = (ea.dstbuf == BUF_X) ? &P.tmXs : &P.tmHs;
-  const uint32_t swz = static_cast<uint32_t>((et.row >> 1) & 3);
-  const int row_hi = plane_row0(P, c.slot, ea.dstbuf, 0), row_lo = plane_row0(P, c.slot, ea.dstbuf, 1);
-  const float2 inv2 = f2s(inv_scale), rstd2 = f2s(rstd), nmr2 = f2s(nmr);
-  const int nblk = nvalid >> 5;
-  for (int blk = 0; blk < nblk; ++blk) {
-    const int c0 = cb + (blk << 5);
-    uint8_t* buf = c.wpf ? stg : stg + (blk & 1) * kStgBuf;
-    const uint32_t rowaddr = ptx::smem_u32(buf) + static_cast<uint32_t>(et.row) * 64u;
-    if (!c.wpf && blk >= 2) {                                     // buffer reuse: its previous store must have read it
-      if (lead_warp && ptx::elect_one()) ptx::bulk_wait_read<1>();
-      group_bar_sync(et.grp);
-    }
-#pragma unroll
-    for (int sub = 0; sub < 32; sub += 16) {
-      uint32_t v[16];
-      ptx::tmem_ld_32x16(et.taddr + c0 + sub, v);
-      ptx::tmem_ld_wait();
-      uint32_t hw[8], lw[8];
-#pragma unroll
-      for (int i4 = 0; i4 < 16; i4 += 4) {
-        const float4 b4 = lds128(sb + c0 + sub + i4);
-        const float4 g4 = lds128(sg + c0 + sub + i4);
-        const float4 e4 = lds128(sbe + c0 + sub + i4);
-        float2 t0 = __ffma2_rn(__ffma2_rn(__ffma2_rn(f2(__uint_as_float(v[i4]), __uint_as_float(v[i4 + 1])), inv2, f2(b4.x, b4.y)),
-                                          rstd2, nmr2), f2(g4.x, g4.y), f2(e4.x, e4.y));
-        float2 t1 = __ffma2_rn(__ffma2_rn(__ffma2_rn(f2(__uint_as_float(v[i4 + 2]), __uint_as_float(v[i4 + 3])), inv2, f2(b4.z, b4.w)),
-                                          rstd2, nmr2), f2(g4.z, g4.w), f2(e4.z, e4.w));
-        if (KIND == EPI_LN_MISH) { t0 = mish_fast2(t0); t1 = mish_fast2(t1); }
-        v[i4] = __float_as_uint(t0.x); v[i4 + 1] = __float_as_uint(t0.y);
-        v[i4 + 2] = __float_as_uint(t1.x); v[i4 + 3] = __float_as_uint(t1.y);
-      }
-      if (KIND == EPI_LN_SIMNORM) {
-        // SimNorm: softmax over groups of 8 consecutive columns (layers.py:84-88)
-#pragma unroll
-        for (int g0 = 0; g0 < 16; g0 += 8) {
-          float y[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) y[i] = __uint_as_float(v[g0 + i]);
-          float m = y[0];
-#pragma unroll
-          for (int i = 1; i < 8; ++i) m = fmaxf(m, y[i]);
-          float t = 0.f;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) { y[i] = exp_fast(y[i] - m); t += y[i]; }
-          const float rt = rcp_ftz(t);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) v[g0 + i] = __float_as_uint(y[i] * rt);
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float a0 = __uint_as_float(v[2 * i]), a1 = __uint_as_float(v[2 * i + 1]);
-        const __half2 h2 = __floats2half2_rn(a0, a1);
-        hw[i] = *reinterpret_cast<const uint32_t*>(&h2);
-        if (!FAST) {
-          const float2 hf = __half22float2(h2);
-          const float2 df = __fadd2_rn(f2(a0, a1), f2(-hf.x, -hf.y));
-          const __half2 l2 = __floats2half2_rn(df.x, df.y);
-          lw[i] = *reinterpret_cast<const uint32_t*>(&l2);
-        }
-      }
-      if (c.wpf && sub == 0 && blk >= 1) {
-        // single staging tile: the previous block's store was issued a whole block of math ago, so this wait is short
-        if (lead_warp && ptx::elect_one()) ptx::bulk_wait_read<0>();
-        group_bar_sync(et.grp);
-      }
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const uint32_t off = ((static_cast<uint32_t>((sub >> 3) + i) ^ swz) << 4);
-        ptx::st_shared_v4(rowaddr + off, hw[4 * i], hw[4 * i + 1], hw[4 * i + 2], hw[4 * i + 3]);
-        if (!FAST) ptx::st_shared_v4(rowaddr + kStgPlane + off, lw[4 * i], lw[4 * i + 1], lw[4 * i + 2], lw[4 * i + 3]);
-      }
-    }
-    ptx::fence_proxy_async_smem();
-    group_bar_sync(et.grp);
-    if (lead_warp && ptx::elect_one()) {
-      if (P.l2hint & 2) {     // evict-last on the activation-plane stores (re-read by the next layer, then overwritten):
-                              // DRAM write-back of the scratch 2.11 -> 1.43 GB per c2 iteration, -0.9 % per plan under the power cap
-        ptx::tma_store_2d_hint(tmD, buf, ea.dst_col0 + c0, row_hi, ptx::kL2EvictLast);
-        if (!FAST) ptx::tma_store_2d_hint(tmD, buf + kStgPlane, ea.dst_col0 + c0, row_lo, ptx::kL2EvictLast);
-      } else {
-        ptx::tma_store_2d(tmD, buf, ea.dst_col0 + c0, row_hi);
-        if (!FAST) ptx::tma_store_2d(tmD, buf + kStgPlane, ea.dst_col0 + c0, row_lo);
-      }
-      ptx::bulk_commit();
-    }
-  }
-  if (lead_warp && ptx::elect_one()) ptx::bulk_wait<0>();                               // stores performed before the layer is published
-}
-
-// bias + LayerNorm + (Mish | SimNorm); planes and/or fp32 rows out.  16 epilogue warps: 4 lane quarters x 4
-// column groups; a group owns whole 64-column blocks (the TMA-store granule).
-// Pass 1 reads the accumulator row once for shifted first/second moments (groups merged with Chan's
-// parallel-variance formula), pass 2 re-reads it 16 columns at a time, normalises, activates and emits.
-__device__ __forceinline__ void epi_ln_fused(const PlanParams& P, Ctx& c, const LayerRec& ly, const EpiArgs& ea) {
-  const EpiThread et = epi_thread(c);
-  const int N = ly.N;
-  const int nblocks = ly.Npad / 64;
-  const int bpg = (nblocks + kEpiGroups - 1) / kEpiGroups;        // 64-column blocks per group
-  const int cb = et.grp * bpg * 64;                               // this thread's columns: [cb, cb + ncols) & < N
-  const int ncols = max(0, min(bpg * 64, ly.Npad - cb));
-  const int nvalid = max(0, min(N - cb, ncols));
-  const float inv_scale = ly.inv_scale;
-  epi_stage_vectors(c, ly, true);
-  const float* sb = c.vec; const float* sg = c.vec + kFusedMaxN; const float* sbe = c.vec + 2 * kFusedMaxN;
-  if (nvalid > 0) {
-    const long long tw = prof_clock();
-    ptx::mbar_wait_long(&c.facc[0], c.fph0);
-    c.pf2 += prof_clock() - tw;
-  }
-  const bool tr0 = (et.grp == 0 && et.q == 0 && c.lane == 0), tr3 = (et.grp == 3 && et.q == 0 && c.lane == 0);
-  if (tr0) TDMPC2_TRACE(P, c, 4);
-  if (tr3) TDMPC2_TRACE(P, c, 10);
-  ptx::tc_fence_after();
-  // ---- pass 1: shifted moments of this group's columns
-  float x0 = 0.f, s = 0.f, q = 0.f;
-  float2 s2 = f2s(0.f), q2 = f2s(0.f);
-  const bool p1_fast = (nvalid > 0) && ((nvalid & 31) == 0);
-  if (p1_fast) {
-    // whole 32-column chunks: x32 loads, four independent packed accumulator chains
-    float2 sa = f2s(0.f), sbb = f2s(0.f), qa = f2s(0.f), qb = f2s(0.f);
-    const float2 inv2 = f2s(inv_scale);
-    for (int c0 = cb; c0 < cb + nvalid; c0 += 32) {
-      uint32_t v[32];
-      ptx::tmem_ld_32x32(et.taddr + c0, v);
-      ptx::tmem_ld_wait();
-      if (c0 == cb) x0 = fmaf(__uint_as_float(v[0]), inv_scale, sb[c0]);
-      const float2 nx0 = f2s(-x0);
-#pragma unroll
-      for (int i4 = 0; i4 < 32; i4 += 4) {
-        const float4 b4 = lds128(sb + c0 + i4);
-        const float2 xa = __ffma2_rn(f2(__uint_as_float(v[i4]), __uint_as_float(v[i4 + 1])), inv2, __fadd2_rn(f2(b4.x, b4.y), nx0));
-        const float2 xb = __ffma2_rn(f2(__uint_as_float(v[i4 + 2]), __uint_as_float(v[i4 + 3])), inv2, __fadd2_rn(f2(b4.z, b4.w), nx0));
-        sa = __fadd2_rn(sa, xa); qa = __ffma2_rn(xa, xa, qa);
-        sbb = __fadd2_rn(sbb, xb); qb = __ffma2_rn(xb, xb, qb);
-      }
-    }
-    s2 = __fadd2_rn(sa, sbb); q2 = __fadd2_rn(qa, qb);
-  }
-  for (int c0 = cb; c0 < cb + (p1_fast ? 0 : nvalid); c0 += 16) {
-    uint32_t v[16];
-    ptx::tmem_ld_32x16(et.taddr + c0, v);
-    ptx::tmem_ld_wait();
-    if (c0 == cb) x0 = fmaf(__uint_as_float(v[0]), inv_scale, sb[c0]);
-    const bool full = (c0 + 16 <= N);
-#pragma unroll
-    for (int i4 = 0; i4 < 16; i4 += 4) {
-      const float4 b4 = lds128(sb + c0 + i4);
-      const float bb[4] = {b4.x, b4.y, b4.z, b4.w};
-      if (full) {
-#pragma unroll
-        for (int j = 0; j < 4; j += 2) {
-          const float2 xv = __ffma2_rn(f2(__uint_as_float(v[i4 + j]), __uint_as_float(v[i4 + j + 1])), f2s(inv_scale),
-                                       f2(bb[j] - x0, bb[j + 1] - x0));
-          s2 = __fadd2_rn(s2, xv);
-          q2 = __ffma2_rn(xv, xv, q2);
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float d = fmaf(__uint_as_float(v[i4 + j]), inv_scale, bb[j]) - x0;
-          if (c0 + i4 + j < N) { s += d; q = fmaf(d, d, q); }
-        }
-      }
-    }
-  }
-  s += s2.x + s2.y;
-  q += q2.x + q2.y;
-  {
-    const float n_g = static_cast<float>(nvalid);
-    c.part[et.grp * kTileM + et.row] = nvalid > 0 ? x0 + s / n_g : 0.f;                       // group mean
-    c.part[(kEpiGroups + et.grp) * kTileM + et.row] = nvalid > 0 ? q - s * s / n_g : 0.f;     // group M2
-  }
-  if (tr0) TDMPC2_TRACE(P, c, 5);
-  epi_bar_sync();
-  if (tr0) TDMPC2_TRACE(P, c, 6);
-  float mean = 0.f, rstd;
-  {
-    float m2 = 0.f, cnt = 0.f;
-#pragma unroll
-    for (int g = 0; g < kEpiGroups; ++g) {
-      const int gb = g * bpg * 64;
-      const float ng = static_cast<float>(max(0, min(N - gb, min(bpg * 64, ly.Npad - gb))));
-      if (ng > 0.f) {
-        const float mg = c.part[g * kTileM + et.row], m2g = c.part[(kEpiGroups + g) * kTileM + et.row];
-        const float tot = cnt + ng, delta = mg - mean;
-        mean += delta * (ng / tot);
-        m2 += m2g + delta * delta * (cnt * ng / tot);
-        cnt = tot;
-      }
-    }
-    rstd = rsqrtf(m2 / static_cast<float>(N) + 1e-5f);            // nn.LayerNorm eps (layers.py:101), biased variance
-  }
-  const float nmr = -mean * rstd;
-  if (ea.dstbuf >= 0 && !ea.out_f32 && (N % 32 == 0) && (ea.dst_col0 % 32 == 0)) {
-    if (P.passes == 1) {
-      if (ea.kind == EPI_LN_MISH) epi_pass2_fast<EPI_LN_MISH, true>(P, c, et, ea, cb, nvalid, inv_scale, rstd, nmr);
-      else epi_pass2_fast<EPI_LN_SIMNORM, true>(P, c, et, ea, cb, nvalid, inv_scale, rstd, nmr);
-    } else {
-      if (ea.kind == EPI_LN_MISH) epi_pass2_fast<EPI_LN_MISH>(P, c, et, ea, cb, nvalid, inv_scale, rstd, nmr);
-      else epi_pass2_fast<EPI_LN_SIMNORM>(P, c, et, ea, cb, nvalid, inv_scale, rstd, nmr);
-    }
-    return;
-  }
-  // ---- pass 2 (general path): normalise, activate, emit
-  __half* dhi = ea.dstbuf >= 0 ? plane_ptr(P, c.slot, ea.dstbuf, 0) : nullptr;
-  __half* dlo = ea.dstbuf >= 0 ? plane_ptr(P, c.slot, ea.dstbuf, 1) : nullptr;
-  const int pitch = ea.dstbuf >= 0 ? plane_pitch(P, ea.dstbuf) : 0;
-  const int orow = ea.rowmap ? ea.rowmap[et.row] : et.row;
-  // Plane output goes through a 128B-swizzled smem tile [128 rows x 64 cols] per plane and a TMA store
-  // (thread-per-row global stores would touch 32 cache lines per instruction).  The staging tiles alias
-  // the operand pipeline stages, which are idle here: every MMA of this layer has retired.
-  const bool use_tma = (dhi != nullptr) && (N % 32 == 0) && (ea.dst_col0 % 32 == 0);
-  uint8_t* stg = c.stage_base + kWRingOff + et.grp * (2 * kStgBuf);   // per group: 2 buffers x (hi 8 KiB | lo 8 KiB)
-  const bool leader = (et.q == 0) && (c.lane == 0);
-  const CUtensorMap* tmD = (ea.dstbuf == BUF_X) ? &P.tmXs : &P.tmHs;
-  const uint32_t swz = static_cast<uint32_t>((et.row >> 1) & 3);     // 64-byte swizzle: chunk ^= (row / 2) % 4
-  for (int c0 = cb; c0 < cb + nvalid; c0 += 16) {
-    const int sub = (c0 - cb) & 31;                               // 0 | 16 within the 32-column block
-    const int blk = (c0 - cb) >> 5;
-    uint8_t* buf = stg + (blk & 1) * kStgBuf;
-    const uint32_t rowaddr = ptx::smem_u32(buf) + static_cast<uint32_t>(et.row) * 64u;
-    if (use_tma && sub == 0 && blk >= 2) {                        // buffer reuse: its previous store must have read it
-      if (leader) ptx::bulk_wait_read<1>();
-      group_bar_sync(et.grp);
-    }
-    uint32_t v[16];
-    ptx::tmem_ld_32x16(et.taddr + c0, v);
-    ptx::tmem_ld_wait();
-    const bool full = (c0 + 16 <= N);
-    float y[16];
-#pragma unroll
-    for (int i4 = 0; i4 < 16; i4 += 4) {
-      const float4 b4 = lds128(sb + c0 + i4);
-      const float4 g4 = lds128(sg + c0 + i4);
-      const float4 e4 = lds128(sbe + c0 + i4);
-      const float bb[4] = {b4.x, b4.y, b4.z, b4.w}, gg[4] = {g4.x, g4.y, g4.z, g4.w}, ee[4] = {e4.x, e4.y, e4.z, e4.w};
-#pragma unroll
-      for (int j = 0; j < 4; j += 2) {
-        const float2 x = __ffma2_rn(f2(__uint_as_float(v[i4 + j]), __uint_as_float(v[i4 + j + 1])), f2s(inv_scale), f2(bb[j], bb[j + 1]));
-        const float2 u = __ffma2_rn(x, f2s(rstd), f2s(nmr));
-        float2 t = __ffma2_rn(u, f2(gg[j], gg[j + 1]), f2(ee[j], ee[j + 1]));
-        if (ea.kind == EPI_LN_MISH) t = mish_fast2(t);
-        y[i4 + j] = t.x; y[i4 + j + 1] = t.y;
-      }
-    }
-    if (!full) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        if (c0 + i >= N) y[i] = (ea.kind == EPI_LN_MISH) ? 0.f : -CUDART_INF_F;
-    }
-    if (ea.kind == EPI_LN_MISH) {
-    } else {
-      // SimNorm: softmax over groups of 8 consecutive columns (layers.py:84-88)
-#pragma unroll
-      for (int g0 = 0; g0 < 16; g0 += 8) {
-        float m = y[g0];
-#pragma unroll
-        for (int i = 1; i < 8; ++i) m = fmaxf(m, y[g0 + i]);
-        float t = 0.f;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) { y[g0 + i] = exp_fast(y[g0 + i] - m); t += y[g0 + i]; }
-        const float rt = rcp_ftz(t);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) y[g0 + i] *= rt;
-      }
-    }
-    if (dhi) {
-      if (use_tma || (full && ((ea.dst_col0 & 7) == 0))) {
-        uint32_t hw[8], lw[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          // |y| <= sqrt(N) max|g| + max|b| after LayerNorm (Mish and SimNorm only shrink it): far inside fp16 range
-          const float a0 = y[2 * i], a1 = y[2 * i + 1];
-          const __half2 h2 = __floats2half2_rn(a0, a1);
-          const float2 hf = __half22float2(h2);
-          const float2 df = __fadd2_rn(f2(a0, a1), f2(-hf.x, -hf.y));
-          const __half2 l2 = __floats2half2_rn(df.x, df.y);
-          hw[i] = *reinterpret_cast<const uint32_t*>(&h2);
-          lw[i] = *reinterpret_cast<const uint32_t*>(&l2);
-        }
-        if (use_tma) {
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const uint32_t chunk = static_cast<uint32_t>((sub >> 3) + i);          // 16-byte chunk index in the 64 B row
-            const uint32_t off = ((chunk ^ swz) << 4);
-            ptx::st_shared_v4(rowaddr + off, hw[4 * i], hw[4 * i + 1], hw[4 * i + 2], hw[4 * i + 3]);
-            ptx::st_shared_v4(rowaddr + kStgPlane + off, lw[4 * i], lw[4 * i + 1], lw[4 * i + 2], lw[4 * i + 3]);
-          }
-          if (sub == 16) {                                        // 32-column block complete: hand it to the TMA unit
-            ptx::fence_proxy_async_smem();
-            group_bar_sync(et.grp);
-            if (leader) {
-              const int col = ea.dst_col0 + c0 - 16;
-              ptx::tma_store_2d(tmD, buf, col, plane_row0(P, c.slot, ea.dstbuf, 0));
-              ptx::tma_store_2d(tmD, buf + kStgPlane, col, plane_row0(P, c.slot, ea.dstbuf, 1));
-              ptx::bulk_commit();
-            }
-          }
-        } else {
-          __half* ph = dhi + static_cast<size_t>(et.row) * pitch + ea.dst_col0 + c0;
-          __half* pl = dlo + static_cast<size_t>(et.row) * pitch + ea.dst_col0 + c0;
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            __stcg(reinterpret_cast<uint4*>(ph) + i, make_uint4(hw[4 * i], hw[4 * i + 1], hw[4 * i + 2], hw[4 * i + 3]));
-            __stcg(reinterpret_cast<uint4*>(pl) + i, make_uint4(lw[4 * i], lw[4 * i + 1], lw[4 * i + 2], lw[4 * i + 3]));
-          }
-        }
-      } else {
-        __half* ph = dhi + static_cast<size_t>(et.row) * pitch + ea.dst_col0 + c0;
-        __half* pl = dlo + static_cast<size_t>(et.row) * pitch + ea.dst_col0 + c0;
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-          if (c0 + i < N) split_store(ph + i, pl + i, y[i]);
-      }
-    }
-    if (ea.out_f32 && orow >= 0) {
-      float* po = ea.out_f32 + static_cast<size_t>(orow) * ea.out_pitch + c0;
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        if (c0 + i < N) po[i] = y[i];
-    }
-  }
-  if (tr0) TDMPC2_TRACE(P, c, 7);
-  if (tr3) TDMPC2_TRACE(P, c, 11);
-  if (use_tma && leader) ptx::bulk_wait<0>();                     // stores performed before the layer is published
-  if (tr0) TDMPC2_TRACE(P, c, 8);
-}
-
-// Head epilogues (plain Linear outputs, Npad <= 256 so the accumulator is chunk 0 only).
-// Two-hot heads with <= 128 bins and pi heads with <= 64 action dims are spread over all four column groups
-// (32 bins / 16 action dims per group); anything larger runs on column group 0 alone.
-// Can this head's epilogue take K-segmented accumulators (segments summed in registers)?  The common shapes only:
-// two-hot heads with <= 128 bins, pi heads with <= 64 action dims, the termination head.
-__device__ __forceinline__ bool head_seg_ok(const PlanParams& P, int kind) {
-  return (kind == EPI_TWOHOT && P.B <= 32 * kEpiGroups) || (kind == EPI_PI && P.A <= 16 * kEpiGroups) || kind == EPI_TERM;
-}
-
-// `nseg` > 1: the accumulator arrives in K-segments alternating between TMEM buffers 0 / 1 (tc_mma_head_seg); each
-// thread adds the segments of its own columns in registers.  v[0..32): this thread's 32 columns at column offset col0
-// (two-hot: bins 32*grp..; pi: 16 mean logits then 16 log_std logits; termination: column 0).
-template <bool EPISODIC>
-__device__ __forceinline__ void epi_head_fused(const PlanParams& P, Ctx& c, const LayerRec& ly, const EpiArgs& ea, int nseg) {
-  const EpiThread et = epi_thread(c);
-  const float inv_scale = ly.inv_scale;
-  epi_stage_vectors(c, ly, false);
-  const float* sb = c.vec;
-  if (ea.kind == EPI_TWOHOT) {
-    // bins -> smem (second vector slot)
-    for (int i = threadIdx.x - kEpiWarp0 * 32; i < P.B; i += kEpiThreads) c.vec[kFusedMaxN + i] = P.bins[i];
-    epi_bar_sync();
-  }
-  const bool wide_twohot = (ea.kind == EPI_TWOHOT) && (P.B <= 32 * kEpiGroups);
-  const bool wide_pi = (ea.kind == EPI_PI) && (P.A <= 16 * kEpiGroups);
-  float v[32];                                         // this thread's accumulator values (scaled domain)
-  if (nseg > 1) {
-    // every epilogue warp takes part in the hand-off protocol, whether or not it owns columns of this head
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = 0.f;
-    const bool mine = wide_twohot || wide_pi || et.grp == 0;
-    for (int seg = 0; seg < nseg; ++seg) {
-      const int b = seg & 1;
-      const uint32_t ph = (b ? c.fph1 : c.fph0) ^ static_cast<uint32_t>((seg >> 1) & 1);
-      ptx::mbar_wait_long(&c.facc[b], ph);
-      ptx::tc_fence_after();
-      if (mine) {
-        const uint32_t ta = et.taddr + b * kNch;
-        // two 16-column loads (keeps the live registers at acc[32] + 16): columns [c_lo, +16) and [c_hi, +16)
-        const uint32_t c_lo = wide_pi ? 16 * et.grp : (wide_twohot ? 32 * et.grp : 0);
-        const uint32_t c_hi = wide_pi ? P.Apad + 16 * et.grp : c_lo + 16;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t a0[16];
-          ptx::tmem_ld_32x16(ta + (h ? c_hi : c_lo), a0);
-          ptx::tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[16 * h + i] += __uint_as_float(a0[i]);
-        }
-      }
-      if (seg + 2 < nseg) {                            // the buffer is reused: tell the MMA issuer it has been read
-        ptx::tc_fence_before();
-        epi_bar_sync();
-        if (threadIdx.x == kEpiWarp0 * 32) {
-          if (c.cg2) ptx::mbar_arrive_leader(&c.acc_empty[b]);
-          else ptx::mbar_arrive(&c.acc_empty[b]);
-        }
-      }
-    }
-    if (!mine) return;
-  } else {
-    if (!wide_twohot && !wide_pi && et.grp != 0) return;
-    {
-      const long long tw = prof_clock();
-      ptx::mbar_wait_long(&c.facc[0], c.fph0);
-      c.pf2 += prof_clock() - tw;
-    }
-    ptx::tc_fence_after();
-  }
-  if (wide_twohot) {
-    // two_hot_inv (math.py:74-83) with the 4 groups each owning 32 bins: max, then exp-sum and bin-weighted sum,
-    // exchanged through smem (part: [0,4) max, [4,8) sum; third array in the unused LN-beta vector slot).
-    const float* bins = c.vec + kFusedMaxN;
-    float* xch = c.vec + 2 * kFusedMaxN;                // [kEpiGroups][128]
-    const int B = P.B, c0 = 32 * et.grp;
-    if (nseg == 1) {
-      uint32_t t32[32];
-      ptx::tmem_ld_32x32(et.taddr + c0, t32);
-      ptx::tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(t32[i]);
-    }
-    float (&x)[32] = v;                                // logits, in place
-    float m = -CUDART_INF_F;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      x[i] = (c0 + i < B) ? fmaf(v[i], inv_scale, sb[min(c0 + i, B - 1)]) : -CUDART_INF_F;
-      m = fmaxf(m, x[i]);
-    }
-    c.part[et.grp * kTileM + et.row] = m;
-    epi_bar_sync();
-#pragma unroll
-    for (int g = 0; g < kEpiGroups; ++g) m = fmaxf(m, c.part[g * kTileM + et.row]);
-    float ssum = 0.f, acc = 0.f;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const float e = (c0 + i < B) ? exp_fast(x[i] - m) : 0.f;     // exp(-inf - m) would be 0 as well; keep NaN rows NaN
-      ssum += e;
-      acc = fmaf(e, bins[min(c0 + i, B - 1)], acc);
-    }
-    c.part[(kEpiGroups + et.grp) * kTileM + et.row] = ssum;
-    xch[et.grp * kTileM + et.row] = acc;
-    epi_bar_sync();
-    if (et.grp == 0) {
-      float S = 0.f, Acc = 0.f;
-#pragma unroll
-      for (int g = 0; g < kEpiGroups; ++g) { S += c.part[(kEpiGroups + g) * kTileM + et.row]; Acc += xch[g * kTileM + et.row]; }
-      head_commit<EPISODIC>(P, c, ea, et.row, symexp_f(__fdiv_rn(Acc, S)));
-    }
-  } else if (EPISODIC && ea.kind == EPI_TERM) {
-    // termination head (one output column): group 0's thread of each row updates the row's sticky flag
-    if (nseg == 1) {
-      uint32_t t16[16];
-      ptx::tmem_ld_32x16(et.taddr, t16);
-      ptx::tmem_ld_wait();
-      v[0] = __uint_as_float(t16[0]);
-    }
-    term_commit(c, et.row, fmaf(v[0], inv_scale, sb[0]));
-  } else if (ea.kind == EPI_TWOHOT) {
-    const float* bins = c.vec + kFusedMaxN;
-    const int B = P.B;
-    float m = -CUDART_INF_F;
-    for (int c0 = 0; c0 < B; c0 += 32) {
-      uint32_t v[32];
-      ptx::tmem_ld_32x32(et.taddr + c0, v);
-      ptx::tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (c0 + i < B) m = fmaxf(m, fmaf(__uint_as_float(v[i]), inv_scale, sb[c0 + i]));
-    }
-    float ssum = 0.f, acc = 0.f;
-    for (int c0 = 0; c0 < B; c0 += 32) {
-      uint32_t v[32];
-      ptx::tmem_ld_32x32(et.taddr + c0, v);
-      ptx::tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (c0 + i < B) {
-          const float e = exp_fast(fmaf(__uint_as_float(v[i]), inv_scale, sb[c0 + i]) - m);
-          ssum += e;
-          acc = fmaf(e, bins[c0 + i], acc);
-        }
-    }
-    head_commit<EPISODIC>(P, c, ea, et.row, symexp_f(__fdiv_rn(acc, ssum)));
-  } else if (ea.kind == EPI_PI) {
-    const RowMap rm = map_row(P, ea.tile, et.row);
-    const int e = rm.env < 0 ? 0 : rm.env, idx = rm.env < 0 ? 0 : rm.idx;
-    const int task = P.task ? P.task[e] : 0;
-    __half* xhi = plane_ptr(P, c.slot, BUF_X, 0) + static_cast<size_t>(et.row) * P.KpadX + P.L + P.T;
-    __half* xlo = plane_ptr(P, c.slot, BUF_X, 1) + static_cast<size_t>(et.row) * P.KpadX + P.L + P.T;
-    const float* eps = ea.eps_base ? ea.eps_base + (static_cast<size_t>(e) * ea.eps_rows + idx) * P.A : nullptr;   // nullptr: in-kernel noise
-    const int a_begin = wide_pi ? 16 * et.grp : 0;
-    const int a_end = wide_pi ? min(P.A, a_begin + 16) : P.A;
-    for (int a0 = a_begin; a0 < a_end; a0 += 16) {
-      uint32_t vm[16], vs[16];
-      if (nseg > 1) {                                   // wide_pi only: one 16-column block per thread, already summed
-#pragma unroll
-        for (int i = 0; i < 16; ++i) { vm[i] = __float_as_uint(v[i]); vs[i] = __float_as_uint(v[16 + i]); }
-      } else {
-        ptx::tmem_ld_32x16(et.taddr + a0, vm);            // mean logits, columns [a0, a0+16)
-        ptx::tmem_ld_32x16(et.taddr + P.Apad + a0, vs);   // log_std logits, columns [Apad+a0, Apad+a0+16) (aligned)
-        ptx::tmem_ld_wait();
-      }
-      // 16 action columns = 32 B per plane: two 16-byte stores when the whole span lies inside the row
-      // (columns past A are zero-weight padding of X, so writing zeros there is harmless)
-      const bool vec = (((P.L + P.T) & 7) == 0) && (P.L + P.T + a0 + 16 <= P.KpadX);
-      uint32_t hw[8], lw[8];
-#pragma unroll
-      for (int i = 0; i < 16; i += 2) {
-        float act2[2];
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int a = a0 + i + u;
-          act2[u] = 0.f;
-          if (a < a_end) {
-            const float mu = fmaf(__uint_as_float(vm[i + u]), inv_scale, sb[a]);
-            const float ls = fmaf(__uint_as_float(vs[i + u]), inv_scale, sb[P.Apad + a]);
-            act2[u] = pi_action(P, mu, ls, eps ? __ldcs(&eps[a]) : noise_pi_at(P, e, idx, a), task, a);
-            if (!vec) split_store(xhi + a, xlo + a, act2[u]);
-            if (ea.act_out && rm.env >= 0)
-              ea.act_out[((static_cast<size_t>(e) * P.H + ea.t_out) * P.P + idx) * P.A + a] = act2[u];
-          }
-        }
-        __half h0, l0, h1, l1;
-        split_f(act2[0], h0, l0);
-        split_f(act2[1], h1, l1);
-        hw[i >> 1] = static_cast<uint32_t>(__half_as_ushort(h0)) | (static_cast<uint32_t>(__half_as_ushort(h1)) << 16);
-        lw[i >> 1] = static_cast<uint32_t>(__half_as_ushort(l0)) | (static_cast<uint32_t>(__half_as_ushort(l1)) << 16);
-      }
-      if (vec) {
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          __stcg(reinterpret_cast<uint4*>(xhi + a0) + i, make_uint4(hw[4 * i], hw[4 * i + 1], hw[4 * i + 2], hw[4 * i + 3]));
-          __stcg(reinterpret_cast<uint4*>(xlo + a0) + i, make_uint4(lw[4 * i], lw[4 * i + 1], lw[4 * i + 2], lw[4 * i + 3]));
-        }
-      }
-    }
-  } else {  // EPI_RAW
-    const int orow = ea.rowmap ? ea.rowmap[et.row] : et.row;
-    for (int c0 = 0; c0 < ly.N; c0 += 32) {
-      uint32_t v[32];
-      ptx::tmem_ld_32x32(et.taddr + c0, v);
-      ptx::tmem_ld_wait();
-      if (orow >= 0) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (c0 + i < ly.N)
-            ea.out_f32[static_cast<size_t>(orow) * ea.out_pitch + c0 + i] = fmaf(__uint_as_float(v[i]), inv_scale, sb[c0 + i]);
-      }
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------ layers wider than TMEM (48M / 317M presets)
-// A LayerNorm layer with Npad > 512 is produced in SUPER-CHUNKS of 512 output columns (the whole TMEM): each is one
-// fused-style GEMM -- K outermost, the A K-chunks streamed once per super-chunk, weights split over the CTA pair --
-// after which all 16 epilogue warps DRAIN the accumulator: x = acc * 2^-k + bias goes to the slot's fp32 raw scratch,
-// stored column-major ([col][128 rows]: a warp's 32 rows of one column are one 128-byte line) while the thread that
-// owns (row, column group) keeps running shifted moments of its row.  The MMA issuer waits for the drain (acc_empty)
-// before it overwrites TMEM; the TMA producer meanwhile refills the operand rings for the next super-chunk.  After the
-// last super-chunk the row statistics are merged across the 4 column groups (Chan) and ONE pass over the raw scratch
-// normalises, activates, splits to fp16 hi/lo and sends the planes out through swizzled smem tiles + TMA stores.
-// Every thread reads back exactly the raw elements it wrote itself.
-struct WideCols { int cb, ncols; };
-__device__ __forceinline__ WideCols wide_cols(const LayerRec& ly, int sc, int grp) {
-  const int wsc = min(kFusedMaxN, ly.Npad - sc * kFusedMaxN);     // 128 .. 512, multiple of 128
-  const int nblocks = wsc / 64;
-  const int bpg = (nblocks + kEpiGroups - 1) / kEpiGroups;
-  WideCols w;
-  w.cb = grp * bpg * 64;
-  w.ncols = max(0, min(bpg * 64, wsc - w.cb));
-  return w;
-}
-
-// LayerNorm affine + activation of 16 consecutive columns (x already holds acc * 2^-k + bias), in place.
-template <int KIND>
-__device__ __forceinline__ void wide_norm16(float (&y)[16], const float* __restrict__ g, const float* __restrict__ be,
-                                            float2 rstd2, float2 nmr2, int nvalid) {
-#pragma unroll
-  for (int i4 = 0; i4 < 16; i4 += 4) {
-    const float4 g4 = __ldg(reinterpret_cast<const float4*>(g + i4));
-    const float4 e4 = __ldg(reinterpret_cast<const float4*>(be + i4));
-    float2 t0 = __ffma2_rn(__ffma2_rn(f2(y[i4], y[i4 + 1]), rstd2, nmr2), f2(g4.x, g4.y), f2(e4.x, e4.y));
-    float2 t1 = __ffma2_rn(__ffma2_rn(f2(y[i4 + 2], y[i4 + 3]), rstd2, nmr2), f2(g4.z, g4.w), f2(e4.z, e4.w));
-    if (KIND == EPI_LN_MISH) { t0 = mish_fast2(t0); t1 = mish_fast2(t1); }
-    y[i4] = t0.x; y[i4 + 1] = t0.y; y[i4 + 2] = t1.x; y[i4 + 3] = t1.y;
-  }
-  if (nvalid < 16) {
-#pragma unroll
-    for (int i = 0; i < 16; ++i)
-      if (i >= nvalid) y[i] = (KIND == EPI_LN_MISH) ? 0.f : -CUDART_INF_F;
-  }
-  if (KIND == EPI_LN_SIMNORM) {
-    // SimNorm: softmax over groups of 8 consecutive columns (layers.py:84-88)
-#pragma unroll
-    for (int g0 = 0; g0 < 16; g0 += 8) {
-      float m = y[g0];
-#pragma unroll
-      for (int i = 1; i < 8; ++i) m = fmaxf(m, y[g0 + i]);
-      float t = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) { y[g0 + i] = exp_fast(y[g0 + i] - m); t += y[g0 + i]; }
-      const float rt = rcp_ftz(t);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) y[g0 + i] *= rt;
-    }
-  }
-}
-
-// The normalise pass of a wide layer, common case (planes out through TMA stores, whole 32-column blocks).  Both operand
-// rings are idle by now (every MMA of the layer has retired), so the whole 192 KiB of operand smem serve as staging:
-// per column group two 16 KiB INPUT buffers in the W ring -- 32 raw columns x 128 rows fp32, exactly one contiguous
-// block of the column-major raw scratch, fetched with one bulk copy (cp.async.bulk, mbarrier completion) two blocks
-// ahead of its use, which hides the HBM latency of the 317M preset's raw scratch (2 MB per slot) -- and one 16 KiB
-// OUTPUT tile (hi | lo planes, 64-byte swizzle) in the A ring that leaves through TMA stores.
-// Block b (columns [32 b, 32 b + 32)) belongs to column group b % 4: the raw scratch is global memory, so the
-// assignment need not follow the drain's (the stats-merge barrier has made every drained value visible).
-template <int KIND>   // EPI_LN_MISH | EPI_LN_SIMNORM
-__device__ __forceinline__ void wide_pass2_tma(const PlanParams& P, Ctx& c, const EpiThread& et, const LayerRec& ly, const EpiArgs& ea,
-                                               float rstd, float nmr) {
-  const int nblk = ly.N >> 5;                                         // N % 32 == 0 on this path
-  const float* rawT = raw_ptr(P, c.slot);                            // block b at rawT + b * 32 * 128
-  uint8_t* inb = c.stage_base + kWRingOff + et.grp * (2 * kStgBuf);  // 2 x 16 KiB raw blocks
-  uint8_t* stg = c.stage_base + et.grp * kStgBuf;                    // 16 KiB output tile (hi 8 KiB | lo 8 KiB)
-  uint64_t* bars = c.rawb + et.grp * 2;
-  const bool lead_warp = (et.q == 0);   // one elected lane of the group's first warp issues, commits and waits (cheap in SASS: no waterfall)
-  const CUtensorMap* tmD = (ea.dstbuf == BUF_X) ? &P.tmXs : &P.tmHs;
-  const uint32_t swz = static_cast<uint32_t>((et.row >> 1) & 3);
-  const int row_hi = plane_row0(P, c.slot, ea.dstbuf, 0), row_lo = plane_row0(P, c.slot, ea.dstbuf, 1);
-  const float2 rstd2 = f2s(rstd), nmr2 = f2s(nmr);
-  const uint32_t rowaddr = ptx::smem_u32(stg) + static_cast<uint32_t>(et.row) * 64u;
-  uint32_t it = c.rb_it;                              // blocks consumed by this group so far: buffer = it & 1
-  if (lead_warp && ptx::elect_one()) {
-    for (int j = 0; j < 2; ++j) {
-      const int b = et.grp + 4 * j;
-      if (b < nblk) {
-        const uint32_t ib = (it + j) & 1u;
-        ptx::mbar_expect_tx(&bars[ib], kStgBuf);
-        ptx::bulk_load(inb + ib * kStgBuf, rawT + static_cast<size_t>(b) * 32 * kTileM, kStgBuf, &bars[ib]);
-      }
-    }
-  }
-  for (int b = et.grp; b < nblk; b += kEpiGroups, ++it) {
-    const uint32_t ib = it & 1u;
-    // the previous block's TMA store has finished reading the output tile
-    if (lead_warp && ptx::elect_one()) ptx::bulk_wait_read<0>();
-    group_bar_sync(et.grp);
-    ptx::mbar_wait(&bars[ib], (it >> 1) & 1u);
-    const float* blk = reinterpret_cast<const float*>(inb + ib * kStgBuf) + et.row;     // element (col, row) at blk[col * 128]
-#pragma unroll
-    for (int sub = 0; sub < 32; sub += 16) {
-      float y[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) y[i] = blk[(sub + i) * kTileM];
-      wide_norm16<KIND>(y, ly.ln_g + b * 32 + sub, ly.ln_b + b * 32 + sub, rstd2, nmr2, 16);
-      uint32_t hw[8], lw[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float a0 = y[2 * i], a1 = y[2 * i + 1];
-        const __half2 h2 = __floats2half2_rn(a0, a1);
-        const float2 hf = __half22float2(h2);
-        const float2 df = __fadd2_rn(f2(a0, a1), f2(-hf.x, -hf.y));
-        const __half2 l2 = __floats2half2_rn(df.x, df.y);
-        hw[i] = *reinterpret_cast<const uint32_t*>(&h2);
-        lw[i] = *reinterpret_cast<const uint32_t*>(&l2);
-      }
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const uint32_t off = ((static_cast<uint32_t>((sub >> 3) + i) ^ swz) << 4);
-        ptx::st_shared_v4(rowaddr + off, hw[4 * i], hw[4 * i + 1], hw[4 * i + 2], hw[4 * i + 3]);
-        ptx::st_shared_v4(rowaddr + kStgPlane + off, lw[4 * i], lw[4 * i + 1], lw[4 * i + 2], lw[4 * i + 3]);
-      }
-    }
-    ptx::fence_proxy_async_smem();
-    group_bar_sync(et.grp);                            // tile complete; every thread of the group is done with raw buffer ib
-    if (lead_warp && ptx::elect_one()) {
-      ptx::tma_store_2d(tmD, stg, ea.dst_col0 + b * 32, row_hi);
-      ptx::tma_store_2d(tmD, stg + kStgPlane, ea.dst_col0 + b * 32, row_lo);
-      ptx::bulk_commit();
-      const int nb = b + 2 * kEpiGroups;               // refill the buffer just released, two blocks ahead
-      if (nb < nblk) {
-        ptx::mbar_expect_tx(&bars[ib], kStgBuf);
-        ptx::bulk_load(inb + ib * kStgBuf, rawT + static_cast<size_t>(nb) * 32 * kTileM, kStgBuf, &bars[ib]);
-      }
-    }
-  }
-  c.rb_it = it;
-  if (lead_warp && ptx::elect_one()) ptx::bulk_wait<0>();                                 // stores performed before the layer is published
-}
-
-// General fallback of the normalise pass (fp32 row output, ragged N, unaligned destination): plain loads of the raw
-// scratch, scalar stores.  Only the encoder's last layer and the diagnostic mode come here.
-template <int KIND>
-__device__ __forceinline__ void wide_pass2_general(const PlanParams& P, Ctx& c, const EpiThread& et, const LayerRec& ly, const EpiArgs& ea,
-                                                   float rstd, float nmr) {
-  const int N = ly.N;
-  const float* rawT = raw_ptr(P, c.slot) + et.row;
-  const bool planes = ea.dstbuf >= 0;
-  __half* dhi = planes ? plane_ptr(P, c.slot, ea.dstbuf, 0) + static_cast<size_t>(et.row) * plane_pitch(P, ea.dstbuf) + ea.dst_col0 : nullptr;
-  __half* dlo = planes ? plane_ptr(P, c.slot, ea.dstbuf, 1) + static_cast<size_t>(et.row) * plane_pitch(P, ea.dstbuf) + ea.dst_col0 : nullptr;
-  const int orow = ea.rowmap ? ea.rowmap[et.row] : et.row;
-  float* po = (ea.out_f32 && orow >= 0) ? ea.out_f32 + static_cast<size_t>(orow) * ea.out_pitch : nullptr;
-  const float2 rstd2 = f2s(rstd), nmr2 = f2s(nmr);
-  for (int c0 = 16 * et.grp; c0 < N; c0 += 16 * kEpiGroups) {        // N <= Npad, the parameter vectors are padded to Npad
-    float y[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) y[i] = (c0 + i < ly.Npad) ? __ldcg(rawT + static_cast<size_t>(c0 + i) * kTileM) : 0.f;
-    wide_norm16<KIND>(y, ly.ln_g + c0, ly.ln_b + c0, rstd2, nmr2, min(16, N - c0));
-#pragma unroll
-    for (int i = 0; i < 16; ++i)
-      if (c0 + i < N) {
-        if (po) po[c0 + i] = y[i];
-        if (planes) split_store(dhi + c0 + i, dlo + c0 + i, y[i]);
-      }
-  }
-}
-
-// Epilogue warps of a wide layer (EPI_LN_MISH | EPI_LN_SIMNORM | EPI_RAW).
-__device__ __forceinline__ void epi_wide(const PlanParams& P, Ctx& c, const LayerRec& ly, const EpiArgs& ea, int nsc, int nseg) {
-  const EpiThread et = epi_thread(c);
-  const int N = ly.N;
-  const float inv_scale = ly.inv_scale;
-  const bool is_ln = (ea.kind != EPI_RAW);
-  float* rawT = raw_ptr(P, c.slot) + et.row;                        // element (col, row) at rawT[col * 128]
-  // running shifted moments of this thread's row over the columns of its group (all super-chunks)
-  float x0 = 0.f, s = 0.f, q = 0.f;
-  float2 sa = f2s(0.f), sbb = f2s(0.f), qa = f2s(0.f), qb = f2s(0.f);
-  bool have_x0 = false;
-  const float2 inv2 = f2s(inv_scale);
-  const bool tr0 = (et.grp == 0 && et.q == 0 && c.lane == 0);
-  for (int sc = 0; sc < nsc; ++sc) {
-   const WideCols wc = wide_cols(ly, sc, et.grp);
-   for (int seg = 0; seg < nseg; ++seg) {
-    // K-segments: the tensor core's fp32 accumulator rounds toward zero on every K = 16 step, an error that grows
-    // linearly with the reduction length; flushing the partial sum every P.kseg K-chunks and adding the segments here
-    // with round-to-nearest bounds it (at the price of one more drain per segment).
-    const bool last_seg = (seg == nseg - 1);
-    {
-      const long long tw = prof_clock();
-      ptx::mbar_wait_sleep(&c.facc[0], c.fph0 ^ static_cast<uint32_t>((sc * nseg + seg) & 1), P.wide_sleep_ns);
-      c.pf2 += prof_clock() - tw;
-    }
-    ptx::tc_fence_after();
-    if (tr0 && sc == 0 && seg == 0) TDMPC2_TRACE(P, c, 4);          // first accumulator ready
-    if (tr0 && sc == nsc - 1 && last_seg) TDMPC2_TRACE(P, c, 10);   // last accumulator ready
-    for (int c0 = wc.cb; c0 < wc.cb + wc.ncols; c0 += 32) {
-      const int gcol = sc * kFusedMaxN + c0;
-      uint32_t v[32];
-      ptx::tmem_ld_32x32(et.taddr + c0, v);
-      if (seg == 0) {
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int i4 = 0; i4 < 32; i4 += 4) {
-          const float4 b4 = __ldg(reinterpret_cast<const float4*>(ly.bias + gcol + i4));
-          const float2 xa = __ffma2_rn(f2(__uint_as_float(v[i4]), __uint_as_float(v[i4 + 1])), inv2, f2(b4.x, b4.y));
-          const float2 xb = __ffma2_rn(f2(__uint_as_float(v[i4 + 2]), __uint_as_float(v[i4 + 3])), inv2, f2(b4.z, b4.w));
-          v[i4] = __float_as_uint(xa.x); v[i4 + 1] = __float_as_uint(xa.y);
-          v[i4 + 2] = __float_as_uint(xb.x); v[i4 + 3] = __float_as_uint(xb.y);
-        }
-      } else {
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int h = 0; h < 32; h += 8) {                          // this thread's own partial sums of the earlier segments
-          float prev[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) prev[i] = __ldcg(rawT + static_cast<size_t>(gcol + h + i) * kTileM);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) v[h + i] = __float_as_uint(fmaf(__uint_as_float(v[h + i]), inv_scale, prev[i]));
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 32; ++i) __stcg(rawT + static_cast<size_t>(gcol + i) * kTileM, __uint_as_float(v[i]));
-      const int nv = last_seg ? max(0, min(32, N - gcol)) : 0;
-      if (is_ln && nv > 0) {
-        if (!have_x0) { x0 = __uint_as_float(v[0]); have_x0 = true; }
-        if (nv == 32) {
-          const float2 nx0 = f2s(-x0);
-#pragma unroll
-          for (int i4 = 0; i4 < 32; i4 += 4) {
-            const float2 da = __fadd2_rn(f2(__uint_as_float(v[i4]), __uint_as_float(v[i4 + 1])), nx0);
-            const float2 db = __fadd2_rn(f2(__uint_as_float(v[i4 + 2]), __uint_as_float(v[i4 + 3])), nx0);
-            sa = __fadd2_rn(sa, da); qa = __ffma2_rn(da, da, qa);
-            sbb = __fadd2_rn(sbb, db); qb = __ffma2_rn(db, db, qb);
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (i < nv) { const float d = __uint_as_float(v[i]) - x0; s += d; q = fmaf(d, d, q); }
-        }
-      }
-    }
-    if (sc + 1 < nsc || !last_seg) {
-      // TMEM may be overwritten by the next segment's / super-chunk's MMAs once every epilogue warp (of both CTAs of a
-      // pair) has read its part
-      ptx::tc_fence_before();
-      epi_bar_sync();
-      if (threadIdx.x == kEpiWarp0 * 32) {
-        if (c.cg2) ptx::mbar_arrive_leader(&c.acc_empty[0]);
-        else ptx::mbar_arrive(&c.acc_empty[0]);
-      }
-    }
-   }
-  }
-  if (!is_ln) {
-    // EPI_RAW (diagnostics): plain Linear output rows; every thread copies out the columns it drained itself
-    const int orow = ea.rowmap ? ea.rowmap[et.row] : et.row;
-    if (orow >= 0)
-      for (int sc = 0; sc < nsc; ++sc) {
-        const WideCols wc = wide_cols(ly, sc, et.grp);
-        for (int c0 = wc.cb; c0 < wc.cb + wc.ncols; ++c0) {
-          const int gcol = sc * kFusedMaxN + c0;
-          if (gcol < N) ea.out_f32[static_cast<size_t>(orow) * ea.out_pitch + gcol] = __ldcg(rawT + static_cast<size_t>(gcol) * kTileM);
-        }
-      }
-    return;
-  }
-  if (tr0) TDMPC2_TRACE(P, c, 5);                                   // every super-chunk drained
-  // ---- merge the 4 column groups' statistics (Chan), as in epi_ln_fused
-  s += (sa.x + sa.y) + (sbb.x + sbb.y);
-  q += (qa.x + qa.y) + (qb.x + qb.y);
-  int cnt_g[kEpiGroups];
-#pragma unroll
-  for (int g = 0; g < kEpiGroups; ++g) {
-    int n = 0;
-    for (int sc = 0; sc < nsc; ++sc) {
-      const WideCols wc = wide_cols(ly, sc, g);
-      n += max(0, min(wc.ncols, N - (sc * kFusedMaxN + wc.cb)));
-    }
-    cnt_g[g] = n;
-  }
-  {
-    const float n_g = static_cast<float>(cnt_g[et.grp]);
-    c.part[et.grp * kTileM + et.row] = cnt_g[et.grp] > 0 ? x0 + s / n_g : 0.f;                       // group mean
-    c.part[(kEpiGroups + et.grp) * kTileM + et.row] = cnt_g[et.grp] > 0 ? q - s * s / n_g : 0.f;     // group M2
-  }
-  // the raw scratch was written through the generic proxy; pass 2 fetches it with bulk copies (async proxy)
-  __threadfence();
-  ptx::fence_proxy_async_all();
-  epi_bar_sync();
-  float mean = 0.f, rstd;
-  {
-    float m2 = 0.f, cnt = 0.f;
-#pragma unroll
-    for (int g = 0; g < kEpiGroups; ++g) {
-      const float ng = static_cast<float>(cnt_g[g]);
-      if (ng > 0.f) {
-        const float mg = c.part[g * kTileM + et.row], m2g = c.part[(kEpiGroups + g) * kTileM + et.row];
-        const float tot = cnt + ng, delta = mg - mean;
-        mean += delta * (ng / tot);
-        m2 += m2g + delta * delta * (cnt * ng / tot);
-        cnt = tot;
-      }
-    }
-    rstd = rsqrtf(m2 / static_cast<float>(N) + 1e-5f);            // nn.LayerNorm eps (layers.py:101), biased variance
-  }
-  const float nmr = -mean * rstd;
-  if (tr0) TDMPC2_TRACE(P, c, 6);
-  const bool tma_out = ea.dstbuf >= 0 && !ea.out_f32 && (N % 32 == 0) && (ea.dst_col0 % 32 == 0);   // == run_layer's tma_only
-  if (tma_out) {
-    if (ea.kind == EPI_LN_MISH) wide_pass2_tma<EPI_LN_MISH>(P, c, et, ly, ea, rstd, nmr);
-    else wide_pass2_tma<EPI_LN_SIMNORM>(P, c, et, ly, ea, rstd, nmr);
-  } else {
-    if (ea.kind == EPI_LN_MISH) wide_pass2_general<EPI_LN_MISH>(P, c, et, ly, ea, rstd, nmr);
-    else wide_pass2_general<EPI_LN_SIMNORM>(P, c, et, ly, ea, rstd, nmr);
-  }
-  if (tr0) TDMPC2_TRACE(P, c, 8);                                   // normalise pass done, stores performed
-}
-
-// GEMM roles + epilogue of a wide layer; returns the number of accumulator hand-offs (= facc phases consumed).
-__device__ __forceinline__ int wide_layer_tc(const PlanParams& P, Ctx& c, const LayerRec& ly, int srcbuf, const EpiArgs& ea, int kc_begin) {
-  const int nnc_all = (ly.Npad + kNch - 1) / kNch;
-  const int nsc = (nnc_all + 1) / 2;
-  const int nkc = ly.Kpad / kKch - kc_begin;          // K-chunks [kc_begin, Kpad / 64): see PlanParams::zbias
-  const int kseg = (P.kseg > 0 && P.kseg < nkc) ? P.kseg : nkc;
-  const int nseg = (nkc + kseg - 1) / kseg;
-  if (c.warp == 0) {
-    for (int sc = 0; sc < nsc; ++sc)
-      for (int seg = 0; seg < nseg; ++seg) tc_producer(P, c, ly, srcbuf, nullptr, 2 * sc, 2, kc_begin + seg * kseg, kseg);
-  } else if (c.warp == 1) {
-    if (!c.cg2 || c.rank == 0)
-      for (int sc = 0; sc < nsc; ++sc)
-        for (int seg = 0; seg < nseg; ++seg) {
-          if (sc + seg > 0) {                           // the previous accumulator has been drained
-            const long long tw = prof_clock();
-            ptx::mbar_wait(&c.acc_empty[0], c.a_it & 1);
-            c.pf0 += prof_clock() - tw;
-            ++c.a_it;
-            ptx::tc_fence_after();
-          }
-          tc_mma(P, c, ly, 2 * sc, 2, kc_begin + seg * kseg, kseg);
-        }
-  } else if (c.warp >= kEpiWarp0) {
-    epi_wide(P, c, ly, ea, nsc, nseg);
-    ptx::tc_fence_before();
-  }
-  return nsc * nseg;
-}
-
 // Make generic-proxy global writes (activation planes) visible to the TMA unit
 // (async proxy) before the next layer's loads, and sync the CTA.
 __device__ __forceinline__ void publish_planes() {
@@ -1753,62 +598,29 @@ __device__ __forceinline__ void publish_planes() {
 
 // ------------------------------------------------------------------------------------ one layer
 // GEMM + epilogue; on return the epilogue's outputs are published (CTA-synchronised, TMA-visible).
-template <int ENGINE, bool EPISODIC, bool WIDE>
+template <int ENGINE, bool EPISODIC>
 __device__ __forceinline__ void run_layer(const PlanParams& P, Ctx& c, const LayerDev& ly_global, int srcbuf, const EpiArgs& ea,
-                                          const LayerDev* next, int kc0 = 0, const float* bias_override = nullptr, int next_kc0 = 0) {
+                                          int kc0 = 0, const float* bias_override = nullptr) {
   LayerRec ly = layer_rec(ly_global);                // registers: see LayerRec
   if (bias_override) ly.bias = bias_override;        // shared-latent fold: see PlanParams::zbias
   const bool is_ln = (ea.kind == EPI_LN_MISH || ea.kind == EPI_LN_SIMNORM);
-  const bool fused = (ENGINE == ENGINE_TC) && (ly.Npad <= kFusedMaxN) && (is_ln || ly.Npad <= kNch) &&
-                     (ea.kind != EPI_RAW || ly.Npad <= kNch);
-  if (fused) {
-    const long long tl = prof_clock();
-    if (threadIdx.x == 0) TDMPC2_TRACE(P, c, 0);
-    const int hseg = (WIDE && !is_ln && head_seg_ok(P, ea.kind)) ? head_segments(P, ly) : 1;   // K <= 512 unless the model is wide
-    if (c.warp == 0) {
-      tc_producer(P, c, ly, srcbuf, next, 0, 1 << 30, kc0, 1 << 30, next_kc0);
-    } else if (c.warp == 1) {
-      if (!c.cg2 || c.rank == 0) {
-        if (hseg > 1) tc_mma_head_seg(P, c, ly, hseg);
-        else tc_mma(P, c, ly, 0, 1 << 30, kc0);
-      }
-    } else if (c.warp >= kEpiWarp0) {
-      if (is_ln) epi_ln_fused(P, c, ly, ea);
-      else epi_head_fused<EPISODIC>(P, c, ly, ea, hseg);
-      ptx::tc_fence_before();
-    }
-    c.pf1 += prof_clock() - tl;
-    // every thread tracks the facc phases: buffer 0 completed ceil(hseg / 2) times, buffer 1 floor(hseg / 2) times
-    c.fph0 ^= static_cast<uint32_t>(((hseg + 1) >> 1) & 1);
-    c.fph1 ^= static_cast<uint32_t>((hseg >> 1) & 1);
-  } else if (ENGINE == ENGINE_TC && WIDE) {
-    // LayerNorm layers (and the diagnostic raw mode) wider than TMEM; heads are never wider than one N-chunk
-    const long long tl = prof_clock();
-    if (threadIdx.x == 0) TDMPC2_TRACE(P, c, 0);
-    const int nph = wide_layer_tc(P, c, ly, srcbuf, ea, kc0);
-    c.pf1 += prof_clock() - tl;
-    c.fph0 ^= static_cast<uint32_t>(nph & 1);         // one facc phase per (super-chunk, K-segment)
-  } else if (ENGINE == ENGINE_SIMT) {
-    gemm_simt(P, c, ly, srcbuf, kc0);
-    if (is_ln) rows_ln_act(P, c, ly, ea);
-    else rows_head<EPISODIC>(P, c, ly, ea);
-  }                                                   // (a tcgen05 kernel without WIDE is never launched on a model with wide layers)
+  const long long tl = prof_clock();
+  if (threadIdx.x == 0) TDMPC2_TRACE(P, c, 0);
+  if (ENGINE == ENGINE_TC) gemm_tc(P, c, ly, srcbuf, kc0);
+  else gemm_simt(P, c, ly, srcbuf, kc0);
+  if (threadIdx.x == 0) TDMPC2_TRACE(P, c, 3);
+  if (is_ln) rows_ln_act(P, c, ly, ea);
+  else rows_head<EPISODIC>(P, c, ly, ea);
+  c.pf1 += prof_clock() - tl;
   const long long tp = prof_clock();
-  // LN layers that went out through TMA stores wrote nothing through the generic proxy: the leaders have
-  // waited for their bulk groups, so a CTA barrier is all the next layer's TMA loads need.
-  const bool tma_only = (ENGINE == ENGINE_TC) && is_ln && ea.dstbuf >= 0 && (ly.N % 32 == 0) && (ea.dst_col0 % 32 == 0) && !ea.out_f32;
-  if (tma_only) __syncthreads();
-  else publish_planes();
+  publish_planes();
   c.pf3 += prof_clock() - tp;
-  if (threadIdx.x == 64 && ENGINE == ENGINE_TC) TDMPC2_TRACE(P, c, 9);
-  if (ENGINE == ENGINE_TC) ptx::tc_fence_after();
 }
 
 // ------------------------------------------------------------------------------------ top-k + MPPI refit
 // Runs in the LAST CTA to finish a tile of environment e (tdmpc2.py:184-197).
-// Thread groups that can run the CTA-wide glue phases: the whole CTA (bar 0) or only the 16 epilogue warps (bar 1).
+// The thread group that runs the CTA-wide glue phases: the whole CTA (bar 0).
 struct GroupAll { static constexpr int N = kThreads; __device__ static int tid() { return threadIdx.x; } __device__ static void sync() { __syncthreads(); } };
-struct GroupEpi { static constexpr int N = kEpiThreads; __device__ static int tid() { return threadIdx.x - kEpiWarp0 * 32; } __device__ static void sync() { epi_bar_sync(); } };
 
 template <class G>
 __device__ __forceinline__ void refit_env(const PlanParams& P, uint8_t* scratch, size_t scratch_bytes, int e, int task) {
@@ -1907,16 +719,9 @@ __device__ __forceinline__ void refit_env(const PlanParams& P, uint8_t* scratch,
 }
 
 // ------------------------------------------------------------------------------------ the kernel
-// CG2: CTA pairs (cluster of 2) run the GEMMs as tcgen05 cta_group::2 MMAs (M = 256: 128 rows of each CTA's own
-// tile; each CTA streams only half of every weight tile).  Only MODE_ITER with an even number of tiles per
-// environment and every layer on the fused path is launched this way.
 // EPISODIC (cfg.episodic, single-task models): every rollout step gains the 3-layer termination head on z_{t+1}
 // and the value bookkeeping its sticky (1 - termination) factor (tdmpc2.py:126-136); compiled out otherwise.
-// WIDE: the model has layers wider than the 512 TMEM columns (48M / 317M presets): adds the super-chunked wide-layer path and
-// the K-segmented heads; compiled out of the kernels the 5M preset runs (their register allocation is untouched by it).
-// WPF (CEM iterations of fully fused models): the TMA producer prefetches the next layer's first weight chunks into
-// the W ring while the epilogue runs; the epilogue stages its output in the A ring instead.  Same arithmetic.
-template <int ENGINE, bool CG2 = false, bool EPISODIC = false, bool WPF = false, bool WIDE = false>
+template <int ENGINE, bool EPISODIC = false>
 __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant__ PlanParams P) {
   constexpr int SPT = EPISODIC ? 9 : 6;      // layer steps per rollout time step (ITER / VALUE)
   extern __shared__ uint8_t smem_raw[];
@@ -1924,84 +729,41 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
   {
     // The operand tiles need 1024-byte alignment (128-byte swizzle atoms).  The kernel has no static shared memory, so
     // the dynamic window starts right after the 1 KiB the system reserves per CTA: it IS 1024-aligned, which is checked
-    // here instead of being fixed up -- every smem pointer below is then the array symbol plus a compile-time constant
-    // (no register, nothing to spill; the round-up through uintptr_t used before cost a 64-bit base that ptxas spilled
-    // and reloaded at ~100 sites).
-    if ((ptx::smem_u32(smem_raw) & 1023u) != 0u) {
-      if (threadIdx.x == 0) printf("tdmpc2_b200: dynamic shared memory is not 1024-byte aligned (0x%x)\n", ptx::smem_u32(smem_raw));
-      __trap();
-    }
+    // here instead of being fixed up -- every smem pointer below is then the array symbol plus a compile-time constant.
+    if ((ptx::smem_u32(smem_raw) & 1023u) != 0u) __trap();   // (no printf: see ptx::mbar_wait)
     c.stage_base = smem_raw;
     uint8_t* ctrl = c.stage_base + kStages * kStageBytes;
-    c.a_full = reinterpret_cast<uint64_t*>(ctrl);
-    c.a_empty = c.a_full + kARing;
-    c.w_full = c.a_empty + kARing;
-    c.w_empty = c.w_full + kWRingPair;
-    c.acc_full = c.w_empty + kWRingPair;
-    c.acc_empty = c.acc_full + 2;
-    c.facc = c.acc_empty + 2;
-    c.tmem_ptr = reinterpret_cast<uint32_t*>(c.facc + 2);
-    c.flags = reinterpret_cast<int*>(c.tmem_ptr + 1);          // [8]
-    c.rawb = reinterpret_cast<uint64_t*>(ctrl + 184);           // [8]  (ends at ctrl + 248)
-    c.G = reinterpret_cast<float*>(ctrl + 256);                 // [128]  (18 mbarriers + tmem ptr + flags live below 256)
+    c.g_full = reinterpret_cast<uint64_t*>(ctrl);
+    c.g_empty = c.g_full + kGStages;
+    c.flags = reinterpret_cast<int*>(c.g_empty + kGStages);     // [8]  (ends at ctrl + 80)
+    c.G = reinterpret_cast<float*>(ctrl + 256);                 // [128]
     c.q1 = c.G + kTileM;                                        // [128]  (ends at ctrl + 1280)
     c.term = c.q1 + kTileM;                                     // [128]  (ends at ctrl + 1792 <= kSmemCtrl)
     c.rowbuf = reinterpret_cast<float*>(ctrl + kSmemCtrl);
     c.rowenv = reinterpret_cast<int*>(ctrl + kSmemCtrl + kSmemRowBuf);
-    c.vec = reinterpret_cast<float*>(ctrl + kSmemCtrl + kSmemRowBuf + kSmemRowEnv);
-    c.part = c.vec + 3 * kFusedMaxN;
   }
   c.slot = blockIdx.x;
-  c.cg2 = CG2 ? 1 : 0;
-  c.wpf = WPF ? 1 : 0;
-  c.w_pref = 0;
-  c.w_ring = CG2 ? kWRingPair : kWRing;
-  c.w_stride = CG2 ? kWSlotBytes / 2 : kWSlotBytes;
-  c.w_lo_off = CG2 ? kAPlane : kWPlane;
-  c.rank = CG2 ? static_cast<int>(ptx::cluster_ctarank()) : 0;
   c.warp = threadIdx.x >> 5;
   c.lane = threadIdx.x & 31;
-  c.pa_it = c.pw_it = c.ma_it = c.mw_it = c.a_it = c.d_it = 0;
-  c.fph0 = c.fph1 = 0;
-  c.rb_it = 0;
+  c.pa_it = c.ma_it = 0;
   c.pf0 = c.pf1 = c.pf2 = c.pf3 = c.pf4 = c.pf5 = c.pf6 = c.pf7 = 0;
   c.trace_step = 1 << 30;
   const long long t_kernel0 = prof_clock();
-  c.tmem_base = 0;
   int* rowenv = c.rowenv;
 
   if (ENGINE == ENGINE_TC) {
     if (threadIdx.x == 0) {
-      for (int s = 0; s < kARing; ++s) { ptx::mbar_init(&c.a_full[s], 1); ptx::mbar_init(&c.a_empty[s], 1); }
-      for (int s = 0; s < kWRingPair; ++s) { ptx::mbar_init(&c.w_full[s], 1); ptx::mbar_init(&c.w_empty[s], 1); }
-      for (int s = 0; s < 2; ++s) {
-        ptx::mbar_init(&c.acc_full[s], 1);
-        ptx::mbar_init(&c.acc_empty[s], CG2 ? 2 : 1);   // wide layers: one arrival per CTA of the pair (its drain is done)
-        ptx::mbar_init(&c.facc[s], 1);
-      }
-      for (int s = 0; s < 2 * kEpiGroups; ++s) ptx::mbar_init(&c.rawb[s], 1);
+      for (int s = 0; s < kGStages; ++s) { ptx::mbar_init(&c.g_full[s], 1); ptx::mbar_init(&c.g_empty[s], 4 * kGWarpGroups); }
       ptx::fence_barrier_init();
       ptx::prefetch_tensormap(&P.tmX);
       ptx::prefetch_tensormap(&P.tmH);
     }
-    if (CG2) ptx::cluster_sync();          // the peer's barriers are initialised before anything can signal them
-    if (c.warp == 1) { if (CG2) ptx::tmem_alloc_2sm(c.tmem_ptr, 512); else ptx::tmem_alloc(c.tmem_ptr, 512); }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    c.tmem_base = *c.tmem_ptr;
   }
 
   const LayerDev* LY = P.layers;
 
-  if (P.stagger != 0u && P.mode == MODE_ITER && ((static_cast<unsigned>(blockIdx.x) >> (CG2 ? 1 : 0)) & 1u)) {
-    const long long t_start = clock64();
-    while (clock64() - t_start < static_cast<long long>(P.stagger)) __nanosleep(500);
-  }
-
-  // pair mode: the two CTAs of a pair take tiles (2p, 2p+1) and run the same number of loop trips
-  for (int tile = CG2 ? 2 * (static_cast<int>(blockIdx.x) >> 1) + c.rank : static_cast<int>(blockIdx.x); tile < P.ntiles;
-       tile += gridDim.x) {
+  for (int tile = static_cast<int>(blockIdx.x); tile < P.ntiles; tile += gridDim.x) {
     // ---------------- tile set-up: fill the input planes of X ----------------
     const long long t_setup = prof_clock();
     for (int r = threadIdx.x; r < kTileM; r += kThreads) {
@@ -2248,21 +1010,7 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
         }
       }
       c.trace_step = (tile == static_cast<int>(blockIdx.x)) ? sidx : (1 << 30);
-      const LayerDev* next = nullptr;
-      int next_kc0 = 0;
-      if (WPF && P.mode == MODE_ITER && sidx + 1 < nsteps) {
-        // layer of the step after this one (same mapping as above, without its side effects); none after the
-        // tile's last step: the refit and the next tile's set-up use the operand smem as scratch
-        const int s1 = sidx + 1;
-        int mlp1, l1;
-        if (s1 < SPT * P.H) { l1 = s1 % SPT; mlp1 = l1 < 3 ? 0 : ((EPISODIC && l1 >= 6) ? 5 : 1); l1 %= 3; }
-        else { const int u1 = s1 - SPT * P.H; mlp1 = 2 + u1 / 3; l1 = u1 % 3; }
-        const int base1 = (EPISODIC && mlp1 == 5) ? P.li_term
-                          : mlp1 == 0 ? P.li_rew : mlp1 == 1 ? P.li_dyn : mlp1 == 2 ? P.li_pi : P.li_q + 3 * qi[mlp1 - 3];
-        next = &LY[base1 + l1];
-        if (P.zb_kc0 > 0 && s1 < SPT && l1 == 0 && mlp1 <= 1) next_kc0 = P.zb_kc0;   // the step after this one is a folded t = 0 layer
-      }
-      run_layer<ENGINE, EPISODIC, WIDE>(P, c, LY[li], src, ea, next, kc0, bias_ov, next_kc0);
+      run_layer<ENGINE, EPISODIC>(P, c, LY[li], src, ea, kc0, bias_ov);
     }
 
     const long long t_refit = prof_clock();
@@ -2286,21 +1034,17 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
   }
 
   if (kProf && P.prof) {
-    // rows: 0 producer (warp 0 lane 0), 1 MMA issuer (warp 1 lane 0), 2 epilogue thread (warp 4 lane 0), 3 idle warp 2
-    // cols: 0 barrier-wait cycles (empty | full), 1 cycles inside fused layers, 2 facc wait, 3 publish, 5 whole kernel
-    const int who = (threadIdx.x == 0) ? 0 : (threadIdx.x == 32) ? 1 : (threadIdx.x == kEpiWarp0 * 32) ? 2
-                    : (threadIdx.x == 64) ? 3 : -1;
+    // rows: 0 TMA producer (warp 16 lane 0), 1 consumer warpgroup 0 (thread 0), 2 consumer warpgroup 3 (thread 384),
+    //       3 idle warp 17 during the GEMM
+    // cols: 0 stage-empty wait cycles, 1 cycles inside layers, 2 stage-full wait, 3 publish, 4 tile set-up, 5 whole kernel,
+    //       6 action pass, 7 refit
+    const int who = (threadIdx.x == kGProducerWarp * 32) ? 0 : (threadIdx.x == 0) ? 1 : (threadIdx.x == 384) ? 2
+                    : (threadIdx.x == (kGProducerWarp + 1) * 32) ? 3 : -1;
     if (who >= 0) {
       long long* o = P.prof + (static_cast<size_t>(blockIdx.x) * 4 + who) * 12;
       o[0] = c.pf0; o[1] = c.pf1; o[2] = c.pf2; o[3] = c.pf3; o[4] = c.pf4; o[5] = prof_clock() - t_kernel0;
       o[6] = c.pf5; o[7] = c.pf6; o[8] = c.pf7;
     }
-  }
-  if (ENGINE == ENGINE_TC) {
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (CG2) ptx::cluster_sync();          // neither CTA may retire while the pair's MMAs / barriers are in use
-    if (c.warp == 1) { if (CG2) ptx::tmem_dealloc_2sm(c.tmem_base, 512); else ptx::tmem_dealloc(c.tmem_base, 512); }
   }
 }
 

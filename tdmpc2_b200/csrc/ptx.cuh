@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / fences) and descriptor builders.
-// Hand-written for this project; encodings follow the PTX ISA for sm_100a.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor),
+// wgmma (warpgroup MMA from shared-memory descriptors) and descriptor builders.
+// Hand-written for this project; encodings follow the PTX ISA for sm_90a.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -46,78 +46,19 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Non-blocking probe (try_wait may suspend the thread for a system-dependent time before it reports failure; loops that
-// watch two barriers at once must not sit out that time on the first one).
-__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, P1;\n\t}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Bounded spin: a protocol bug must trap (-> CUDA error on the host) instead of
-// hanging the GPU box.  ~2^28 polls is seconds; real waits are microseconds.
+// Bounded spin: a protocol bug must trap (-> CUDA error on the host) instead of hanging the device.  ~2^28 polls is
+// seconds; real waits are microseconds.  No printf here: a function call inside the kernel makes ptxas serialise every
+// wgmma (C7510), so the wait path stays call-free.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 28)) {
-      printf("tdmpc2_b200: mbarrier wait timed out (block %d thread %d bar %p parity %u)\n", (int)blockIdx.x,
-             (int)threadIdx.x, (void*)bar, parity);
-      __trap();
-    }
+    if (++spins > (1u << 28)) __trap();
   }
 }
-// Long waits of many warps (the 16 epilogue warps wait ~28 k cycles per layer for the accumulator): TDMPC2_EPI_SLEEP_NS
-// > 0 puts a nanosleep between polls -- fewer issue slots and less power under the 1000 W cap, at the price of a
-// slower wake-up.  Experiment knob for an A/B build (build.build_variant); 0 = plain mbar_wait.
-#ifndef TDMPC2_EPI_SLEEP_NS
-#define TDMPC2_EPI_SLEEP_NS 0
-#endif
-__device__ __forceinline__ void mbar_wait_long(uint64_t* bar, uint32_t parity) {
-#if TDMPC2_EPI_SLEEP_NS > 0
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    __nanosleep(TDMPC2_EPI_SLEEP_NS);
-    if (++spins > (1u << 24)) {
-      printf("tdmpc2_b200: mbarrier wait timed out (block %d thread %d bar %p parity %u)\n", (int)blockIdx.x,
-             (int)threadIdx.x, (void*)bar, parity);
-      __trap();
-    }
-  }
-#else
-  mbar_wait(bar, parity);
-#endif
-}
-
-// Run-time variant: `ns` > 0 sleeps between polls (a wide layer's GEMM keeps 16 epilogue warps waiting for 50 - 100 us;
-// spinning costs issue slots and power under the 1 kW cap).
-__device__ __forceinline__ void mbar_wait_sleep(uint64_t* bar, uint32_t parity, uint32_t ns) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if (ns) __nanosleep(ns);
-    if (++spins > (1u << 28)) {
-      printf("tdmpc2_b200: mbarrier wait timed out (block %d thread %d bar %p parity %u)\n", (int)blockIdx.x,
-             (int)threadIdx.x, (void*)bar, parity);
-      __trap();
-    }
-  }
-}
-
 // ------------------------------------------------------------------ proxies / fences
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;\n" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
 
 // ------------------------------------------------------------------ TMA
-// L2 cache-hint operands of cp.async.bulk.tensor (the encodings createpolicy.fractional.L2::evict_* returns for fraction 1.0)
-constexpr uint64_t kL2EvictNormal = 0x1000000000000000ull, kL2EvictFirst = 0x12F0000000000000ull, kL2EvictLast = 0x14F0000000000000ull;
 __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];\n" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
 }
@@ -131,14 +72,6 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar,
       : "memory");
 }
 
-// Contiguous bulk copy global -> shared (bytes % 16 == 0, both addresses 16-byte aligned), mbarrier completion.
-__device__ __forceinline__ void bulk_load(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
-                   smem_u32(smem_dst)),
-               "l"(reinterpret_cast<uint64_t>(gmem_src)), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-
 // Bulk prefetch of a contiguous global range into L2 (no completion tracking): the 16-byte-aligned part of [p, p + bytes).
 __device__ __forceinline__ void bulk_prefetch_l2(const void* p, size_t bytes) {
   const uint64_t a = reinterpret_cast<uint64_t>(p), a0 = (a + 15ull) & ~15ull, a1 = (a + bytes) & ~15ull;
@@ -146,162 +79,40 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void* p, size_t bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;\n" ::"l"(a0), "r"(static_cast<uint32_t>(a1 - a0)) : "memory");
 }
 
-// 2D tile store shared -> global (bulk async group).
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-// The same with an L2 cache-hint operand (kL2Evict*, below): the activation planes are re-read by the very next layer.
-__device__ __forceinline__ void tma_store_2d_hint(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1, uint64_t policy) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;\n" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "l"(policy)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() {   // at most N groups still reading their smem source
-  asm volatile("cp.async.bulk.wait_group.read %0;\n" ::"n"(N) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void bulk_wait() {        // at most N groups not yet complete (writes performed)
-  asm volatile("cp.async.bulk.wait_group %0;\n" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void st_shared_v4(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};\n" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-
-// ------------------------------------------------------------------ CTA pairs (cluster of 2, tcgen05 cta_group::2)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-}
-// Clearing this bit of a shared::cluster address selects the even (leader) CTA of the pair.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-// 2D tile load into THIS CTA's smem whose transaction bytes are counted on the LEADER CTA's mbarrier.
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* m, uint64_t* bar, void* smem_dst, int32_t c0,
-                                                int32_t c1, uint64_t policy = kL2EvictNormal) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "l"(policy)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {  // whole warp, both CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[256 rows: 128 from each CTA's smem] * B[N rows: N/2 from each CTA's smem]^T
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on the mbarrier at this smem offset in BOTH CTAs when all previously issued pair-MMAs complete.
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  const uint16_t mask = 3;
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-
-// Arrive on the barrier at this smem offset in the LEADER CTA (rank 0) of the pair; release at cluster scope.
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  uint32_t raddr;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(raddr) : "r"(smem_u32(bar)), "r"(0));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(raddr) : "memory");
-}
-
-// ------------------------------------------------------------------ tcgen05: TMEM alloc
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ------------------------------------------------------------------ tcgen05: descriptors
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle, tile rows
-// of 64 fp16 (128 B), 8-row swizzle atoms 1024 B apart (SBO), version 1 (sm_100).
-//   bits [0,14)  start address >> 4      bits [16,30) LBO >> 4 (ignored for swizzled K-major; 1)
-//   bits [32,46) SBO >> 4                bits [46,48) version = 1
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
+// ------------------------------------------------------------------ wgmma
+// Shared-memory matrix descriptor (sm_90 wgmma), K-major operand, 128-byte swizzle, tile rows of 64 fp16 (128 B),
+// 8-row swizzle atoms 1024 B apart (SBO):
+//   bits [0,14)  start address >> 4      bits [16,30) LBO >> 4 (unused for swizzled K-major; 1)
+//   bits [32,46) SBO >> 4                bits [62,64) layout type: 1 = SWIZZLE_128B
+// A K-step of 16 elements inside the 128-byte row advances the start address by 32 bytes.
 __device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Instruction descriptor, kind::f16: A,B fp16 (format 0), D fp32, both K-major.
-//   [4,6) c_format=1(F32)  [7,10) a_format  [10,13) b_format  [15] a_major  [16] b_major
-//   [17,23) N>>3           [24,29) M>>4
-__host__ __device__ __forceinline__ uint32_t make_idesc_f16(uint32_t M, uint32_t N) {
-  uint32_t d = 0;
-  d |= 1u << 4;
-  d |= (N >> 3) << 17;
-  d |= (M >> 4) << 24;
-  return d;
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; single issuing thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
+// D[64 x 64, fp32 registers of the warpgroup] += A[64 x 16, smem] * B[64 x 16, smem]^T, fp16 operands, both K-major.
+// Thread t of the warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and columns 8 j + 2 (t % 4) (+ 1):
+// d[4 j + 0 | 1] = row r, d[4 j + 2 | 3] = row r + 8.
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued MMAs of this thread complete.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// ------------------------------------------------------------------ tcgen05: TMEM -> registers
-// 32 lanes x 32 consecutive 32-bit columns; thread i of the warp gets lane (base+i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc));
 }
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
 
 }  // namespace ptx

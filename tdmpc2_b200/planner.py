@@ -1,6 +1,6 @@
-"""Python host of the fused B200 planner: owns the device buffers (torch tensors)
+"""Python host of the fused H100 planner: owns the device buffers (torch tensors)
 and drives the C ABI (include/tdmpc2_b200.h).  torch is plumbing here -- device
-memory, streams, RNG -- the planning math runs in the sm_100a kernels.
+memory, streams, RNG -- the planning math runs in the sm_90a kernels.
 
 Call sequence of one `plan()` (reference tdmpc2.py:138-206):
     prologue  -> encode, policy-prior trajectories, mean/std init
@@ -21,16 +21,11 @@ from . import _cabi
 from .config import Config, get_discount
 
 
-# GEMM engine of the CEM-iteration kernel (include/tdmpc2_b200.h, tdmpc2_engine).  "tcgen05pp" falls back to
-# "tcgen05x2" and that to "tcgen05" inside the library when a model / shape does not fit; TDMPC2_B200_ENGINE overrides.
-# "auto": batches that fit one trip of the persistent grid (tiles <= SMs: latency-bound, e.g. the reference's one environment per
-# act()) take the ping-pong engine, which needs 23 % fewer cycles per iteration; larger batches run at the board's power cap, where
-# the busier kernel is simply clocked lower and the CTA-pair engine's smaller operand traffic makes it the faster one by a few
-# per cent (profiles/README.md, "The c2 kernel is power-bound now").
+# GEMM engine of the CEM-iteration kernel (include/tdmpc2_b200.h, tdmpc2_engine); TDMPC2_B200_ENGINE overrides.  On sm_90a
+# "tcgen05pp", "tcgen05x2" and "tcgen05x2pf" run as "tcgen05" (the TMA + wgmma engine); "auto" picks among those names.
 DEFAULT_ENGINE = os.environ.get("TDMPC2_B200_ENGINE", "auto")
-# Wide layers (48M / 317M presets): elements of the reduction dimension accumulated in TMEM before the partial sum is
-# flushed and added in fp32 round-to-nearest.  2048 keeps the 317M preset (K = 4096) inside the parity tolerance
-# (5e-5 + 1e-5 |v|) at +6 % time; 1024 halves the error again at +20 %; 0 = one accumulation (fastest, 2.8e-4 on |v| ~ 16).
+# Reduction-segment knob of the C ABI (tdmpc2_planner_set_kseg); the wgmma engine adds every 64-element K-chunk with
+# round-to-nearest, so the value has no effect on this build.
 DEFAULT_KSEG = 2048
 
 
@@ -172,7 +167,7 @@ class Planner:
         self.cfg, self.E = cfg, int(num_envs)
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise _cabi.CabiError("the B200 planner needs a CUDA device; there is no CPU fallback")
+            raise _cabi.CabiError("the H100 planner needs a CUDA device; there is no CPU fallback")
         self.rgb = cfg.get("obs", "state") == "rgb"
         d = _cabi.Dims(
             num_envs=self.E, num_samples=cfg.num_samples, num_pi_trajs=cfg.num_pi_trajs, num_elites=cfg.num_elites,
@@ -216,7 +211,7 @@ class Planner:
         if self.l2_persist:
             with torch.cuda.device(self.device):
                 _cabi.check(self.lib.tdmpc2_planner_set_l2_persist(self.h, 1))
-        # wide presets: K elements accumulated in TMEM per segment (see include/tdmpc2_b200.h, tdmpc2_planner_set_kseg)
+        # reduction-segment knob (see include/tdmpc2_b200.h, tdmpc2_planner_set_kseg)
         self.kseg = int(os.environ.get("TDMPC2_B200_KSEG", cfg.get("kseg", DEFAULT_KSEG)))
         _cabi.check(self.lib.tdmpc2_planner_set_kseg(self.h, self.kseg))
         if "TDMPC2_B200_HEAD_KSEG" in os.environ or cfg.get("head_kseg", None) is not None:

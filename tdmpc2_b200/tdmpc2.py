@@ -1,4 +1,4 @@
-"""TDMPC2 agent with the reference's inference surface, planning on the B200 kernels.
+"""TDMPC2 agent with the reference's inference surface, planning on the H100 kernels.
 
 Drop-in for the inference half of the reference class `TDMPC2`
 (tdmpc2/tdmpc2.py:10-206): `TDMPC2(cfg)`, `.model`, `.cfg`, `.device`,

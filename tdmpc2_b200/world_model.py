@@ -3,7 +3,7 @@
 The planner's kernels read the weights straight from `state_dict()` (tdmpc2_b200/planner.py packs them into the
 kernel layout), so this class holds tensors, not a module tree: there are no eager forward methods here -- every
 forward of the planning path (encode / next / reward / pi / Q / termination, reference common/world_model.py:103-216)
-runs in the fused sm_100a kernels, including the non-MPC `act()` branch (TDMPC2.act -> the policy-prior kernel mode).
+runs in the fused sm_90a kernels, including the non-MPC `act()` branch (TDMPC2.act -> the policy-prior kernel mode).
 
 What is kept, because reference checkpoints and `evaluate.py` depend on it (SURVEY.md section 8(b)):
 
@@ -82,7 +82,7 @@ class WorldModel(nn.Module):
         return sum(p.numel() for p in self.parameters() if p.requires_grad)
 
     def __repr__(self):
-        return f"TD-MPC2 World Model (B200 planner build, flat parameter container)\nLearnable parameters: {self.total_params:,}"
+        return f"TD-MPC2 World Model (H100 planner build, flat parameter container)\nLearnable parameters: {self.total_params:,}"
 
     # ------------------------------------------------------------------ (de)serialisation with the reference's keys
     def _save_to_state_dict(self, destination, prefix, keep_vars):

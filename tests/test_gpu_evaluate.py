@@ -1,5 +1,5 @@
 """The vectorised evaluation loop driving the real planner: E toy environments in lock-step, one batched act() per step
-(CUDA-graph replay), slots out of phase with per-slot t0.  Run on the B200 box: pytest -m gpu."""
+(CUDA-graph replay), slots out of phase with per-slot t0.  Run on an H100: pytest -m gpu."""
 from collections import defaultdict
 
 import pytest

@@ -1,7 +1,7 @@
 """The DECLARED NON-PARITY fast mode (tdmpc2_planner_set_passes(p, 1): one fp16 MMA per product instead of the three of
 the fp32-parity path).  It is not held to the oracle's 5e-5: these tests pin down what it IS -- the same plan with
 fp16-rounded operands (values within ~1e-2 of the oracle, far outside 5e-5, elite sets mostly but not exactly the
-reference's) -- and that switching it on does not disturb the parity mode.  Run on the B200 box: pytest -m gpu."""
+reference's) -- and that switching it on does not disturb the parity mode.  Run on an H100: pytest -m gpu."""
 import pytest
 import torch
 

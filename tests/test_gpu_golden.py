@@ -1,6 +1,6 @@
 """The fused kernels, driven through the reference-shaped agent API (TDMPC2._plan), against the
 golden vectors minted from the REFERENCE's own unmodified `_plan` (oracle/make_golden.py).
-E == 1, every model preset of BASELINE.json.  Run on the B200 box: pytest -m gpu."""
+E == 1, every model preset of BASELINE.json.  Run on an H100: pytest -m gpu."""
 import pytest
 import torch
 

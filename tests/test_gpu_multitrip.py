@@ -1,14 +1,14 @@
 """Parity in the regime bench.py times: more tiles than persistent CTAs, so that every CTA runs SEVERAL trips of the tile
 loop -- mbarrier phases / pipeline counters carried across tiles, operand smem reused as refit scratch between tiles,
-the cross-CTA "last tile of this environment" hand-off with tiles of one environment finishing in different trips, CTA
-pairs desynchronised by refits.  Checked two ways:
+the cross-CTA "last tile of this environment" hand-off with tiles of one environment finishing in different trips, CTAs
+desynchronised by refits.  Checked two ways:
 
   * bit-identity: a row's arithmetic does not depend on which CTA / trip / batch it runs in, so every environment of a
     big batch must reproduce, bit for bit, a 2-environment run of the same inputs and noise (single trip);
   * the CPU oracle on sampled environments of the big batch (same tolerances as tests/test_gpu_parity.py).
 
 Also: the c5 planner shape (N=1024, H=8, I=10 -> 8 tiles per environment, 57 layer steps per tile) on a 5M-sized model,
-and the 48M / 317M presets (wide layers) at E > 1.  Run on the B200 box: pytest -m gpu."""
+and the 48M / 317M presets (wide layers) at E > 1.  Run on an H100: pytest -m gpu."""
 import pytest
 import torch
 
@@ -49,11 +49,11 @@ def _two_plans(pl, obs, task, t0, prev, nz_a, nz_b):
     return (a1, m1, tr1), (a2, m2, tr2)
 
 
-@pytest.mark.parametrize("engine", ["tcgen05x2", "tcgen05pp"])
+@pytest.mark.parametrize("engine", ["tcgen05", "simt"])
 @pytest.mark.parametrize("E", [64, 256])
 def test_many_trip_batch_is_bit_identical_to_small_runs_and_matches_oracle(E, engine):
-    """c1 model (the bench's 5M dog-run net) on the CTA-pair engine and on the ping-pong engine (the default for this
-    model): E=64 -> 256 tiles (1.7 trips/CTA), E=256 -> 1024 tiles (6.9 trips/CTA; exactly bench.py's c2 schedule)."""
+    """c1 model (the bench's 5M dog-run net) on the tensor-core engine (the default) and on the CUDA-core engine:
+    E=64 -> 256 tiles (1.9 trips/CTA on 132 SMs), E=256 -> 1024 tiles (7.8 trips/CTA; exactly bench.py's c2 schedule)."""
     from oracle.plan_oracle import plan_oracle
     cfg = workload("c1", num_envs=E)
     assert E * ((cfg.num_samples + 127) // 128) > _num_sms()
@@ -93,8 +93,9 @@ def test_many_trip_batch_is_bit_identical_to_small_runs_and_matches_oracle(E, en
 
 def test_c5_planner_shape_on_5m_model():
     """N=1024, H=8, I=10 (BASELINE config c5's planner shape): 8 tiles per environment, 57 layer steps per tile, 20
-    environments -> 160 tiles > 148 CTAs.  Pair engine vs the oracle on 2 environments, and bit-identical to the
-    single-CTA engine on all of them."""
+    environments -> 160 tiles > 132 CTAs.  Tensor-core engine vs the oracle on 2 environments, and its first-iteration
+    trajectory values within the parity tolerance of the CUDA-core engine on all of them (the first iteration's inputs do
+    not depend on either engine's refit)."""
     from oracle.plan_oracle import plan_oracle
     E = 20
     cfg = workload("c1", num_envs=E, num_samples=1024, horizon=8, iterations=10)
@@ -104,27 +105,26 @@ def test_c5_planner_shape_on_5m_model():
     oracle_envs = [3, E - 1]
     nz, on = mixed_noise(cfg, E, oracle_envs, 300)
     out = {}
-    for engine in ("tcgen05x2", "tcgen05"):
+    for engine in ("simt", "tcgen05"):
         pl = _planner(cfg, E, engine, sd)
         a, m, tr = pl.plan(obs.cuda(), None, t0.cuda(), prev.cuda(), nz, trace=True)
         torch.cuda.synchronize()
         out[engine] = (a, m, tr)
         del pl
-    for name in ("values", "elite_idx", "iter_mean", "iter_std"):
-        assert torch.equal(out["tcgen05x2"][2][name], out["tcgen05"][2][name]), name
-    assert torch.equal(out["tcgen05x2"][0], out["tcgen05"][0])
+    v_tc, v_simt = out["tcgen05"][2]["values"][:, 0].cpu(), out["simt"][2]["values"][:, 0].cpu()
+    assert torch.allclose(v_tc, v_simt, atol=5e-5, rtol=1e-5), (v_tc - v_simt).abs().max()
     sel = torch.tensor(oracle_envs)
     want = plan_oracle(cfg, sd, obs[sel], t0=[bool(t0[e]) for e in oracle_envs], prev_mean=prev[sel], noise=on)
-    a, m, tr = out["tcgen05x2"]
+    a, m, tr = out["tcgen05"]
     n = compare_with_oracle(cfg, tr, a, m, want, on, oracle_envs)
     assert n["topk"] > 0 and n["refit"] > 0, n
     print(f"[c5-shape] {n}")
 
 
 # The wide presets keep the tolerance of every other parity test (values: 5e-5 + 1e-5 |v|; their values reach 8 / 17).
-# What makes that possible on tensor cores: tcgen05's fp32 accumulate step rounds toward zero, a drift that grows with
-# the reduction length (K = 1792 / 4096 here); the heads' and the wide layers' partial sums are therefore handed off
-# every 512 / 1024 elements of K and added with round-to-nearest (planner.DEFAULT_KSEG, tdmpc2_planner_set_head_kseg).
+# What makes that possible on tensor cores: the tensor core's internal accumulation is not round-to-nearest, a drift that
+# would grow with the reduction length (K = 1792 / 4096 here); every 64-element K-chunk's partial sum is therefore added
+# in fp32 with round-to-nearest (gemm_tc in plan_kernels.cuh).
 @pytest.mark.parametrize("wl", ["c3", "c4"])
 def test_wide_presets_multi_env(wl):
     """humanoid-walk 48M (M=1792) and mt80 317M (M=4096, multi-task) at E=3: 12 tiles on the wide-layer path, one

@@ -1,7 +1,7 @@
 """Pixel observations (cfg.obs == 'rgb'): the conv encoder kernel (ShiftAug + PixelPreprocess + 4 x Conv2d + SimNorm,
 reference common/layers.py:36-71,136-150) and the planner behind it, against the CPU oracle, whose pixel path is pinned to
 a fixture minted from the reference's own `_plan` on pixel observations (tests/golden/tiny_rgb.npz; the full-plan golden
-comparison is tests/test_gpu_golden.py::tiny_rgb).  Run on the B200 box: pytest -m gpu."""
+comparison is tests/test_gpu_golden.py::tiny_rgb).  Run on an H100: pytest -m gpu."""
 import pytest
 import torch
 

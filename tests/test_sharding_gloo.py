@@ -1,5 +1,5 @@
 """N > 1 path on CPU: environment-axis sharding + the single action all-gather, world_size 2 over gloo.
-The per-rank planner is replaced by a deterministic stand-in (the kernels need a B200); what is under
+The per-rank planner is replaced by a deterministic stand-in (the kernels need a H100); what is under
 test is the host logic bench.py and ShardedActor use: contiguous env blocks, rank-local planning,
 all_gather_into_tensor of [E/G, A] actions in rank order."""
 import os
