@@ -490,7 +490,11 @@ __device__ __forceinline__ float ln_act_lane(float y, bool valid, int act) {
   return valid ? __fdiv_rn(e, t) : 0.f;
 }
 
-// LayerNorm (+ Mish | SimNorm) over raw rows; one warp per row, lane-strided columns; raw re-read from L2 per pass.
+// LayerNorm (+ Mish | SimNorm) over raw rows; one warp per row, lane-strided columns (lane + 32 j).  The output pass
+// re-reads raw from L2; the statistics read it once (512-wide rows) or once per statistic (other widths).  The output
+// pass stays a compact loop: keeping the row in registers through it too raises the kernel's spills (248 B of spill
+// stores instead of 84 with ptxas for sm_90a).
+constexpr int kLnRegCols = 16;
 __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const LayerRec& ly, const EpiArgs& ea) {
   const float* rawbase = raw_ptr(P, c.slot);
   const int N = ly.N;
@@ -503,15 +507,39 @@ __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const L
   const int ncolj = (N + 31) / 32;
   for (int r = c.warp; r < kTileM; r += kWarps) {
     const float* rr = rawbase + static_cast<size_t>(r) * P.NpadMax;
-    float s = 0.f;
-    for (int col = c.lane; col < N; col += 32) s += fmaf(__ldcg(rr + col), inv_scale, bias[col]);
-    const float mean = warp_sum(s) * invN;
-    float sq = 0.f;
-    for (int col = c.lane; col < N; col += 32) {
-      const float d = fmaf(__ldcg(rr + col), inv_scale, bias[col]) - mean;
-      sq = fmaf(d, d, sq);
+    float mean, var;
+    if (N == 32 * kLnRegCols) {
+      // 512-wide rows (every hidden layer of the 5M model): mean and variance from ONE read of the row.  The loads are
+      // unconditional and all issued before the first use, so the row costs one L2 round trip instead of one per
+      // unrolled batch of each statistic's loop.  Same expressions in the same order as below: same bits.
+      float x[kLnRegCols];
+#pragma unroll
+      for (int j = 0; j < kLnRegCols; ++j) x[j] = __ldcg(rr + c.lane + 32 * j);
+      float s = 0.f;
+#pragma unroll
+      for (int j = 0; j < kLnRegCols; ++j) {
+        x[j] = fmaf(x[j], inv_scale, bias[c.lane + 32 * j]);
+        s += x[j];
+      }
+      mean = warp_sum(s) * invN;
+      float sq = 0.f;
+#pragma unroll
+      for (int j = 0; j < kLnRegCols; ++j) {
+        const float d = x[j] - mean;
+        sq = fmaf(d, d, sq);
+      }
+      var = warp_sum(sq) * invN;
+    } else {
+      float s = 0.f;
+      for (int col = c.lane; col < N; col += 32) s += fmaf(__ldcg(rr + col), inv_scale, bias[col]);
+      mean = warp_sum(s) * invN;
+      float sq = 0.f;
+      for (int col = c.lane; col < N; col += 32) {
+        const float d = fmaf(__ldcg(rr + col), inv_scale, bias[col]) - mean;
+        sq = fmaf(d, d, sq);
+      }
+      var = warp_sum(sq) * invN;
     }
-    const float var = warp_sum(sq) * invN;
     const float rstd = 1.f / sqrtf(var + 1e-5f);   // nn.LayerNorm eps (layers.py:101)
     const int orow = ea.rowmap ? ea.rowmap[r] : r;
     for (int j = 0; j < ncolj; ++j) {
