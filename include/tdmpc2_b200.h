@@ -35,10 +35,11 @@
 extern "C" {
 #endif
 
-#define TDMPC2_B200_ABI_VERSION 6   /* 2: tdmpc2_weights.termination, dims.episodic = 1 accepted; 3: tdmpc2_planner_set_l2_persist;
+#define TDMPC2_B200_ABI_VERSION 7   /* 2: tdmpc2_weights.termination, dims.episodic = 1 accepted; 3: tdmpc2_planner_set_l2_persist;
                                        4: tdmpc2_planner_set_passes (declared non-parity fast mode), set_kseg, iter_engine;
                                        5: pixel encoder (tdmpc2_pixel_*), tdmpc2_plan_prologue_latent, dims.num_enc_layers = 0;
-                                       6: tdmpc2_plan_iter_rng (declared non-parity in-kernel noise), tdmpc2_debug_rng */
+                                       6: tdmpc2_plan_iter_rng (declared non-parity in-kernel noise), tdmpc2_debug_rng;
+                                       7: world-model methods on a flat batch (tdmpc2_wm_*, tdmpc2_td_target), target Q blob */
 #define TDMPC2_MAX_ENC_LAYERS 8
 
 typedef enum tdmpc2_status {
@@ -232,6 +233,52 @@ int tdmpc2_plan_get_state(tdmpc2_planner* p, float* mean, float* std, float* z,
 int tdmpc2_estimate_value(tdmpc2_planner* p, const float* z, const float* actions,
                           const int32_t* task, const float* noise_pi, const int32_t* qidx,
                           float* value_out, void* stream);
+
+/* ---- world-model methods on a flat batch of rows ------------------------------
+ * The training-side and analysis calls of the reference's WorldModel (world_model.py:103-216) and TDMPC2._td_target
+ * (tdmpc2.py:242-257), each one launch of the fused kernel over `rows` independent rows (any count >= 1; a leading
+ * [H, B] of the reference is flattened by the caller).  They share the planner's packed weights and scratch, and leave
+ * its planning state untouched.  Every random number is an input (the reference draws them inside pi() and Q()).
+ *   task: int32 [rows] or NULL (single-task); all fp32 row tensors are contiguous [rows, .]. */
+
+/* The target Q ensemble (_target_Qs_params.*, world_model.py:41) lives in its own caller-owned blob, so that a planner
+ * that never runs a target op keeps its memory.  bytes: size of that blob (TDMPC2_ERR_UNSUPPORTED when the model's
+ * weight-map classes leave no room for the target's).  bind: attach it (256-byte aligned; again after
+ * tdmpc2_planner_bind).  pack: target_qs[l] = _target_Qs_params.{l}.* with the leading [num_q] dim; call again after
+ * every target update (soft_update_target_Q, world_model.py:76-80).  Ops with target weights fail with
+ * TDMPC2_ERR_STATE until both ran. */
+int tdmpc2_planner_target_q_bytes(const tdmpc2_planner* p, size_t* out);
+int tdmpc2_planner_bind_target_q(tdmpc2_planner* p, void* blob);
+int tdmpc2_pack_target_q(tdmpc2_planner* p, const tdmpc2_linear target_qs[3], void* stream);
+
+/* Replaces WorldModel.encode (world_model.py:103-112), state observations: obs [rows, obs_dim] -> z_out [rows, L]. */
+int tdmpc2_wm_encode(tdmpc2_planner* p, const float* obs, const int32_t* task, int rows, float* z_out, void* stream);
+/* Replaces WorldModel.next (world_model.py:114-121): z [rows, L], a [rows, A] -> z_out [rows, L]. */
+int tdmpc2_wm_next(tdmpc2_planner* p, const float* z, const float* a, const int32_t* task, int rows, float* z_out, void* stream);
+/* Replaces WorldModel.reward (world_model.py:123-130): -> logits_out [rows, num_bins]. */
+int tdmpc2_wm_reward(tdmpc2_planner* p, const float* z, const float* a, const int32_t* task, int rows, float* logits_out,
+                     void* stream);
+/* Replaces WorldModel.termination (world_model.py:132-141; episodic single-task models, else TDMPC2_ERR_UNSUPPORTED):
+ * out [rows, 1] = sigmoid(logit) (sigmoid != 0) or the logit (unnormalized=True). */
+int tdmpc2_wm_termination(tdmpc2_planner* p, const float* z, int rows, int sigmoid, float* out, void* stream);
+/* Replaces WorldModel.pi (world_model.py:144-184) with eps [rows, A] = its randn_like draw: action_out, mean_out
+ * (= tanh(mean), info["mean"]), log_std_out [rows, A]; log_prob_out [rows, 2] = (gaussian_logprob(eps, log_std),
+ * sum of the squash terms log(relu(1 - action^2) + 1e-6)) (math.py:16-29): entropy = -(lp - sq); scaled_entropy =
+ * entropy * lp * size / (lp - sq + 1e-8), size = A or the task's action-mask sum. */
+int tdmpc2_wm_pi(tdmpc2_planner* p, const float* z, const int32_t* task, const float* eps, int rows, float* action_out,
+                 float* mean_out, float* log_std_out, float* log_prob_out, void* stream);
+/* Replaces WorldModel.Q (world_model.py:186-216).  target != 0: the target ensemble (else the online one; `detach`
+ * reads the same weights).  TDMPC2_Q_ALL: out [num_q, rows, num_bins] logits, qidx unused; TDMPC2_Q_MIN / _AVG:
+ * qidx [2] int32 (= randperm(num_q)[:2]), out [rows, 1] = min (NaN-propagating, like torch.min) or average of the
+ * two heads' two_hot_inv values. */
+typedef enum tdmpc2_q_return { TDMPC2_Q_ALL = 0, TDMPC2_Q_MIN = 1, TDMPC2_Q_AVG = 2 } tdmpc2_q_return;
+int tdmpc2_wm_q(tdmpc2_planner* p, const float* z, const float* a, const int32_t* task, int rows, int target,
+                int return_type, const int32_t* qidx, float* out, void* stream);
+/* Replaces TDMPC2._td_target (tdmpc2.py:242-257) in one launch: action = pi(next_z) with eps [rows, A], then
+ * out [rows, 1] = reward + discount[task] * (1 - terminated) * min(Q_target[qidx[0]], Q_target[qidx[1]]);
+ * reward, terminated [rows, 1]. */
+int tdmpc2_td_target(tdmpc2_planner* p, const float* next_z, const float* reward, const float* terminated,
+                     const int32_t* task, const float* eps, const int32_t* qidx, int rows, float* out, void* stream);
 
 /* Diagnostics: y[rows, out] = act(LN(x W^T + b)) for ONE packed layer, through
  * the same fused kernels (rows <= 128).  layer index: 0.. = enc, then dynamics

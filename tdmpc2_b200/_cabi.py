@@ -11,7 +11,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("TDMPC2_B200_LIB") or os.path.join(HERE, "libtdmpc2_b200.so")
 MAX_ENC_LAYERS = 8
 ENGINE_TCGEN05, ENGINE_SIMT, ENGINE_TCGEN05_2SM, ENGINE_TCGEN05_PP, ENGINE_TCGEN05_2SM_PF = 0, 1, 2, 3, 4
-ABI_VERSION = 6            # TDMPC2_B200_ABI_VERSION of include/tdmpc2_b200.h this binding was written against
+Q_ALL, Q_MIN, Q_AVG = 0, 1, 2   # tdmpc2_q_return
+ABI_VERSION = 7            # TDMPC2_B200_ABI_VERSION of include/tdmpc2_b200.h this binding was written against
 
 # every symbol include/tdmpc2_b200.h declares
 SYMBOLS = [
@@ -21,6 +22,9 @@ SYMBOLS = [
     "tdmpc2_pixel_encoder_create", "tdmpc2_pixel_encoder_destroy", "tdmpc2_pixel_encoder_workspace_bytes", "tdmpc2_pixel_encode", "tdmpc2_plan_iter", "tdmpc2_plan_iter_rng", "tdmpc2_debug_rng",
     "tdmpc2_plan_epilogue", "tdmpc2_plan_get_state", "tdmpc2_estimate_value", "tdmpc2_debug_layer",
     "tdmpc2_planner_layer_count", "tdmpc2_planner_launch_count", "tdmpc2_planner_set_profile",
+    "tdmpc2_planner_target_q_bytes", "tdmpc2_planner_bind_target_q", "tdmpc2_pack_target_q",
+    "tdmpc2_wm_encode", "tdmpc2_wm_next", "tdmpc2_wm_reward", "tdmpc2_wm_termination", "tdmpc2_wm_pi", "tdmpc2_wm_q",
+    "tdmpc2_td_target",
 ]
 
 
@@ -107,6 +111,16 @@ def load():
     lib.tdmpc2_planner_set_profile.argtypes = [vp, vp]
     lib.tdmpc2_planner_launch_count.argtypes = [vp]
     lib.tdmpc2_planner_launch_count.restype = i64
+    lib.tdmpc2_planner_target_q_bytes.argtypes = [vp, C.POINTER(C.c_size_t)]
+    lib.tdmpc2_planner_bind_target_q.argtypes = [vp, vp]
+    lib.tdmpc2_pack_target_q.argtypes = [vp, C.POINTER(Linear), vp]
+    lib.tdmpc2_wm_encode.argtypes = [vp, vp, vp, C.c_int, vp, vp]
+    lib.tdmpc2_wm_next.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp]
+    lib.tdmpc2_wm_reward.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp]
+    lib.tdmpc2_wm_termination.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp]
+    lib.tdmpc2_wm_pi.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
+    lib.tdmpc2_wm_q.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]
+    lib.tdmpc2_td_target.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_int, vp, vp]
     for s in SYMBOLS:
         f = getattr(lib, s)
         if f.restype is C.c_int and s not in ("tdmpc2_abi_version", "tdmpc2_planner_layer_count"):

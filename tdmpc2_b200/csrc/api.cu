@@ -114,6 +114,18 @@ struct LayerHost {
   size_t off_hi, off_lo, off_bias, off_g, off_b;   // byte offsets into the packed blob
 };
 
+// Target Q ensemble (_target_Qs_params.*, world_model.py:41): its own caller-owned blob, so that a planner that never
+// runs a target op keeps its packed_bytes.  Same layer shapes as the online heads; own weight maps (tmW[base_map + m]).
+struct TargetQ {
+  std::vector<LayerHost> layers;   // 3 * num_q, head h layer l at 3 h + l
+  int nmaps = 0, base_map = 0;
+  int map_kpad[kMaxWMaps], map_rows[kMaxWMaps];
+  size_t map_off[kMaxWMaps];
+  size_t off_table = 0, off_absmax = 0, bytes = 0;   // bytes == 0: the model's maps leave no room (target ops unsupported)
+  uint8_t* blob = nullptr;
+  bool packed = false;
+};
+
 struct tdmpc2_planner {
   tdmpc2_dims d;
   int num_sms = 0, nslots = 0;
@@ -134,7 +146,8 @@ struct tdmpc2_planner {
   PlanParams base;
   int engine = TDMPC2_ENGINE_TCGEN05;
   bool bound = false, weights_ok = false;
-  bool attr_done[4] = {};           // dynamic-smem opt-in done, per plan_kernel instantiation
+  bool attr_done[6] = {};           // dynamic-smem opt-in done, per plan_kernel instantiation
+  TargetQ tq;
   int64_t launches = 0;
   size_t l2_window_bytes = 0;       // > 0: launches carry a persisting-L2 access-policy window over the activation scratch
   float l2_hit_ratio = 1.f;
@@ -290,6 +303,49 @@ extern "C" int tdmpc2_planner_create(const tdmpc2_dims* dims, tdmpc2_planner** o
   p->zb_kc0 = env_uint("TDMPC2_B200_ZFOLD", 1) ? (L + T) / kKch : 0;
   p->off_zbias = off; off = align_up(off + 2 * E * static_cast<size_t>(p->zb_pitch) * 4, 256);
   p->ws_bytes = align_up(off, 1024);
+
+  // ---- target Q blob layout: table | absmax | per-layer vectors | one weight map per Kpad class of the online heads
+  TargetQ& tq = p->tq;
+  tq.base_map = p->nmaps;
+  bool tq_ok = true;
+  for (int h = 0; h < d.num_q && tq_ok; ++h)
+    for (int l = 0; l < 3; ++l) {
+      LayerHost t = p->layers[p->li_q + 3 * h + l];
+      int m = -1;
+      for (int i = 0; i < tq.nmaps; ++i) if (tq.map_kpad[i] == t.Kpad) m = i;
+      if (m < 0) {
+        if (tq.base_map + tq.nmaps == kMaxWMaps) { tq_ok = false; break; }
+        m = tq.nmaps++;
+        tq.map_kpad[m] = t.Kpad;
+        tq.map_rows[m] = 0;
+      }
+      t.wmap = tq.base_map + m;
+      t.wrow = tq.map_rows[m];
+      tq.map_rows[m] += 2 * t.Npad;
+      tq.layers.push_back(t);
+    }
+  if (tq_ok) {
+    off = 0;
+    tq.off_table = off; off = align_up(off + tq.layers.size() * sizeof(LayerDev), 256);
+    tq.off_absmax = off; off = align_up(off + tq.layers.size() * sizeof(unsigned), 256);
+    for (auto& l : tq.layers) {
+      l.off_bias = off; off = align_up(off + l.Npad * 4, 256);
+      l.off_g = off; off = align_up(off + l.Npad * 4, 256);
+      l.off_b = off; off = align_up(off + l.Npad * 4, 256);
+    }
+    for (int m = 0; m < tq.nmaps; ++m) {
+      off = align_up(off, 1024);
+      tq.map_off[m] = off;
+      off += static_cast<size_t>(tq.map_rows[m]) * tq.map_kpad[m] * 2;
+    }
+    tq.bytes = align_up(off, 1024);
+    for (auto& l : tq.layers) {
+      l.off_hi = tq.map_off[l.wmap - tq.base_map] + static_cast<size_t>(l.wrow) * l.Kpad * 2;
+      l.off_lo = l.off_hi + static_cast<size_t>(l.Npad) * l.Kpad * 2;
+    }
+  } else {
+    tq.layers.clear();
+  }
   *out = p;
   return 0;
 }
@@ -355,6 +411,33 @@ static int make_map(EncodeTiledFn enc, CUtensorMap* m, void* base, uint64_t kpad
   return 0;
 }
 
+// Layer table (host part; inv_scale is filled by the pack kernel) of `layers`, whose offsets are relative to `blob`.
+static int write_layer_table(const std::vector<LayerHost>& layers, uint8_t* blob, size_t off_table) {
+  std::vector<LayerDev> tab(layers.size());
+  for (size_t i = 0; i < tab.size(); ++i) {
+    const LayerHost& l = layers[i];
+    LayerDev& t = tab[i];
+    t.K = l.K; t.Kpad = l.Kpad; t.N = l.N; t.Npad = l.Npad; t.wmap = l.wmap; t.wrow = l.wrow; t.has_ln = l.has_ln;
+    t.inv_scale = 1.f;
+    t.bias = reinterpret_cast<const float*>(blob + l.off_bias);
+    t.ln_g = reinterpret_cast<const float*>(blob + l.off_g);
+    t.ln_b = reinterpret_cast<const float*>(blob + l.off_b);
+    t.w_hi = reinterpret_cast<const __half*>(blob + l.off_hi);
+    t.w_lo = reinterpret_cast<const __half*>(blob + l.off_lo);
+  }
+  CUDA_TRY(cudaMemcpy(blob + off_table, tab.data(), tab.size() * sizeof(LayerDev), cudaMemcpyHostToDevice));
+  return 0;
+}
+
+static EncodeTiledFn encode_tiled_fn() {
+  void* fn = nullptr;
+  cudaDriverEntryPointQueryResult qres;
+  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess ||
+      qres != cudaDriverEntryPointSuccess)
+    return nullptr;
+  return reinterpret_cast<EncodeTiledFn>(fn);
+}
+
 extern "C" int tdmpc2_planner_bind(tdmpc2_planner* p, void* packed, void* workspace) {
   if (!p || !packed || !workspace) return fail(TDMPC2_ERR_INVALID, "null argument");
   if ((reinterpret_cast<uintptr_t>(packed) & 255) || (reinterpret_cast<uintptr_t>(workspace) & 255))
@@ -362,11 +445,8 @@ extern "C" int tdmpc2_planner_bind(tdmpc2_planner* p, void* packed, void* worksp
   p->packed = static_cast<uint8_t*>(packed);
   p->ws = static_cast<uint8_t*>(workspace);
   CUDA_TRY(cudaMemset(p->ws, 0, p->ws_bytes));
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  CUDA_TRY(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-  if (!fn || qres != cudaDriverEntryPointSuccess) return fail(TDMPC2_ERR_CUDA, "cuTensorMapEncodeTiled not available");
-  EncodeTiledFn enc = reinterpret_cast<EncodeTiledFn>(fn);
+  EncodeTiledFn enc = encode_tiled_fn();
+  if (!enc) return fail(TDMPC2_ERR_CUDA, "cuTensorMapEncodeTiled not available");
 
   const tdmpc2_dims& d = p->d;
   PlanParams& B = p->base;
@@ -377,20 +457,7 @@ extern "C" int tdmpc2_planner_bind(tdmpc2_planner* p, void* packed, void* worksp
   for (int m = 0; m < p->nmaps; ++m)
     if ((rc = make_map(enc, &B.tmW[m], p->packed + p->map_off[m], p->map_kpad[m], p->map_rows[m]))) return rc;
 
-  // layer table (host part; inv_scale is filled by the pack kernel)
-  std::vector<LayerDev> tab(p->layers.size());
-  for (size_t i = 0; i < tab.size(); ++i) {
-    const LayerHost& l = p->layers[i];
-    LayerDev& t = tab[i];
-    t.K = l.K; t.Kpad = l.Kpad; t.N = l.N; t.Npad = l.Npad; t.wmap = l.wmap; t.wrow = l.wrow; t.has_ln = l.has_ln;
-    t.inv_scale = 1.f;
-    t.bias = reinterpret_cast<const float*>(p->packed + l.off_bias);
-    t.ln_g = reinterpret_cast<const float*>(p->packed + l.off_g);
-    t.ln_b = reinterpret_cast<const float*>(p->packed + l.off_b);
-    t.w_hi = reinterpret_cast<const __half*>(p->packed + l.off_hi);
-    t.w_lo = reinterpret_cast<const __half*>(p->packed + l.off_lo);
-  }
-  CUDA_TRY(cudaMemcpy(p->packed + p->off_table, tab.data(), tab.size() * sizeof(LayerDev), cudaMemcpyHostToDevice));
+  if ((rc = write_layer_table(p->layers, p->packed, p->off_table))) return rc;
 
   B.layers = reinterpret_cast<const LayerDev*>(p->packed + p->off_table);
   B.E = d.num_envs; B.N = d.num_samples; B.P = d.num_pi_trajs; B.Ppad = p->Ppad; B.K = d.num_elites; B.H = d.horizon;
@@ -420,6 +487,35 @@ extern "C" int tdmpc2_planner_bind(tdmpc2_planner* p, void* packed, void* worksp
   B.zb_kc0 = 0; B.zb_pitch = p->zb_pitch;       // zb_kc0 is set on the CEM-iteration launches only
   p->bound = true;
   p->weights_ok = false;
+  p->tq.blob = nullptr;       // re-encoded maps / table: the target blob must be bound again
+  p->tq.packed = false;
+  return 0;
+}
+
+// Pack Linear `lin` (head `head` of a stacked ensemble tensor) into layer li of `layers`, whose offsets are relative to `blob`.
+static int pack_layer(tdmpc2_planner* p, const std::vector<LayerHost>& layers, uint8_t* blob, size_t off_table, size_t off_absmax,
+                      int li, const tdmpc2_linear& lin, size_t head, cudaStream_t st) {
+  const LayerHost& l = layers[li];
+  LayerDev* table = reinterpret_cast<LayerDev*>(blob + off_table);
+  unsigned* absmax = reinterpret_cast<unsigned*>(blob + off_absmax);
+  if (!lin.weight || !lin.bias) return fail(TDMPC2_ERR_INVALID, "layer %d: null weight/bias", li);
+  if (l.has_ln && (!lin.ln_weight || !lin.ln_bias)) return fail(TDMPC2_ERR_INVALID, "layer %d: missing LayerNorm tensors", li);
+  const float* W = lin.weight + head * static_cast<size_t>(l.src_n) * l.K;
+  const size_t n = static_cast<size_t>(l.src_n) * l.K;
+  const int blocks = static_cast<int>(std::min<size_t>((n + 255) / 256, 1024));
+  absmax_kernel<<<blocks, 256, 0, st>>>(W, n, absmax + li);
+  const size_t tot = static_cast<size_t>(l.Npad) * l.Kpad;
+  split_weight_kernel<<<static_cast<int>(std::min<size_t>((tot + 255) / 256, 2048)), 256, 0, st>>>(
+      W, l.N, l.K, l.Npad, l.Kpad, reinterpret_cast<__half*>(blob + l.off_hi),
+      reinterpret_cast<__half*>(blob + l.off_lo), absmax + li, table + li, l.src_n, l.split_at, l.split_to);
+  const int vb = (l.Npad + 255) / 256;
+  pad_vector_kernel<<<vb, 256, 0, st>>>(lin.bias + head * l.src_n, l.N, l.Npad, reinterpret_cast<float*>(blob + l.off_bias),
+                                        0.f, l.src_n, l.split_at, l.split_to);
+  pad_vector_kernel<<<vb, 256, 0, st>>>(l.has_ln ? lin.ln_weight + head * l.src_n : nullptr, l.N, l.Npad,
+                                        reinterpret_cast<float*>(blob + l.off_g), 1.f, l.src_n, l.split_at, l.split_to);
+  pad_vector_kernel<<<vb, 256, 0, st>>>(l.has_ln ? lin.ln_bias + head * l.src_n : nullptr, l.N, l.Npad,
+                                        reinterpret_cast<float*>(blob + l.off_b), 0.f, l.src_n, l.split_at, l.split_to);
+  p->launches += 5;
   return 0;
 }
 
@@ -432,29 +528,8 @@ extern "C" int tdmpc2_pack_weights(tdmpc2_planner* p, const tdmpc2_weights* w, v
   if (!w->discount_pow || !w->bins) return fail(TDMPC2_ERR_INVALID, "discount_pow and bins are required");
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   CUDA_TRY(cudaMemsetAsync(p->packed + p->off_absmax, 0, p->layers.size() * sizeof(unsigned), st));
-  LayerDev* table = reinterpret_cast<LayerDev*>(p->packed + p->off_table);
-  unsigned* absmax = reinterpret_cast<unsigned*>(p->packed + p->off_absmax);
   auto pack_one = [&](int li, const tdmpc2_linear& lin, size_t head) -> int {
-    const LayerHost& l = p->layers[li];
-    if (!lin.weight || !lin.bias) return fail(TDMPC2_ERR_INVALID, "layer %d: null weight/bias", li);
-    if (l.has_ln && (!lin.ln_weight || !lin.ln_bias)) return fail(TDMPC2_ERR_INVALID, "layer %d: missing LayerNorm tensors", li);
-    const float* W = lin.weight + head * static_cast<size_t>(l.src_n) * l.K;
-    const size_t n = static_cast<size_t>(l.src_n) * l.K;
-    const int blocks = static_cast<int>(std::min<size_t>((n + 255) / 256, 1024));
-    absmax_kernel<<<blocks, 256, 0, st>>>(W, n, absmax + li);
-    const size_t tot = static_cast<size_t>(l.Npad) * l.Kpad;
-    split_weight_kernel<<<static_cast<int>(std::min<size_t>((tot + 255) / 256, 2048)), 256, 0, st>>>(
-        W, l.N, l.K, l.Npad, l.Kpad, reinterpret_cast<__half*>(p->packed + l.off_hi),
-        reinterpret_cast<__half*>(p->packed + l.off_lo), absmax + li, table + li, l.src_n, l.split_at, l.split_to);
-    const int vb = (l.Npad + 255) / 256;
-    pad_vector_kernel<<<vb, 256, 0, st>>>(lin.bias + head * l.src_n, l.N, l.Npad, reinterpret_cast<float*>(p->packed + l.off_bias),
-                                          0.f, l.src_n, l.split_at, l.split_to);
-    pad_vector_kernel<<<vb, 256, 0, st>>>(l.has_ln ? lin.ln_weight + head * l.src_n : nullptr, l.N, l.Npad,
-                                          reinterpret_cast<float*>(p->packed + l.off_g), 1.f, l.src_n, l.split_at, l.split_to);
-    pad_vector_kernel<<<vb, 256, 0, st>>>(l.has_ln ? lin.ln_bias + head * l.src_n : nullptr, l.N, l.Npad,
-                                          reinterpret_cast<float*>(p->packed + l.off_b), 0.f, l.src_n, l.split_at, l.split_to);
-    p->launches += 5;
-    return 0;
+    return pack_layer(p, p->layers, p->packed, p->off_table, p->off_absmax, li, lin, head, st);
   };
   int rc;
   for (int i = 0; i < p->num_enc; ++i) if ((rc = pack_one(p->li_enc + i, w->enc[i], 0))) return rc;
@@ -780,4 +855,166 @@ extern "C" int tdmpc2_debug_layer(tdmpc2_planner* p, int layer, int mode, const 
   prm.dbg_layer = layer; prm.dbg_mode = mode; prm.dbg_rows = rows; prm.dbg_x = x; prm.dbg_y = y;
   prm.ntiles = 1;
   return launch_plan(p, prm, 1, static_cast<cudaStream_t>(stream_));
+}
+
+// ------------------------------------------------------------------------------------ target Q ensemble
+extern "C" int tdmpc2_planner_target_q_bytes(const tdmpc2_planner* p, size_t* out) {
+  if (!p || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (p->tq.bytes == 0) return fail(TDMPC2_ERR_UNSUPPORTED, "the model's weight maps leave no room for the target Q maps (%d)", kMaxWMaps);
+  *out = p->tq.bytes;
+  return 0;
+}
+
+extern "C" int tdmpc2_planner_bind_target_q(tdmpc2_planner* p, void* blob) {
+  if (!p || !blob) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (!p->bound) return fail(TDMPC2_ERR_STATE, "tdmpc2_planner_bind must be called first");
+  if (p->tq.bytes == 0) return fail(TDMPC2_ERR_UNSUPPORTED, "the model's weight maps leave no room for the target Q maps");
+  if (reinterpret_cast<uintptr_t>(blob) & 255) return fail(TDMPC2_ERR_INVALID, "buffers must be 256-byte aligned");
+  TargetQ& tq = p->tq;
+  EncodeTiledFn enc = encode_tiled_fn();
+  if (!enc) return fail(TDMPC2_ERR_CUDA, "cuTensorMapEncodeTiled not available");
+  int rc;
+  for (int m = 0; m < tq.nmaps; ++m)
+    if ((rc = make_map(enc, &p->base.tmW[tq.base_map + m], static_cast<uint8_t*>(blob) + tq.map_off[m], tq.map_kpad[m], tq.map_rows[m])))
+      return rc;
+  if ((rc = write_layer_table(tq.layers, static_cast<uint8_t*>(blob), tq.off_table))) return rc;
+  tq.blob = static_cast<uint8_t*>(blob);
+  tq.packed = false;
+  return 0;
+}
+
+extern "C" int tdmpc2_pack_target_q(tdmpc2_planner* p, const tdmpc2_linear* target_qs, void* stream_) {
+  if (!p || !target_qs) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (!p->bound || !p->tq.blob) return fail(TDMPC2_ERR_STATE, "tdmpc2_planner_bind_target_q must be called first");
+  TargetQ& tq = p->tq;
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  CUDA_TRY(cudaMemsetAsync(tq.blob + tq.off_absmax, 0, tq.layers.size() * sizeof(unsigned), st));
+  int rc;
+  for (int h = 0; h < p->d.num_q; ++h)
+    for (int l = 0; l < 3; ++l)
+      if ((rc = pack_layer(p, tq.layers, tq.blob, tq.off_table, tq.off_absmax, 3 * h + l, target_qs[l], h, st))) return rc;
+  CUDA_TRY(cudaGetLastError());
+  tq.packed = true;
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------ world-model methods (MODE_ROWS)
+static int rows_ready(tdmpc2_planner* p, int rows) {
+  if (!p) {
+    int n = 0;
+    const int rc = check_device(&n);
+    return rc ? rc : fail(TDMPC2_ERR_INVALID, "null planner");
+  }
+  int rc = ready(p);
+  if (rc) return rc;
+  if (rows < 1) return fail(TDMPC2_ERR_INVALID, "rows must be >= 1");
+  return 0;
+}
+
+static PlanParams rows_params(tdmpc2_planner* p, int rop, int rows, const int32_t* task) {
+  PlanParams prm = p->base;
+  prm.mode = MODE_ROWS;
+  prm.rop = rop;
+  prm.rows = rows;
+  prm.task = p->d.task_dim > 0 ? task : nullptr;
+  prm.rows_q = reinterpret_cast<const LayerDev*>(p->packed + p->off_table) + p->li_q;
+  prm.ntiles = (rows + kTileM - 1) / kTileM;
+  return prm;
+}
+
+static int launch_rows(tdmpc2_planner* p, const PlanParams& prm, void* stream_) {
+  const int grid = std::min(prm.ntiles, p->nslots);
+  PlanParams prm2 = prm;
+  prm2.prof = nullptr;
+  prm2.passes = p->passes;
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  if (p->engine == TDMPC2_ENGINE_SIMT) return launch_big(p, plan_kernel<ENGINE_SIMT, false, true>, &p->attr_done[4], grid, st, prm2);
+  return launch_big(p, plan_kernel<ENGINE_TC, false, true>, &p->attr_done[5], grid, st, prm2);
+}
+
+static int need_task(tdmpc2_planner* p, const int32_t* task) {
+  if (p->d.task_dim > 0 && !task) return fail(TDMPC2_ERR_INVALID, "multi-task model needs task indices");
+  return 0;
+}
+
+extern "C" int tdmpc2_wm_encode(tdmpc2_planner* p, const float* obs, const int32_t* task, int rows, float* z_out, void* stream_) {
+  int rc = rows_ready(p, rows);
+  if (rc || (rc = need_task(p, task))) return rc;
+  if (!obs || !z_out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (p->num_enc == 0) return fail(TDMPC2_ERR_STATE, "this planner was created without a state encoder (num_enc_layers = 0)");
+  PlanParams prm = rows_params(p, ROP_ENCODE, rows, task);
+  prm.rows_in = obs; prm.rows_out = z_out;
+  return launch_rows(p, prm, stream_);
+}
+
+static int rows_za(tdmpc2_planner* p, int rop, const float* z, const float* a, const int32_t* task, int rows, float* out, void* stream_) {
+  int rc = rows_ready(p, rows);
+  if (rc || (rc = need_task(p, task))) return rc;
+  if (!z || !a || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  PlanParams prm = rows_params(p, rop, rows, task);
+  prm.rows_in = z; prm.rows_act = a; prm.rows_out = out;
+  return launch_rows(p, prm, stream_);
+}
+extern "C" int tdmpc2_wm_next(tdmpc2_planner* p, const float* z, const float* a, const int32_t* task, int rows, float* z_out, void* stream_) {
+  return rows_za(p, ROP_NEXT, z, a, task, rows, z_out, stream_);
+}
+extern "C" int tdmpc2_wm_reward(tdmpc2_planner* p, const float* z, const float* a, const int32_t* task, int rows, float* logits_out,
+                                void* stream_) {
+  return rows_za(p, ROP_REWARD, z, a, task, rows, logits_out, stream_);
+}
+
+extern "C" int tdmpc2_wm_termination(tdmpc2_planner* p, const float* z, int rows, int sigmoid, float* out, void* stream_) {
+  int rc = rows_ready(p, rows);
+  if (rc) return rc;
+  if (!z || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (p->d.task_dim > 0 || !p->d.episodic)   // world_model.py:28,136: an episodic single-task model has the head
+    return fail(TDMPC2_ERR_UNSUPPORTED, "termination needs an episodic single-task model");
+  PlanParams prm = rows_params(p, ROP_TERM, rows, nullptr);
+  prm.rows_in = z; prm.rows_out = out; prm.rows_flag = sigmoid ? 1 : 0;
+  return launch_rows(p, prm, stream_);
+}
+
+extern "C" int tdmpc2_wm_pi(tdmpc2_planner* p, const float* z, const int32_t* task, const float* eps, int rows, float* action_out,
+                            float* mean_out, float* log_std_out, float* log_prob_out, void* stream_) {
+  int rc = rows_ready(p, rows);
+  if (rc || (rc = need_task(p, task))) return rc;
+  if (!z || !eps || !action_out || !mean_out || !log_std_out || !log_prob_out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  PlanParams prm = rows_params(p, ROP_PI, rows, task);
+  prm.rows_in = z; prm.rows_eps = eps;
+  prm.rows_out = action_out; prm.rows_out2 = mean_out; prm.rows_out3 = log_std_out; prm.rows_out4 = log_prob_out;
+  return launch_rows(p, prm, stream_);
+}
+
+static int select_q(tdmpc2_planner* p, int target, PlanParams& prm) {
+  if (!target) return 0;
+  if (!p->tq.blob || !p->tq.packed)
+    return fail(TDMPC2_ERR_STATE, "target Q op before tdmpc2_planner_bind_target_q + tdmpc2_pack_target_q");
+  prm.rows_q = reinterpret_cast<const LayerDev*>(p->tq.blob + p->tq.off_table);
+  return 0;
+}
+
+extern "C" int tdmpc2_wm_q(tdmpc2_planner* p, const float* z, const float* a, const int32_t* task, int rows, int target,
+                           int return_type, const int32_t* qidx, float* out, void* stream_) {
+  int rc = rows_ready(p, rows);
+  if (rc || (rc = need_task(p, task))) return rc;
+  if (!z || !a || !out || (return_type != TDMPC2_Q_ALL && !qidx)) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (return_type != TDMPC2_Q_ALL && return_type != TDMPC2_Q_MIN && return_type != TDMPC2_Q_AVG)
+    return fail(TDMPC2_ERR_INVALID, "bad return_type %d", return_type);
+  PlanParams prm = rows_params(p, return_type == TDMPC2_Q_ALL ? ROP_Q_ALL : ROP_Q_PAIR, rows, task);
+  if ((rc = select_q(p, target, prm))) return rc;
+  prm.rows_in = z; prm.rows_act = a; prm.rows_out = out; prm.qidx = qidx;
+  prm.rows_flag = return_type == TDMPC2_Q_AVG ? 1 : 0;
+  return launch_rows(p, prm, stream_);
+}
+
+extern "C" int tdmpc2_td_target(tdmpc2_planner* p, const float* next_z, const float* reward, const float* terminated,
+                                const int32_t* task, const float* eps, const int32_t* qidx, int rows, float* out, void* stream_) {
+  int rc = rows_ready(p, rows);
+  if (rc || (rc = need_task(p, task))) return rc;
+  if (!next_z || !reward || !terminated || !eps || !qidx || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  PlanParams prm = rows_params(p, ROP_TD, rows, task);
+  if ((rc = select_q(p, 1, prm))) return rc;
+  prm.rows_in = next_z; prm.rows_eps = eps; prm.qidx = qidx;
+  prm.rows_reward = reward; prm.rows_term = terminated; prm.rows_out = out;
+  return launch_rows(p, prm, stream_);
 }

@@ -11,6 +11,11 @@
 //                   -> value -> [last tile of an env] top-k, MPPI weights, mean/std refit.
 //   MODE_VALUE  : MODE_ITER's rollout on caller-given z / actions, no refit (reference tdmpc2.py:122-136)
 //   MODE_LAYER  : one layer, for diagnostics.
+//   MODE_ROWS   : rows = the caller's flat batch (row r: tile r / 128, tile row r % 128).  ONE world-model method per
+//                 launch (RowOp: encode / next / reward / termination / pi / Q / TD target, reference
+//                 world_model.py:103-216, tdmpc2.py:242-257).  Its own instantiation plan_kernel<ENGINE, false, true>:
+//                 the planning instantiations do not carry its code.  It touches no planner state, only the per-slot
+//                 X / H / raw scratch, which is dead between launches.
 //
 // Every dense layer is `acc = A[128, Kpad] * W[Npad, Kpad]^T` with both operands stored as two fp16 planes (hi, lo;
 // x ~= hi + lo to ~22 bits).  The tensor-core engine (ENGINE_TC) streams 64-element K-chunks of both operands with TMA
@@ -56,7 +61,9 @@ constexpr int kSmemRowBuf = kWarps * kMaxHeadCols * 4;  // one head-output row p
 constexpr int kSmemRowEnv = kTileM * 4;                 // env index of each tile row
 constexpr int kSmemBytes = kStages * kStageBytes + kSmemCtrl + kSmemRowBuf + kSmemRowEnv;
 
-enum Mode { MODE_ENCODE = 0, MODE_PRIOR = 1, MODE_ITER = 2, MODE_VALUE = 3, MODE_LAYER = 4 };
+enum Mode { MODE_ENCODE = 0, MODE_PRIOR = 1, MODE_ITER = 2, MODE_VALUE = 3, MODE_LAYER = 4, MODE_ROWS = 5 };
+// MODE_ROWS: which world-model method a launch runs (PlanParams::rop)
+enum RowOp { ROP_ENCODE = 0, ROP_NEXT = 1, ROP_REWARD = 2, ROP_TERM = 3, ROP_PI = 4, ROP_Q_ALL = 5, ROP_Q_PAIR = 6, ROP_TD = 7 };
 enum Engine { ENGINE_TC = 0, ENGINE_SIMT = 1 };
 // X = [z | emb | a] input planes; H = hidden planes.  ONE hidden buffer is enough: a layer's epilogue only runs after
 // every MMA of its GEMM has consumed the A operand, so layer 1 overwrites its own input in place.
@@ -116,6 +123,19 @@ struct PlanParams {
   // (noise_r / noise_pi are null then); rng_iter = index of this iteration within the plan (selects the Philox stream)
   const unsigned long long* rng_state;
   int rng_iter;
+  // MODE_ROWS (world-model methods on the caller's flat batch of `rows` rows; fp32 inputs / outputs, caller-owned)
+  int rows, rop;
+  int rows_flag;                   // ROP_TERM: 1 = sigmoid; ROP_Q_PAIR / ROP_TD: 0 = min of the two heads, 1 = average
+  const float* rows_in;            // obs [rows, obs_dim] (ROP_ENCODE) or z [rows, L]
+  const float* rows_act;           // a [rows, A]
+  const float* rows_eps;           // pi noise [rows, A]
+  const float* rows_reward;        // ROP_TD: reward [rows], terminated [rows]
+  const float* rows_term;
+  const LayerDev* rows_q;          // the 3 num_q layers of the Q ensemble this launch reads (online or target weights)
+  float* rows_out;                 // z' / logits [rows, .]; Q all [num_q, rows, B]; pi action [rows, A]; Q pair / TD [rows]
+  float* rows_out2;                // ROP_PI: tanh(mean) [rows, A]
+  float* rows_out3;                // ROP_PI: log_std [rows, A]
+  float* rows_out4;                // ROP_PI: [rows, 2] = (gaussian log-prob, sum of the squash terms)
 };
 
 // The layer table lives in global memory; role loops are full of asm volatile(... "memory") (TMA issue, mbarrier waits,
@@ -578,7 +598,57 @@ __device__ __forceinline__ float two_hot_inv_row(const PlanParams& P, Ctx& c, co
   return symexp_f(acc);
 }
 
-template <bool EPISODIC>
+// ------------------------------------------------------------------------------------ MODE_ROWS epilogues
+// torch.min(0) of two values: NaN if either is NaN (fminf would return the other one)
+__device__ __forceinline__ float nan_min(float a, float b) { return (isnan(a) || isnan(b)) ? CUDART_NAN_F : fminf(a, b); }
+
+// Q pair (world_model.py:211-216) and TD target (tdmpc2.py:255-257) of tile row r; one thread per row.
+__device__ __forceinline__ void rows_commit(const PlanParams& P, Ctx& c, const EpiArgs& ea, int r, float val) {
+  if (ea.head == HEAD_Q1) { c.q1[r] = val; return; }
+  const float q = P.rows_flag ? __fmul_rn(__fadd_rn(c.q1[r], val), 0.5f) : nan_min(c.q1[r], val);   // Q.sum(0) / 2 | Q.min(0)
+  const int row = c.rowenv[r];
+  if (row < 0) return;
+  if (P.rop == ROP_TD) {
+    // reward + discount * (1 - terminated) * Q, evaluated left to right like the reference's fp32 expression
+    const int task = P.task ? P.task[row] : 0;
+    const float disc = P.disc_pow[static_cast<size_t>(task) * (P.H + 1) + 1];
+    P.rows_out[row] = __fadd_rn(P.rows_reward[row], __fmul_rn(__fmul_rn(disc, __fsub_rn(1.f, P.rows_term[row])), q));
+  } else {
+    P.rows_out[row] = q;
+  }
+}
+
+// WorldModel.pi (world_model.py:144-184, math.py:12-29) for tile row r: the action goes to the X action columns (the
+// TD target's Q heads read it there) and, for ROP_PI, to the outputs with tanh(mean), log_std and the two row sums the
+// host turns into entropy / scaled_entropy.
+__device__ __forceinline__ void rows_pi(const PlanParams& P, Ctx& c, const float* myrow, int r, __half* xhi, __half* xlo) {
+  const int row = c.rowenv[r];
+  const int e = row < 0 ? 0 : row;
+  const int task = P.task ? P.task[e] : 0;
+  float lp = 0.f, sq = 0.f;
+  for (int a = c.lane; a < P.A; a += 32) {
+    float mu = myrow[a];
+    float ls = __fadd_rn(P.log_std_min, __fmul_rn(__fmul_rn(0.5f, P.log_std_dif), __fadd_rn(tanhf(myrow[P.Apad + a]), 1.f)));
+    float eps = P.rows_eps[static_cast<size_t>(e) * P.A + a];
+    if (P.masks) { const float mk = P.masks[static_cast<size_t>(task) * P.A + a]; mu *= mk; ls *= mk; eps *= mk; }
+    lp += __fsub_rn(__fsub_rn(__fmul_rn(-0.5f, __fmul_rn(eps, eps)), ls), 0.9189385175704956f);   // gaussian_logprob
+    const float act = tanhf(__fadd_rn(mu, __fmul_rn(eps, expf(ls))));
+    sq += logf(__fadd_rn(fmaxf(__fsub_rn(1.f, __fmul_rn(act, act)), 0.f), 1e-6f));                // squash
+    const size_t o = static_cast<size_t>(r) * P.KpadX + P.L + P.T + a;
+    split_store(xhi + o, xlo + o, act);
+    if (P.rows_out2 && row >= 0) {
+      const size_t ro = static_cast<size_t>(row) * P.A + a;
+      P.rows_out[ro] = act;
+      P.rows_out2[ro] = tanhf(mu);
+      P.rows_out3[ro] = ls;
+    }
+  }
+  lp = warp_sum(lp);
+  sq = warp_sum(sq);
+  if (P.rows_out4 && row >= 0 && c.lane == 0) { P.rows_out4[2 * static_cast<size_t>(row)] = lp; P.rows_out4[2 * static_cast<size_t>(row) + 1] = sq; }
+}
+
+template <bool EPISODIC, bool ROWS>
 __device__ __forceinline__ void rows_head(const PlanParams& P, Ctx& c, const LayerRec& ly, const EpiArgs& ea) {
   float* myrow = c.rowbuf + c.warp * kMaxHeadCols;
   __half* xhi = plane_ptr(P, c.slot, BUF_X, 0);
@@ -588,13 +658,21 @@ __device__ __forceinline__ void rows_head(const PlanParams& P, Ctx& c, const Lay
       const int orow = ea.rowmap ? ea.rowmap[r] : r;
       const float* rr = raw_ptr(P, c.slot) + static_cast<size_t>(r) * P.NpadMax;
       if (orow >= 0)
-        for (int col = c.lane; col < ly.N; col += 32)
-          ea.out_f32[static_cast<size_t>(orow) * ea.out_pitch + col] = fmaf(__ldcg(rr + col), ly.inv_scale, ly.bias[col]);
+        for (int col = c.lane; col < ly.N; col += 32) {
+          float v = fmaf(__ldcg(rr + col), ly.inv_scale, ly.bias[col]);
+          if (ROWS && ea.head) v = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-v)));      // termination: sigmoid
+          ea.out_f32[static_cast<size_t>(orow) * ea.out_pitch + col] = v;
+        }
       continue;
     }
     head_row_to_smem(P, c, ly, r, myrow);
     if (EPISODIC && ea.kind == EPI_TERM) {
       if (c.lane == 0) term_commit(c, r, myrow[0]);
+    } else if (ROWS && ea.kind == EPI_TWOHOT) {
+      const float v = two_hot_inv_row(P, c, myrow);
+      if (c.lane == 0) rows_commit(P, c, ea, r, v);
+    } else if (ROWS && ea.kind == EPI_PI) {
+      rows_pi(P, c, myrow, r, xhi, xlo);
     } else if (ea.kind == EPI_TWOHOT) {
       const float v = two_hot_inv_row(P, c, myrow);
       if (c.lane == 0) head_commit<EPISODIC>(P, c, ea, r, v);
@@ -626,7 +704,7 @@ __device__ __forceinline__ void publish_planes() {
 
 // ------------------------------------------------------------------------------------ one layer
 // GEMM + epilogue; on return the epilogue's outputs are published (CTA-synchronised, TMA-visible).
-template <int ENGINE, bool EPISODIC>
+template <int ENGINE, bool EPISODIC, bool ROWS>
 __device__ __forceinline__ void run_layer(const PlanParams& P, Ctx& c, const LayerDev& ly_global, int srcbuf, const EpiArgs& ea,
                                           int kc0 = 0, const float* bias_override = nullptr) {
   LayerRec ly = layer_rec(ly_global);                // registers: see LayerRec
@@ -638,7 +716,7 @@ __device__ __forceinline__ void run_layer(const PlanParams& P, Ctx& c, const Lay
   else gemm_simt(P, c, ly, srcbuf, kc0);
   if (threadIdx.x == 0) TDMPC2_TRACE(P, c, 3);
   if (is_ln) rows_ln_act(P, c, ly, ea);
-  else rows_head<EPISODIC>(P, c, ly, ea);
+  else rows_head<EPISODIC, ROWS>(P, c, ly, ea);
   c.pf1 += prof_clock() - tl;
   const long long tp = prof_clock();
   publish_planes();
@@ -749,7 +827,8 @@ __device__ __forceinline__ void refit_env(const PlanParams& P, uint8_t* scratch,
 // ------------------------------------------------------------------------------------ the kernel
 // EPISODIC (cfg.episodic, single-task models): every rollout step gains the 3-layer termination head on z_{t+1}
 // and the value bookkeeping its sticky (1 - termination) factor (tdmpc2.py:126-136); compiled out otherwise.
-template <int ENGINE, bool EPISODIC = false>
+// ROWS: MODE_ROWS only (world-model methods on a flat batch); compiled out of the planning instantiations.
+template <int ENGINE, bool EPISODIC = false, bool ROWS = false>
 __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant__ PlanParams P) {
   constexpr int SPT = EPISODIC ? 9 : 6;      // layer steps per rollout time step (ITER / VALUE)
   extern __shared__ uint8_t smem_raw[];
@@ -795,7 +874,8 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
     // ---------------- tile set-up: fill the input planes of X ----------------
     const long long t_setup = prof_clock();
     for (int r = threadIdx.x; r < kTileM; r += kThreads) {
-      rowenv[r] = map_row(P, tile, r).env; c.G[r] = 0.f; c.q1[r] = 0.f;
+      rowenv[r] = ROWS ? (tile * kTileM + r < P.rows ? tile * kTileM + r : -1) : map_row(P, tile, r).env;
+      c.G[r] = 0.f; c.q1[r] = 0.f;
       if (EPISODIC) c.term[r] = 0.f;
     }
     __syncthreads();
@@ -804,7 +884,25 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
     const int env_tile = (P.mode == MODE_ITER || P.mode == MODE_VALUE) ? tile / P.tiles_per_env : 0;
     const int task_tile = (P.task && (P.mode == MODE_ITER || P.mode == MODE_VALUE)) ? P.task[env_tile] : 0;
 
-    if (P.mode == MODE_LAYER) {
+    if (ROWS) {
+      // the call's input columns, zeros in every other column of X (stale action columns of an earlier launch
+      // must not reach a GEMM) and in the padding rows:
+      //   encode [obs | emb]; next / reward / Q [z | emb | a]; termination [z]; pi / TD target [z | emb]
+      const int in_w = P.rop == ROP_ENCODE ? P.obs_dim : P.L;
+      const int W = in_w + (P.rop == ROP_TERM ? 0 : P.T);
+      const bool has_a = P.rop == ROP_NEXT || P.rop == ROP_REWARD || P.rop == ROP_Q_ALL || P.rop == ROP_Q_PAIR;
+      for (int i = threadIdx.x; i < kTileM * P.KpadX; i += kThreads) {
+        const int r = i / P.KpadX, col = i % P.KpadX;
+        const int e = rowenv[r];
+        float x = 0.f;
+        if (e >= 0) {
+          if (col < in_w) x = P.rows_in[static_cast<size_t>(e) * in_w + col];
+          else if (col < W) x = P.emb[static_cast<size_t>(P.task ? P.task[e] : 0) * P.T + (col - in_w)];
+          else if (has_a && col < W + P.A) x = P.rows_act[static_cast<size_t>(e) * P.A + (col - W)];
+        }
+        split_store(xhi + static_cast<size_t>(r) * P.KpadX + col, xlo + static_cast<size_t>(r) * P.KpadX + col, x);
+      }
+    } else if (P.mode == MODE_LAYER) {
       const LayerDev& ly = LY[P.dbg_layer];
       for (int i = threadIdx.x; i < kTileM * ly.Kpad; i += kThreads) {
         const int r = i / ly.Kpad, col = i % ly.Kpad;
@@ -891,7 +989,9 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
     //   PRIOR  : per t: pi.0-2 [, dyn.0-2 if t < H-1]
     //   ITER   : per t: [a_t -> X] rew.0-2, dyn.0-2 [, term.0-2 if EPISODIC] ; then pi.0-2, q_a.0-2, q_b.0-2
     int nsteps;
-    if (P.mode == MODE_LAYER) nsteps = 1;
+    if (ROWS) nsteps = P.rop == ROP_ENCODE ? P.num_enc : P.rop == ROP_Q_ALL ? 3 * P.num_q : P.rop == ROP_Q_PAIR ? 6
+                     : P.rop == ROP_TD ? 9 : 3;
+    else if (P.mode == MODE_LAYER) nsteps = 1;
     else if (P.mode == MODE_ENCODE) nsteps = P.num_enc;
     else if (P.mode == MODE_PRIOR) nsteps = 6 * (P.H - 1) + 3;
     else nsteps = SPT * P.H + 9;
@@ -905,7 +1005,42 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
       int li, src;
       int kc0 = 0;                       // first K-chunk of the GEMM and bias vector: the shared-latent fold (PlanParams::zbias)
       const float* bias_ov = nullptr;
-      if (P.mode == MODE_LAYER) {
+      const LayerDev* lyt = LY;          // layer table of this step (MODE_ROWS Q heads: P.rows_q)
+      if (ROWS) {
+        // ROWS program:  encode enc.0..n-1 | next dyn.0-2 | reward rew.0-2 | termination term.0-2 | pi pi.0-2
+        //                | Q all: head h = 0..num_q-1, layers 0-2 | Q pair: heads qidx[0], qidx[1] | TD: pi.0-2, then Q pair
+        const int l = P.rop == ROP_ENCODE ? sidx : sidx % 3;
+        src = l == 0 ? BUF_X : BUF_H1;
+        ea.rowmap = rowenv;
+        const bool last = P.rop == ROP_ENCODE ? sidx == P.num_enc - 1 : l == 2;
+        if (!last) { ea.kind = EPI_LN_MISH; ea.dstbuf = BUF_H1; }
+        if (P.rop == ROP_ENCODE) {
+          li = P.li_enc + sidx;
+          if (last) { ea.kind = EPI_LN_SIMNORM; ea.out_f32 = P.rows_out; ea.out_pitch = P.L; }
+        } else if (P.rop == ROP_NEXT) {
+          li = P.li_dyn + l;
+          if (last) { ea.kind = EPI_LN_SIMNORM; ea.out_f32 = P.rows_out; ea.out_pitch = P.L; }
+        } else if (P.rop == ROP_REWARD) {
+          li = P.li_rew + l;
+          if (last) { ea.kind = EPI_RAW; ea.out_f32 = P.rows_out; ea.out_pitch = P.B; }
+        } else if (P.rop == ROP_TERM) {
+          li = P.li_term + l;
+          if (last) { ea.kind = EPI_RAW; ea.out_f32 = P.rows_out; ea.out_pitch = 1; ea.head = P.rows_flag; }
+        } else if (P.rop == ROP_PI || (P.rop == ROP_TD && sidx < 3)) {
+          li = P.li_pi + l;
+          if (last) ea.kind = EPI_PI;
+        } else {
+          const int u = P.rop == ROP_TD ? sidx / 3 - 1 : sidx / 3;     // head slot
+          const int h = P.rop == ROP_Q_ALL ? u : P.qidx[u];
+          lyt = P.rows_q;
+          li = 3 * h + l;
+          if (last && P.rop == ROP_Q_ALL) {
+            ea.kind = EPI_RAW; ea.out_f32 = P.rows_out + static_cast<size_t>(h) * P.rows * P.B; ea.out_pitch = P.B;
+          } else if (last) {
+            ea.kind = EPI_TWOHOT; ea.head = u == 0 ? HEAD_Q1 : HEAD_Q2;
+          }
+        }
+      } else if (P.mode == MODE_LAYER) {
         li = P.dbg_layer; src = BUF_X;
         ea.kind = P.dbg_mode == 0 ? EPI_RAW : (P.dbg_mode == 1 ? EPI_LN_MISH : EPI_LN_SIMNORM);
         ea.out_f32 = P.dbg_y; ea.out_pitch = LY[li].N; ea.rowmap = rowenv;
@@ -1038,7 +1173,7 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
         }
       }
       c.trace_step = (tile == static_cast<int>(blockIdx.x)) ? sidx : (1 << 30);
-      run_layer<ENGINE, EPISODIC>(P, c, LY[li], src, ea, kc0, bias_ov);
+      run_layer<ENGINE, EPISODIC, ROWS>(P, c, lyt[li], src, ea, kc0, bias_ov);
     }
 
     const long long t_refit = prof_clock();

@@ -233,6 +233,8 @@ class Planner:
         self._e1_noise = {}   # eval_mode -> static noise buffers of plan_interleaved
         self._draw_stream = None
         self._graph_launches = 0
+        self.target_blob = None      # target Q ensemble (tdmpc2_planner_bind_target_q), allocated by the first target op
+        self.target_version = None
 
     def __del__(self):
         try:
@@ -523,6 +525,84 @@ class Planner:
         self._graph_launches -= st["launches"]         # the capture pass itself launched nothing
         self._graphs[eval_mode] = st
         return st
+
+    # ------------------------------------------------------------------ world-model methods on a flat batch of rows
+    # Inputs are [rows, .] fp32 and task [rows] int32 | None, contiguous on self.device; outputs are fresh tensors.
+    def pack_target_q(self, sd: Dict[str, torch.Tensor]) -> None:
+        """Pack `_target_Qs_params.*` of a reference-layout state dict into the target blob (allocated on first use)."""
+        f = lambda k: sd[k].detach().to(self.device, torch.float32).contiguous()
+        with torch.cuda.device(self.device):
+            if self.target_blob is None:
+                nb = C.c_size_t()
+                _cabi.check(self.lib.tdmpc2_planner_target_q_bytes(self.h, C.byref(nb)))
+                blob = torch.empty(nb.value, dtype=torch.uint8, device=self.device)
+                _cabi.check(self.lib.tdmpc2_planner_bind_target_q(self.h, blob.data_ptr()))
+                self.target_blob = blob
+            keep, lins = [], (_cabi.Linear * 3)()
+            for i in range(3):
+                pfx = f"_target_Qs_params.{i}"
+                t = [f(pfx + ".weight"), f(pfx + ".bias")]
+                if pfx + ".ln.weight" in sd:
+                    t += [f(pfx + ".ln.weight"), f(pfx + ".ln.bias")]
+                keep.extend(t)
+                lins[i] = _cabi.Linear(*[x.data_ptr() for x in t])
+            _cabi.check(self.lib.tdmpc2_pack_target_q(self.h, lins, self._stream()))
+            torch.cuda.current_stream(self.device).synchronize()   # `keep` tensors may be freed afterwards
+
+    def _rows_out(self, *shape) -> torch.Tensor:
+        return torch.empty(*shape, device=self.device, dtype=torch.float32)
+
+    def wm_encode(self, obs, task) -> torch.Tensor:
+        z = self._rows_out(obs.shape[0], self.cfg.latent_dim)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_wm_encode(self.h, _ptr(obs), _ptr(task), obs.shape[0], _ptr(z), self._stream()))
+        return z
+
+    def wm_next(self, z, a, task) -> torch.Tensor:
+        out = self._rows_out(z.shape[0], self.cfg.latent_dim)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_wm_next(self.h, _ptr(z), _ptr(a), _ptr(task), z.shape[0], _ptr(out), self._stream()))
+        return out
+
+    def wm_reward(self, z, a, task) -> torch.Tensor:
+        out = self._rows_out(z.shape[0], self.cfg.num_bins)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_wm_reward(self.h, _ptr(z), _ptr(a), _ptr(task), z.shape[0], _ptr(out), self._stream()))
+        return out
+
+    def wm_termination(self, z, sigmoid: bool) -> torch.Tensor:
+        out = self._rows_out(z.shape[0], 1)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_wm_termination(self.h, _ptr(z), z.shape[0], int(bool(sigmoid)), _ptr(out),
+                                                       self._stream()))
+        return out
+
+    def wm_pi(self, z, task, eps):
+        """-> action, tanh(mean), log_std [rows, A] and [rows, 2] = (gaussian log-prob, sum of the squash terms)."""
+        R, A = z.shape[0], self.cfg.action_dim
+        act, mean, ls, lp = self._rows_out(R, A), self._rows_out(R, A), self._rows_out(R, A), self._rows_out(R, 2)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_wm_pi(self.h, _ptr(z), _ptr(task), _ptr(eps), R, _ptr(act), _ptr(mean), _ptr(ls),
+                                              _ptr(lp), self._stream()))
+        return act, mean, ls, lp
+
+    def wm_q(self, z, a, task, target: bool, return_type: str, qidx=None) -> torch.Tensor:
+        """return_type 'all' -> logits [num_q, rows, B]; 'min' / 'avg' of heads qidx [2] int32 -> [rows, 1]."""
+        R = z.shape[0]
+        rt = {"all": _cabi.Q_ALL, "min": _cabi.Q_MIN, "avg": _cabi.Q_AVG}[return_type]
+        out = self._rows_out(self.cfg.num_q, R, self.cfg.num_bins) if rt == _cabi.Q_ALL else self._rows_out(R, 1)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_wm_q(self.h, _ptr(z), _ptr(a), _ptr(task), R, int(bool(target)), rt, _ptr(qidx),
+                                             _ptr(out), self._stream()))
+        return out
+
+    def td_target(self, next_z, reward, terminated, task, eps, qidx) -> torch.Tensor:
+        R = next_z.shape[0]
+        out = self._rows_out(R, 1)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_td_target(self.h, _ptr(next_z), _ptr(reward), _ptr(terminated), _ptr(task),
+                                                  _ptr(eps), _ptr(qidx), R, _ptr(out), self._stream()))
+        return out
 
     def estimate_value(self, z, actions, task, noise_pi, qidx):
         """z [E,N,L], actions [E,H,N,A], noise_pi [E,N,A], qidx [E,2] int32 -> [E,N]."""

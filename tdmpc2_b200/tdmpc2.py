@@ -3,9 +3,11 @@
 Drop-in for the inference half of the reference class `TDMPC2`
 (tdmpc2/tdmpc2.py:10-206): `TDMPC2(cfg)`, `.model`, `.cfg`, `.device`,
 `._prev_mean`, `.discount`, `.load()`, `.save()`, `.act()`, `.plan`, `._plan()`,
-`._estimate_value()` keep their names, argument meaning and return shapes, so
-`evaluate.py:57-80` of the reference runs unchanged on it (INTEGRATION.md).
-Training (`update`, optimisers, RunningScale) is out of scope (SURVEY.md 2.1 #1b).
+`._estimate_value()`, `._td_target()` keep their names, argument meaning and return shapes, so
+`evaluate.py:57-80` of the reference runs unchanged on it (INTEGRATION.md), and so does the
+no-grad block of `_update` (`model.encode` + `_td_target`, tdmpc2.py:259-264).
+Gradients (`update`, optimisers, RunningScale) are out of scope (SURVEY.md 2.1 #1b);
+call `sync_weights()` after changing the model's parameters (incl. the target Q update).
 
 New: an environments axis.  `obs [E, obs_dim]`, `t0 [E]`, `task [E]` plan E
 independent environments in one call; E == 1 (1-D obs) is the reference API.
@@ -13,6 +15,7 @@ independent environments in one call; E == 1 (1-D obs) is the reference API.
 from __future__ import annotations
 
 import os
+import weakref
 from typing import Optional, Sequence, Union
 
 import torch
@@ -29,6 +32,7 @@ class TDMPC2(torch.nn.Module):
         self.device = torch.device("cuda:0" if device is None else device)      # tdmpc2.py:20
         self.model = WorldModel(cfg).to(self.device)
         self.model.eval()                                                        # tdmpc2.py:32
+        self.model._agent = weakref.ref(self)                                    # the model's methods share self.planner
         if not cfg.get("iterations_effective", False):
             self.cfg.iterations += 2 * int(cfg.action_dim >= 20)                # tdmpc2.py:34
             self.cfg.iterations_effective = True
@@ -52,14 +56,17 @@ class TDMPC2(torch.nn.Module):
         if self._planner is None:
             self._planner = Planner(self.cfg, self.num_envs, self.device, engine=self._engine)
             self._weights_dirty = True
-        if self._weights_dirty:
+        if self._weights_dirty or self._planner.weights_version != self.model._version:
             self._planner.pack(self.model.state_dict())
+            self._planner.weights_version = self.model._version
             self._weights_dirty = False
         return self._planner
 
     def sync_weights(self) -> None:
-        """Call after modifying `self.model`'s parameters in place."""
+        """Call after modifying `self.model`'s parameters in place (an optimiser step, the Polyak update of the
+        target Q ensemble): the online and target weights are re-packed before the next call that reads them."""
         self._weights_dirty = True
+        self.model.sync_weights()
 
     @property
     def plan(self):
@@ -181,6 +188,13 @@ class TDMPC2(torch.nn.Module):
         self._prev_mean.copy_(new_mean.reshape(self._prev_mean.shape))           # tdmpc2.py:205
         out = action[0] if E == 1 else action
         return (out, trace) if return_trace else out
+
+    @torch.no_grad()
+    def _td_target(self, next_z, reward, terminated, task, *, eps=None, qidx=None):
+        """tdmpc2.py:242-257 as one fused launch: next_z [..., L], reward / terminated [..., 1] ->
+        reward + discount * (1 - terminated) * Q(next_z, pi(next_z), 'min', target=True)  [..., 1].
+        `eps` / `qidx` (default: drawn from self.generator in the reference's order) are pi's noise and the two heads."""
+        return self.model.td_target(next_z, reward, terminated, task, eps=eps, qidx=qidx)
 
     @torch.no_grad()
     def _estimate_value(self, z, actions, task, eps_pi=None, qidx=None):

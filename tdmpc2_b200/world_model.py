@@ -1,9 +1,13 @@
-"""`WorldModel`: the reference's checkpoint surface as a FLAT parameter container.
+"""`WorldModel`: the reference's checkpoint surface as a FLAT parameter container with kernel-backed methods.
 
 The planner's kernels read the weights straight from `state_dict()` (tdmpc2_b200/planner.py packs them into the
-kernel layout), so this class holds tensors, not a module tree: there are no eager forward methods here -- every
-forward of the planning path (encode / next / reward / pi / Q / termination, reference common/world_model.py:103-216)
-runs in the fused sm_90a kernels, including the non-MPC `act()` branch (TDMPC2.act -> the policy-prior kernel mode).
+kernel layout), so this class holds tensors, not a module tree.  Every forward of the planning path runs in the fused
+sm_90a kernels, including the non-MPC `act()` branch (TDMPC2.act -> the policy-prior kernel mode).  The reference's
+methods -- `encode`, `next`, `reward`, `termination`, `pi`, `Q` (common/world_model.py:103-216) -- exist with its
+signatures and shapes and run on the kernels' row mode (one launch per call, any [..., .] batch); `td_target` is
+TDMPC2._td_target's fused launch.  They use the owning agent's Planner, or a one-environment Planner of their own; the
+packed copies are re-packed after `load_state_dict()` / `sync_weights()` (the target ensemble at its next use).  There
+is no CPU fallback: on the CPU the methods raise.
 
 What is kept, because reference checkpoints and `evaluate.py` depend on it (SURVEY.md section 8(b)):
 
@@ -19,11 +23,12 @@ What is kept, because reference checkpoints and `evaluate.py` depend on it (SURV
 """
 from __future__ import annotations
 
-from typing import List
+from typing import List, Optional
 
 import torch
 import torch.nn as nn
 
+from .planner import Planner
 from .synth import QS_PREFIXES, synth_state_dict
 
 _LAYER_PARAM_NAMES = ("weight", "bias", "ln.weight", "ln.bias")
@@ -52,6 +57,9 @@ class WorldModel(nn.Module):
         init["_reward.2.weight"].zero_()                                 # world_model.py:32
         init["_Qs.params.2.weight"].zero_()
         init["_target_Qs_params.2.weight"].zero_()
+        self._agent = None           # weakref to the owning TDMPC2: its Planner serves the forward methods
+        self._planner: Optional[Planner] = None
+        self._version = 0            # bumped by load_state_dict / sync_weights: packed copies compare against it
         self._keys: List[str] = []                                       # owned tensors, in state-dict order
         for key, val in init.items():
             if key.startswith("_detach_Qs_params."):
@@ -119,6 +127,124 @@ class WorldModel(nn.Module):
         known |= {prefix + p + m for p in QS_PREFIXES for m in _META}
         if strict:
             unexpected_keys.extend(k for k in state_dict if k.startswith(prefix) and k not in known)
+        self._version += 1                                               # packed copies are stale
+
+    # ------------------------------------------------------------------ forward methods on the kernels
+    def sync_weights(self) -> None:
+        """Call after modifying parameters in place (an optimiser step, the Polyak update of `_target_Qs_params.*`):
+        the kernels' packed copies are re-packed before the next call that reads them."""
+        self._version += 1
+
+    def _kernels(self) -> Planner:
+        """The Planner whose packed weights these methods run on: the owning agent's, or a one-environment planner of
+        this model's own (created on first use; CUDA only -- there is no CPU fallback)."""
+        agent = self._agent() if self._agent is not None else None
+        if agent is not None:
+            return agent.planner
+        dev = self.tensor(self._keys[0]).device
+        if dev.type != "cuda":
+            raise RuntimeError("WorldModel's forward methods run on the sm_90a kernels: move the model to a CUDA device "
+                               "(there is no CPU fallback)")
+        if self._planner is None or self._planner.device != dev:
+            self._planner = Planner(self.cfg, 1, dev)
+        if self._planner.weights_version != self._version:
+            self._planner.pack(self.state_dict())
+            self._planner.weights_version = self._version
+        return self._planner
+
+    def _target_kernels(self) -> Planner:
+        pl = self._kernels()
+        if pl.target_version != self._version:
+            pl.pack_target_q(self.state_dict())
+            pl.target_version = self._version
+        return pl
+
+    def _generator(self) -> Optional[torch.Generator]:
+        agent = self._agent() if self._agent is not None else None
+        return agent.generator if agent is not None else None
+
+    def _rows(self, pl: Planner, x) -> torch.Tensor:
+        return x.to(pl.device, torch.float32).reshape(-1, x.shape[-1]).contiguous()
+
+    def _task_rows(self, pl: Planner, task, lead) -> Optional[torch.Tensor]:
+        """Per-row int32 task of a batch with leading shape `lead`: an int or [1] applies to every row, a [B] task to
+        the rows of each leading [.., B] slice (task_emb's broadcast, world_model.py:88-101)."""
+        if not self.cfg.multitask:
+            return None
+        t = torch.as_tensor(task, device=pl.device).reshape(-1).to(torch.int32)
+        return t.expand(*lead).reshape(-1).contiguous()
+
+    def encode(self, obs, task):
+        """world_model.py:103-112 (state observations): obs [..., obs_dim] -> z [..., L]."""
+        if self.cfg.get("obs", "state") == "rgb":
+            raise NotImplementedError("row-batched pixel encoding is not built: the pixel encoder is sized per environment")
+        pl = self._kernels()
+        lead = obs.shape[:-1]
+        return pl.wm_encode(self._rows(pl, obs), self._task_rows(pl, task, lead)).view(*lead, -1)
+
+    def next(self, z, a, task):
+        """world_model.py:114-121: z [..., L], a [..., A] -> z' [..., L]."""
+        pl = self._kernels()
+        lead = z.shape[:-1]
+        return pl.wm_next(self._rows(pl, z), self._rows(pl, a), self._task_rows(pl, task, lead)).view(*lead, -1)
+
+    def reward(self, z, a, task):
+        """world_model.py:123-130: -> reward logits [..., num_bins]."""
+        pl = self._kernels()
+        lead = z.shape[:-1]
+        return pl.wm_reward(self._rows(pl, z), self._rows(pl, a), self._task_rows(pl, task, lead)).view(*lead, -1)
+
+    def termination(self, z, task, unnormalized=False):
+        """world_model.py:132-141 (episodic models): -> sigmoid(logit), or the logit, [..., 1]."""
+        assert task is None
+        if not self.cfg.episodic:
+            raise AttributeError("this model has no termination head (cfg.episodic is False)")
+        pl = self._kernels()
+        return pl.wm_termination(self._rows(pl, z), not unnormalized).view(*z.shape[:-1], 1)
+
+    def pi(self, z, task, *, eps: Optional[torch.Tensor] = None):
+        """world_model.py:144-184: -> (action [..., A], info).  `eps` (default: randn_like(mean) from the agent's
+        generator, the reference's draw) is the policy noise."""
+        pl = self._kernels()
+        lead, A = z.shape[:-1], self.cfg.action_dim
+        if eps is None:
+            eps = torch.randn(*lead, A, device=pl.device, generator=self._generator())
+        taskv = self._task_rows(pl, task, lead)
+        act, mean, log_std, lp = pl.wm_pi(self._rows(pl, z), taskv, self._rows(pl, eps))
+        log_prob, log_pi = lp[:, :1], lp[:, :1] - lp[:, 1:]                # gaussian log-prob; after squash (math.py:23-29)
+        size = float(A) if taskv is None else self.tensor("_action_masks").sum(-1)[taskv.long()].unsqueeze(-1)
+        entropy_scale = log_prob * size / (log_pi + 1e-8)
+        info = {"mean": mean.view(*lead, A), "log_std": log_std.view(*lead, A), "action_prob": 1.,
+                "entropy": (-log_pi).view(*lead, 1), "scaled_entropy": (-log_pi * entropy_scale).view(*lead, 1)}
+        return act.view(*lead, A), info
+
+    def _qidx(self, pl: Planner, qidx) -> torch.Tensor:
+        if qidx is None:
+            qidx = torch.randperm(self.cfg.num_q, device=pl.device, generator=self._generator())[:2]
+        return torch.as_tensor(qidx, device=pl.device).reshape(2).to(torch.int32).contiguous()
+
+    def Q(self, z, a, task, return_type='min', target=False, detach=False, *, qidx=None):
+        """world_model.py:186-216: 'all' -> logits [num_q, ..., num_bins]; 'min' / 'avg' of two heads -> [..., 1].
+        `detach` reads the online weights (the reference's _detach_Qs shares them); `qidx` (default:
+        randperm(num_q)[:2] from the agent's generator) picks the two heads."""
+        assert return_type in {'min', 'avg', 'all'}
+        pl = self._target_kernels() if target else self._kernels()
+        lead = z.shape[:-1]
+        qi = None if return_type == 'all' else self._qidx(pl, qidx)
+        out = pl.wm_q(self._rows(pl, z), self._rows(pl, a), self._task_rows(pl, task, lead), target, return_type, qi)
+        return out.view(self.cfg.num_q, *lead, -1) if return_type == 'all' else out.view(*lead, 1)
+
+    def td_target(self, next_z, reward, terminated, task, *, eps=None, qidx=None):
+        """TDMPC2._td_target (tdmpc2.py:242-257) in one launch: reward + discount * (1 - terminated) *
+        Q(next_z, pi(next_z), 'min', target=True).  Draws like the reference: pi's noise, then the Q heads."""
+        pl = self._target_kernels()
+        lead, A = next_z.shape[:-1], self.cfg.action_dim
+        if eps is None:
+            eps = torch.randn(*lead, A, device=pl.device, generator=self._generator())
+        qi = self._qidx(pl, qidx)
+        out = pl.td_target(self._rows(pl, next_z), self._rows(pl, reward), self._rows(pl, terminated),
+                           self._task_rows(pl, task, lead), self._rows(pl, eps), qi)
+        return out.view(*lead, 1)
 
 
 def convert_legacy_checkpoint(target_state_dict, source_state_dict):
