@@ -25,7 +25,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from tdmpc2_b200.config import workload            # noqa: E402
-from tdmpc2_b200.synth import synth_state_dict, state_dict_checksum  # noqa: E402
+from tdmpc2_b200.synth import synth_state_dict, state_dict_checksum, trained_scale  # noqa: E402
 from oracle import ref_harness as rh               # noqa: E402
 
 # name -> (workload, overrides, weight seed, perturb, emb_scale, [(t0, eval_mode, task, noise seed), ...])
@@ -57,7 +57,13 @@ CASES = {
     "tiny_knobs": ("tiny", {"num_samples": 200, "num_elites": 7, "num_pi_trajs": 5, "temperature": 2.0, "min_std": 0.1,
                             "max_std": 1.5, "num_q": 5, "iterations": 4, "num_bins": 51, "vmin": -5, "vmax": 5}, 17, True, 1.0,
                    [(True, False, None, 520), (False, False, None, 521), (False, True, None, 522)]),
+    # trained-scale weights (synth.trained_scale, level and seed in TRAINED): peaked two-hot heads, saturated policy,
+    # refits dominated by one elite and clamped to min_std -- branches the init-scale cases never reach
+    "tiny_sharp": ("tiny", {}, 18, True, 1.0,
+                   [(True, False, None, 530), (False, False, None, 531), (False, True, None, 532)]),
 }
+TRAINED = {"tiny_sharp": ("sharp", 218)}     # name -> (trained_scale level, seed)
+OBS_SCALE = {"tiny_sharp": 30.0}
 
 
 def main(only=None):
@@ -69,6 +75,8 @@ def main(only=None):
         t = time.time()
         cfg = workload(wl, **over)
         sd = synth_state_dict(cfg, seed=wseed, perturb=perturb, emb_scale=emb_scale)
+        if name in TRAINED:
+            sd = trained_scale(cfg, sd, *TRAINED[name])
         term_bias = None
         if cfg.episodic:      # synthetic termination logits all share one sign: centre them (see balance_termination)
             from oracle.plan_oracle import balance_termination
@@ -82,10 +90,13 @@ def main(only=None):
                    torch_version=torch.__version__)
         if term_bias is not None:
             rec["term_bias"] = term_bias
+        if name in TRAINED:
+            rec["trained_level"], rec["trained_seed"] = TRAINED[name]
+            rec["obs_scale"] = OBS_SCALE[name]
         prev_mean = torch.zeros(cfg.horizon, cfg.action_dim)
         for i, (t0, ev, task, seed) in enumerate(calls):
             obs = (torch.randint(0, 256, tuple(cfg.obs_shape["rgb"]), generator=g).float() if rgb
-                   else torch.randn(obs_dim, generator=g))
+                   else torch.randn(obs_dim, generator=g) * OBS_SCALE.get(name, 1.0))
             out = rh.run_plan(agent, obs, seed=seed, t0=t0, eval_mode=ev, task=task, prev_mean=prev_mean)
             rec.update({f"c{i}_obs": obs.numpy(), f"c{i}_t0": t0, f"c{i}_eval_mode": ev,
                         f"c{i}_task": -1 if task is None else task, f"c{i}_seed": seed,

@@ -122,9 +122,11 @@ def two_hot_inv(x: torch.Tensor, cfg) -> torch.Tensor:
 class OracleModel:
     """Functional restatement of the reference WorldModel's planning methods."""
 
-    def __init__(self, cfg, sd: Dict[str, torch.Tensor]):
+    def __init__(self, cfg, sd: Dict[str, torch.Tensor], dtype: torch.dtype = torch.float32):
+        """dtype: fp32 (the reference's arithmetic) or torch.float64 (an error yardstick for fp32 results)."""
         self.cfg = cfg
-        self.sd = {k: (v.detach().float().cpu() if isinstance(v, torch.Tensor) else v) for k, v in sd.items()}
+        self.dtype = dtype
+        self.sd = {k: (v.detach().to(dtype).cpu() if isinstance(v, torch.Tensor) else v) for k, v in sd.items()}
         self.log_std_min = self.sd["log_std_min"]
         self.log_std_dif = self.sd["log_std_dif"]
 
@@ -171,7 +173,7 @@ class OracleModel:
         """layers.conv (layers.py:136-150) on obs [n, C, 64, 64]: ShiftAug (:36-59) with its randint made explicit
         (`shift` [n, 2], values 0..6), PixelPreprocess (:62-71), 4 x Conv2d (+ ReLU between), Flatten, SimNorm."""
         pad = 3
-        x = obs.float()
+        x = obs.to(self.dtype)
         n, _, h, w = x.size()
         assert h == w == 64                                                          # layers.py:141
         x = F.pad(x, (pad,) * 4, "replicate")
@@ -233,22 +235,23 @@ class OracleModel:
 
 
 # --------------------------------------------------------------------------- planner
-def _discount(cfg, task: Optional[int]) -> float:
+def _discount(cfg, task: Optional[int], dtype: torch.dtype = torch.float32) -> float:
     frac_of = lambda ep: ep / cfg.discount_denom
     d = lambda ep: min(max((frac_of(ep) - 1) / frac_of(ep), cfg.discount_min), cfg.discount_max)
     if cfg.multitask:
-        return torch.tensor([d(ep) for ep in cfg.episode_lengths], dtype=torch.float32)[task]
+        return torch.tensor([d(ep) for ep in cfg.episode_lengths], dtype=dtype)[task]
     return d(cfg.episode_length)
 
 
 def estimate_value(model: OracleModel, z, actions, task, eps_pi, qidx, info: Optional[dict] = None):
     """tdmpc2.py:122-136.  `info` (test aid, not in the reference) receives `term_margin` [N]: the smallest
     |termination logit| a sample saw, so parity tests can skip samples that sit on the 0.5 decision boundary."""
-    cfg = model.cfg
+    cfg, dt = model.cfg, model.dtype
+    z, actions, eps_pi = z.to(dt), actions.to(dt), eps_pi.to(dt)
     G, discount = 0, 1
-    termination = torch.zeros(z.shape[0], 1, dtype=torch.float32)
-    margin = torch.full((z.shape[0],), float("inf"))
-    gamma = _discount(cfg, task)
+    termination = torch.zeros(z.shape[0], 1, dtype=dt)
+    margin = torch.full((z.shape[0],), float("inf"), dtype=dt)
+    gamma = _discount(cfg, task, dt)
     for t in range(cfg.horizon):
         reward = two_hot_inv(model.reward(z, actions[t], task), cfg)
         z = model.next(z, actions[t], task)
@@ -299,33 +302,34 @@ class PlanTrace:
 
 @torch.no_grad()
 def plan_one(model: OracleModel, obs, task, t0: bool, prev_mean, noise: PlanNoise, eval_mode: bool):
-    """One reference `_plan` call (tdmpc2.py:138-206) with explicit noise; E == 1."""
-    cfg = model.cfg
+    """One reference `_plan` call (tdmpc2.py:138-206) with explicit noise; E == 1.  Runs in `model.dtype`."""
+    cfg, dt = model.cfg, model.dtype
+    obs, prev_mean = obs.to(dt), prev_mean.to(dt)
     H, N, P, A, K = cfg.horizon, cfg.num_samples, cfg.num_pi_trajs, cfg.action_dim, cfg.num_elites
     if cfg.get("obs", "state") == "rgb":
         z = model.encode(obs.unsqueeze(0), task, noise.shift[0:1])                   # tdmpc2.py:111 unsqueezes; :153 encodes
     else:
         z = model.encode(obs.view(1, -1), task)
     z0 = z
-    pi_actions = torch.zeros(H, P, A)
+    pi_actions = torch.zeros(H, P, A, dtype=dt)
     if P > 0:
         _z = z.repeat(P, 1)
         for t in range(H - 1):
-            pi_actions[t] = model.pi(_z, task, noise.prior[0, t])
+            pi_actions[t] = model.pi(_z, task, noise.prior[0, t].to(dt))
             _z = model.next(_z, pi_actions[t], task)
-        pi_actions[-1] = model.pi(_z, task, noise.prior[0, H - 1])
+        pi_actions[-1] = model.pi(_z, task, noise.prior[0, H - 1].to(dt))
     z = z.repeat(N, 1)
-    mean = torch.zeros(H, A)
-    std = torch.full((H, A), float(cfg.max_std), dtype=torch.float)
+    mean = torch.zeros(H, A, dtype=dt)
+    std = torch.full((H, A), float(cfg.max_std), dtype=dt)
     if not t0:
         mean[:-1] = prev_mean[1:]
-    actions = torch.empty(H, N, A)
+    actions = torch.empty(H, N, A, dtype=dt)
     if P > 0:
         actions[:, :P] = pi_actions
     mask = model.sd["_action_masks"][task] if cfg.multitask else None
     vals, idxs, means, stds, margins = [], [], [], [], []
     for it in range(cfg.iterations):
-        r = noise.r[0, it]
+        r = noise.r[0, it].to(dt)
         actions_sample = mean.unsqueeze(1) + std.unsqueeze(1) * r
         actions_sample = actions_sample.clamp(-1, 1)
         actions[:, P:] = actions_sample
@@ -349,12 +353,12 @@ def plan_one(model: OracleModel, obs, task, t0: bool, prev_mean, noise: PlanNois
         vals.append(value.squeeze(1)); idxs.append(elite_idxs); means.append(mean); stds.append(std)
     # gumbel pick, math.py:86-94 with the exponential draw made explicit
     logits = score.squeeze(1).log()
-    gumbels = -noise.expo[0].log()
+    gumbels = -noise.expo[0].to(dt).log()
     y_soft = ((logits + gumbels) / 1.0).softmax(0)
     rand_idx = y_soft.argmax(-1)
     a = elite_actions[0, rand_idx]
     if not eval_mode:
-        a = a + std[0] * noise.final[0]
+        a = a + std[0] * noise.final[0].to(dt)
     out = dict(action=a.clamp(-1, 1), mean=mean, std=std, z=z0[0], pi_actions=pi_actions,
                values=torch.stack(vals), elite_idx=torch.stack(idxs), iter_mean=torch.stack(means),
                iter_std=torch.stack(stds), score=score.squeeze(1), pick=rand_idx)
@@ -365,11 +369,12 @@ def plan_one(model: OracleModel, obs, task, t0: bool, prev_mean, noise: PlanNois
 
 @torch.no_grad()
 def plan_oracle(cfg, sd, obs, task=None, t0=None, prev_mean=None, noise: PlanNoise = None,
-                eval_mode: bool = False) -> PlanTrace:
+                eval_mode: bool = False, dtype: torch.dtype = torch.float32) -> PlanTrace:
     """Env-batched planner: obs [E, obs_dim], task [E] or None, t0 [E] bool,
-    prev_mean [E, H, A]; loops the E independent reference plans."""
-    model = sd if isinstance(sd, OracleModel) else OracleModel(cfg, sd)
-    obs = torch.as_tensor(obs, dtype=torch.float32)
+    prev_mean [E, H, A]; loops the E independent reference plans.  `dtype` applies when `sd` is a state dict; an
+    OracleModel brings its own."""
+    model = sd if isinstance(sd, OracleModel) else OracleModel(cfg, sd, dtype)
+    obs = torch.as_tensor(obs, dtype=model.dtype)
     E = obs.shape[0]
     if t0 is None:
         t0 = [True] * E

@@ -64,30 +64,32 @@ def attach_target_qs(agent, sd: Dict[str, torch.Tensor]) -> None:
 
 
 class WMOracle(OracleModel):
-    """Row-wise restatement of the reference WorldModel's inference methods (fp32, CPU)."""
+    """Row-wise restatement of the reference WorldModel's inference methods (CPU; fp32 unless `dtype` says otherwise).
+    Inputs are cast to the model's dtype."""
 
     def _emb(self, task: torch.Tensor) -> torch.Tensor:
-        rows = [self.task_emb(torch.zeros(1, 0), t)[0] for t in range(self.sd["_task_emb.weight"].shape[0])]
+        rows = [self.task_emb(torch.zeros(1, 0, dtype=self.dtype), t)[0] for t in range(self.sd["_task_emb.weight"].shape[0])]
         return torch.stack(rows)[task.long()]                  # nn.Embedding(max_norm=1) lookup, world_model.py:21
 
     def _cat(self, x, task):
         return torch.cat([x, self._emb(task)], dim=-1) if self.cfg.multitask else x
 
     def encode(self, obs, task):
-        return self._mlp("_encoder.state", self._cat(obs, task), "simnorm")
+        return self._mlp("_encoder.state", self._cat(obs.to(self.dtype), task), "simnorm")
 
     def next(self, z, a, task):
-        return self._mlp("_dynamics", torch.cat([self._cat(z, task), a], dim=-1), "simnorm")
+        return self._mlp("_dynamics", torch.cat([self._cat(z.to(self.dtype), task), a.to(self.dtype)], dim=-1), "simnorm")
 
     def reward(self, z, a, task):
-        return self._mlp("_reward", torch.cat([self._cat(z, task), a], dim=-1), "none")
+        return self._mlp("_reward", torch.cat([self._cat(z.to(self.dtype), task), a.to(self.dtype)], dim=-1), "none")
 
     def termination(self, z, task=None, unnormalized=False):
-        x = self._mlp("_termination", z, "none")
+        x = self._mlp("_termination", z.to(self.dtype), "none")
         return x if unnormalized else torch.sigmoid(x)
 
     def pi(self, z, task, eps):
         """world_model.py:144-184 -> (action, info)."""
+        z, eps = z.to(self.dtype), eps.to(self.dtype)
         mean, log_std = self._mlp("_pi", self._cat(z, task), "none").chunk(2, dim=-1)
         log_std = self.log_std_min + 0.5 * self.log_std_dif * (torch.tanh(log_std) + 1)         # math.py:12-13
         if self.cfg.multitask:
@@ -107,7 +109,7 @@ class WMOracle(OracleModel):
 
     def Q(self, z, a, task, return_type="min", target=False, qidx=None):
         """world_model.py:186-216; detach=True reads the online weights (same tensors)."""
-        x = torch.cat([self._cat(z, task), a], dim=-1)
+        x = torch.cat([self._cat(z.to(self.dtype), task), a.to(self.dtype)], dim=-1)
         prefix = TARGET[:-1] if target else QS[:-1]
         out = torch.stack([self._mlp(prefix, x, "none", head=h) for h in range(self.cfg.num_q)])
         if return_type == "all":
@@ -117,8 +119,10 @@ class WMOracle(OracleModel):
 
     def td_target(self, next_z, reward, terminated, task, eps, qidx):
         """tdmpc2.py:255-257."""
+        reward, terminated = reward.to(self.dtype), terminated.to(self.dtype)
         action, _ = self.pi(next_z, task, eps)
-        discount = _discount(self.cfg, task.long()).unsqueeze(-1) if self.cfg.multitask else _discount(self.cfg, None)
+        discount = (_discount(self.cfg, task.long(), self.dtype).unsqueeze(-1) if self.cfg.multitask
+                    else _discount(self.cfg, None))
         return reward + discount * (1 - terminated) * self.Q(next_z, action, task, "min", target=True, qidx=qidx)
 
 
@@ -130,6 +134,12 @@ CASES = {
     "tiny_episodic_wm": ("tiny", {"episodic": True}, 23, 123, 1.0, 3, 50, 620),
     "c1_dog5m_wm": ("c1", {}, 24, 124, 1.0, 3, 10, 630),           # 512-wide rows: the register LayerNorm path
 }
+# Trained-scale cases (same fields), kept apart from CASES because fixed fp32 tolerances do not apply to them:
+# TRAINED gives the synth.trained_scale (level, seed) applied after the target blend -- peaked two-hot heads with values
+# of 1e3 - 1e4, saturated tanh, log-stds at their bounds
+TRAINED_CASES = {"c1_sharp_wm": ("c1", {}, 25, 125, 1.0, 3, 10, 640)}
+TRAINED = {"c1_sharp_wm": ("sharp", 225)}
+OBS_SCALE = {"c1_sharp_wm": 30.0}
 SUB_B = 8            # 'all' logits are recorded for batch columns [0, SUB_B) to keep the fixtures small
 
 
@@ -137,19 +147,23 @@ def case_model(name):
     """(cfg, state dict with a blended target ensemble) of a golden case."""
     from tdmpc2_b200.config import workload
     from tdmpc2_b200.synth import synth_state_dict
-    wl, over, wseed, tseed, emb_scale, H, B, _ = CASES[name]
+    wl, over, wseed, tseed, emb_scale, H, B, _ = {**CASES, **TRAINED_CASES}[name]
     cfg = workload(wl, **over)
     sd = synth_state_dict(cfg, seed=wseed, perturb=True, emb_scale=emb_scale)
     if cfg.episodic:
         from oracle.plan_oracle import balance_termination
         balance_termination(cfg, sd)
-    return cfg, with_target_blend(cfg, sd, tseed)
+    sd = with_target_blend(cfg, sd, tseed)
+    if name in TRAINED:
+        from tdmpc2_b200.synth import trained_scale
+        sd = trained_scale(cfg, sd, *TRAINED[name])
+    return cfg, sd
 
 
-def case_inputs(cfg, H, B, seed):
+def case_inputs(cfg, H, B, seed, obs_scale=1.0):
     """obs [H, B, obs_dim], a [H, B, A], reward / terminated [H, B, 1], task [B] int64 or None."""
     g = torch.Generator().manual_seed(seed)
-    obs = torch.randn(H, B, cfg.obs_shape["state"][0], generator=g)
+    obs = torch.randn(H, B, cfg.obs_shape["state"][0], generator=g) * obs_scale
     a = torch.rand(H, B, cfg.action_dim, generator=g) * 2 - 1
     reward = torch.randn(H, B, 1, generator=g)
     terminated = (torch.rand(H, B, 1, generator=g) < 0.3).float()
@@ -206,15 +220,17 @@ def main(only=None):
     from oracle import ref_harness as rh
     from tdmpc2_b200.synth import state_dict_checksum
     out_dir = os.path.join(ROOT, "tests", "golden")
-    for name, (wl, over, wseed, tseed, emb_scale, H, B, seed) in CASES.items():
+    for name, (wl, over, wseed, tseed, emb_scale, H, B, seed) in {**CASES, **TRAINED_CASES}.items():
         if only and name not in only:
             continue
         t = time.time()
         cfg, sd = case_model(name)
         agent = rh.build_agent(cfg, sd)
         attach_target_qs(agent, sd)
-        obs, a, reward, terminated, task = case_inputs(cfg, H, B, seed)
+        obs, a, reward, terminated, task = case_inputs(cfg, H, B, seed, OBS_SCALE.get(name, 1.0))
         rec = dict(case=name, weight_checksum=state_dict_checksum(sd), torch_version=torch.__version__)
+        if name in TRAINED:
+            rec["trained_level"], rec["trained_seed"] = TRAINED[name]
         # the [H, B] batch (one full 128-row tile and a partial one for B = 50) and one 2-D row
         one = (obs[0, :1], a[0, :1], reward[0, :1], terminated[0, :1], None if task is None else task[:1])
         for pfx, (o, a_, rw, te, tk), s in (("b", (obs, a, reward, terminated, task), seed), ("r", one, seed + 1)):
@@ -233,10 +249,12 @@ def load_case(name):
     from tdmpc2_b200.synth import state_dict_checksum
     f = np.load(os.path.join(ROOT, "tests", "golden", name + ".npz"), allow_pickle=False)
     cfg, sd = case_model(name)
+    if name in TRAINED:
+        assert (str(f["trained_level"]), int(f["trained_seed"])) == TRAINED[name], "fixture minted with another transform"
     chk = state_dict_checksum(sd)
     assert abs(chk - float(f["weight_checksum"])) <= 1e-9 * abs(chk), "synthetic weights differ from the fixture's"
-    wl, over, wseed, tseed, emb_scale, H, B, seed = CASES[name]
-    obs, a, reward, terminated, task = case_inputs(cfg, H, B, seed)
+    wl, over, wseed, tseed, emb_scale, H, B, seed = {**CASES, **TRAINED_CASES}[name]
+    obs, a, reward, terminated, task = case_inputs(cfg, H, B, seed, OBS_SCALE.get(name, 1.0))
     inputs = {"b": (obs, a, reward, terminated, task),
               "r": (obs[0, :1], a[0, :1], reward[0, :1], terminated[0, :1], None if task is None else task[:1])}
     recs = {}

@@ -113,6 +113,103 @@ def synth_state_dict(cfg: Config, seed: int = 1, perturb: bool = False,
     return sd
 
 
+# Logit spread (standard deviation over rows and bins, in units of the layer's fan-in-normalised scale) that each level
+# targets at the reward / Q / termination outputs, and the pre-activation scale of the policy's mean and log-std.  The
+# gains are divided by sigma(W) sqrt(fan_in), so that one level lands in the same regime on every preset: a plain
+# gain that sharpens a 512-wide model leaves a 64-wide one near-uniform.
+TRAINED_LEVELS = {
+    #          two-hot heads, pi mean, pi log-std, termination
+    "mid": dict(twohot=1.15, pi_mean=1.5, pi_log_std=1.5, term=20.0),
+    "sharp": dict(twohot=8.0, pi_mean=12.0, pi_log_std=12.0, term=60.0),
+}
+# Per-preset (Config.task) two-hot spreads where the level's default does not land in its regime: how far trajectory
+# values spread also depends on how much the latent varies between samples, which the fan-in normalisation misses.
+TRAINED_TWOHOT = {("tiny", "mid"): 1.2, ("tiny-mt", "mid"): 3.5, ("tiny-mt", "sharp"): 12.0}
+OUTLIERS_PER_MATRIX = 3
+
+
+def trained_scale(cfg: Config, sd: Dict[str, torch.Tensor], level: str, seed: int) -> Dict[str, torch.Tensor]:
+    """A deterministic transform of a synthetic state dict towards what a trained model looks like, for parity tests
+    beyond the benign initialisation regime:
+
+      * LayerNorm gamma ~ lognormal(0, 0.5), beta ~ N(0, 0.5^2);
+      * reward / Q output layers scaled so that the two-hot softmax is peaked (values reach 1e3 - 1e4 at "sharp");
+      * the policy's mean rows scaled so that tanh saturates, its log-std rows so that log-stds reach their clamp;
+      * the termination output scaled so that logits reach +-20 (re-centre it with balance_termination afterwards);
+      * OUTLIERS_PER_MATRIX entries of every weight matrix (per Q head) set to 30 - 60 x the matrix's sigma, which
+        moves the power-of-two scale the packer gives the matrix by several binades.
+
+    Q-ensemble tensors (online, detach, target) get the same draws, so the online / target difference of the input
+    (e.g. a target blend made before this transform) is kept.  Returns a new dict; `sd` is not modified."""
+    lv = dict(TRAINED_LEVELS[level])
+    lv["twohot"] = TRAINED_TWOHOT.get((cfg.task, level), lv["twohot"])
+    gen = torch.Generator(device="cpu").manual_seed(seed)
+    out = dict(sd)
+    A = cfg.action_dim
+
+    def fan_in_gain(w: torch.Tensor, spread: float) -> float:
+        return spread / (float(w.std()) * w.shape[-1] ** 0.5)
+
+    def per_key(key: str):
+        """Same transform for every copy of a Q-ensemble tensor."""
+        for p in QS_PREFIXES:
+            if key.startswith(p):
+                return "_Qs.params." + key[len(p):]
+        return key
+
+    draws: Dict[str, object] = {}
+
+    def draw(key, make):
+        k = per_key(key)
+        if k not in draws:
+            draws[k] = make()
+        return draws[k]
+
+    for key in sorted(sd):
+        v = sd[key]
+        if not isinstance(v, torch.Tensor) or not v.is_floating_point() or key.startswith(("_task_emb", "_action_masks",
+                                                                                           "log_std", "_encoder.rgb")):
+            continue
+        if key.endswith(".ln.weight"):
+            out[key] = draw(key, lambda: torch.exp(0.5 * torch.randn(v.shape, generator=gen)))
+        elif key.endswith(".ln.bias"):
+            out[key] = draw(key, lambda: 0.5 * torch.randn(v.shape, generator=gen))
+        elif key.endswith(".weight"):
+            def outliers(v=v):
+                w = v.reshape(-1, v.shape[-2] * v.shape[-1])           # one row per Q head
+                pos = torch.stack([torch.randperm(w.shape[1], generator=gen)[:OUTLIERS_PER_MATRIX] for _ in range(w.shape[0])])
+                mag = (30.0 + 30.0 * torch.rand(pos.shape, generator=gen)) * torch.where(
+                    torch.rand(pos.shape, generator=gen) < 0.5, -1.0, 1.0)
+                return pos, mag
+            pos, mag = draw(key, outliers)
+            w = v.detach().clone().reshape(-1, v.shape[-2] * v.shape[-1])
+            sigma = w.std(dim=1, keepdim=True)
+            w.scatter_(1, pos, mag * sigma)
+            out[key] = w.reshape(v.shape)
+    # output-layer gains (after the outliers, so that sigma(W) includes them as a trained matrix's would)
+    def gain(prefix: str, spread: float, rows=slice(None)):
+        w = out[prefix + ".weight"]
+        heads = w.reshape(-1, *w.shape[-2:])
+        g = torch.ones(heads.shape[:2])
+        for h in range(heads.shape[0]):
+            g[h, rows] = fan_in_gain(heads[h][rows], spread)
+        g = g.reshape(w.shape[:-1])
+        out[prefix + ".weight"] = w * g.unsqueeze(-1)
+        out[prefix + ".bias"] = out[prefix + ".bias"] * g
+    if cfg.num_bins > 1:
+        gain("_reward.2", lv["twohot"])
+        for p in ("_Qs.params.", "_target_Qs_params."):
+            gain(p + "2", lv["twohot"])
+    gain("_pi.2", lv["pi_mean"], slice(0, A))
+    gain("_pi.2", lv["pi_log_std"], slice(A, 2 * A))
+    if cfg.episodic:
+        gain("_termination.2", lv["term"])
+    for k in sd:
+        if k.startswith("_detach_Qs_params."):          # shares the online tensors, as in the reference (world_model.py:40)
+            out[k] = out["_Qs.params." + k[len("_detach_Qs_params."):]]
+    return out
+
+
 def state_dict_checksum(sd: Dict[str, torch.Tensor]) -> float:
     """Order-independent fingerprint used by golden fixtures to detect RNG drift."""
     tot = 0.0

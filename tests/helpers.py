@@ -17,6 +17,9 @@ def load_golden(name):
     cfg = workload(str(f["workload"]), **over)
     sd = synth_state_dict(cfg, seed=int(f["weight_seed"]), perturb=bool(f["perturb"]),
                           emb_scale=float(f["emb_scale"]))
+    if "trained_level" in f.files:  # trained-scale fixtures: the synth.trained_scale transform they were minted with
+        from tdmpc2_b200.synth import trained_scale
+        sd = trained_scale(cfg, sd, str(f["trained_level"]), int(f["trained_seed"]))
     if "term_bias" in f.files:      # episodic fixtures: the calibrated termination bias they were minted with
         sd["_termination.2.bias"] = torch.full_like(sd["_termination.2.bias"], float(f["term_bias"]))
     chk = state_dict_checksum(sd)
@@ -32,6 +35,48 @@ def load_golden(name):
                           mean=torch.from_numpy(g("mean")), values=torch.from_numpy(g("values")),
                           elite_idx=torch.from_numpy(g("elite_idx"))))
     return cfg, sd, calls
+
+
+OBS_SCALES = (1.0, 30.0, 1e3)
+OBS_BIG = 6e4          # one observation column near the top of fp16's range (the kernels clamp activations to +-65000)
+
+
+def trained_model(wl, level, seed, **over):
+    """(cfg, state dict) of a trained-scale model: synthetic weights (seed), a blended target ensemble (seed + 100),
+    synth.trained_scale(level, seed + 200) and, for episodic models, a re-centred termination bias."""
+    from oracle.plan_oracle import balance_termination
+    from oracle.wm_oracle import with_target_blend
+    from tdmpc2_b200.synth import trained_scale
+    cfg = workload(wl, **over)
+    sd = synth_state_dict(cfg, seed=seed, perturb=True, emb_scale=60.0 if cfg.multitask else 1.0)
+    sd = trained_scale(cfg, with_target_blend(cfg, sd, seed + 100), level, seed + 200)
+    if cfg.episodic:
+        balance_termination(cfg, sd)
+    return cfg, sd
+
+
+def trained_obs(cfg, rows, seed):
+    """[rows, obs_dim] observations whose rows cycle through the scales OBS_SCALES and a fourth kind: scale 1 with
+    column 0 near +-OBS_BIG (it dominates the encoder's first LayerNorm, so only one row in four carries it)."""
+    g = torch.Generator().manual_seed(seed)
+    obs = torch.randn(rows, cfg.obs_shape["state"][0], generator=g)
+    kind = torch.arange(rows) % (len(OBS_SCALES) + 1)
+    obs *= torch.tensor(OBS_SCALES + (1.0,))[kind].unsqueeze(1)
+    big = OBS_BIG * (0.9 + 0.1 * torch.rand(rows, generator=g)) * torch.where(torch.rand(rows, generator=g) < 0.5, -1.0, 1.0)
+    obs[:, 0] = torch.where(kind == len(OBS_SCALES), big, obs[:, 0])
+    return obs
+
+
+def refit_stats(cfg, tr):
+    """Per (env, iteration) of an oracle PlanTrace: the largest normalised elite weight, and whether the refit clamped
+    some std to min_std."""
+    top = torch.gather(tr.values, -1, tr.elite_idx)                          # [E, I, K] elite values, sorted
+    w = torch.softmax(cfg.temperature * (top - top[..., :1]).double(), -1)   # the refit's score
+    live = torch.ones_like(tr.iter_std, dtype=torch.bool)
+    if cfg.multitask:
+        live = tr.iter_std > 0                                               # masked action dims are zeroed after the clamp
+    clamped = ((tr.iter_std == torch.tensor(cfg.min_std, dtype=tr.iter_std.dtype)) & live).flatten(2).any(-1)
+    return w.max(-1).values, clamped
 
 
 def stable_positions(values, k, tol):
