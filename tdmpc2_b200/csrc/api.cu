@@ -114,14 +114,60 @@ struct LayerHost {
   size_t off_hi, off_lo, off_bias, off_g, off_b;   // byte offsets into the packed blob
 };
 
-// Target Q ensemble (_target_Qs_params.*, world_model.py:41): its own caller-owned blob, so that a planner that never
-// runs a target op keeps its packed_bytes.  Same layer shapes as the online heads; own weight maps (tmW[base_map + m]).
-struct TargetQ {
-  std::vector<LayerHost> layers;   // 3 * num_q, head h layer l at 3 h + l
-  int nmaps = 0, base_map = 0;
+// Byte layout of a packed weight blob: layer table | absmax slots | per-layer vectors | `extra` bytes of the caller |
+// one 1024-aligned weight map per Kpad class, map m read through the TMA map tmW[base_map + m].
+struct BlobLayout {
+  int base_map = 0, nmaps = 0;
   int map_kpad[kMaxWMaps], map_rows[kMaxWMaps];
   size_t map_off[kMaxWMaps];
-  size_t off_table = 0, off_absmax = 0, bytes = 0;   // bytes == 0: the model's maps leave no room (target ops unsupported)
+  size_t off_table = 0, off_absmax = 0, off_extra = 0, bytes = 0;
+};
+
+// Assigns the weight maps of `layers` (a new class per new Kpad, numbered from base_map), their rows in those maps and
+// every byte offset.  false: the classes do not fit the kMaxWMaps TMA maps (`b` is then empty).
+static bool layout_blob(std::vector<LayerHost>& layers, int base_map, size_t extra, BlobLayout& b) {
+  b = BlobLayout{};
+  b.base_map = base_map;
+  for (auto& l : layers) {
+    int m = 0;
+    while (m < b.nmaps && b.map_kpad[m] != l.Kpad) ++m;
+    if (m == b.nmaps) {
+      if (base_map + b.nmaps == kMaxWMaps) { b = BlobLayout{}; return false; }
+      b.map_kpad[m] = l.Kpad;
+      b.map_rows[m] = 0;
+      ++b.nmaps;
+    }
+    l.wmap = base_map + m;
+    l.wrow = b.map_rows[m];
+    b.map_rows[m] += 2 * l.Npad;
+  }
+  size_t off = 0;
+  b.off_table = off; off = align_up(off + layers.size() * sizeof(LayerDev), 256);
+  b.off_absmax = off; off = align_up(off + layers.size() * sizeof(unsigned), 256);
+  for (auto& l : layers) {
+    l.off_bias = off; off = align_up(off + l.Npad * 4, 256);
+    l.off_g = off; off = align_up(off + l.Npad * 4, 256);
+    l.off_b = off; off = align_up(off + l.Npad * 4, 256);
+  }
+  b.off_extra = off; off += extra;
+  for (int m = 0; m < b.nmaps; ++m) {
+    off = align_up(off, 1024);
+    b.map_off[m] = off;
+    off += static_cast<size_t>(b.map_rows[m]) * b.map_kpad[m] * 2;
+  }
+  b.bytes = align_up(off, 1024);
+  for (auto& l : layers) {
+    l.off_hi = b.map_off[l.wmap - base_map] + static_cast<size_t>(l.wrow) * l.Kpad * 2;
+    l.off_lo = l.off_hi + static_cast<size_t>(l.Npad) * l.Kpad * 2;
+  }
+  return true;
+}
+
+// Target Q ensemble (_target_Qs_params.*, world_model.py:41): its own caller-owned blob, so that a planner that never
+// runs a target op keeps its packed_bytes.  Same layer shapes as the online heads; its maps follow the online ones.
+struct TargetQ {
+  std::vector<LayerHost> layers;   // 3 * num_q, head h layer l at 3 h + l
+  BlobLayout lay;                  // lay.bytes == 0: the model's maps leave no room (target ops unsupported)
   uint8_t* blob = nullptr;
   bool packed = false;
 };
@@ -131,13 +177,10 @@ struct tdmpc2_planner {
   int num_sms = 0, nslots = 0;
   std::vector<LayerHost> layers;
   int li_enc = 0, li_dyn = 0, li_rew = 0, li_pi = 0, li_q = 0, li_term = -1, num_enc = 0;
-  int nmaps = 0;
-  int map_kpad[kMaxWMaps];
-  int map_rows[kMaxWMaps];
-  size_t map_off[kMaxWMaps];
   int KpadX = 0, KpadH = 0, NpadMax = 0, Ppad = 1, tiles_per_env = 0;
-  // packed blob offsets
-  size_t off_table = 0, off_absmax = 0, off_emb = 0, off_masks = 0, off_disc = 0, off_bins = 0, packed_bytes = 0;
+  // packed blob: the layers' layout, then the extra vectors in its `extra` bytes
+  BlobLayout lay;
+  size_t off_emb = 0, off_masks = 0, off_disc = 0, off_bins = 0;
   // workspace offsets
   size_t off_X = 0, off_H = 0, off_raw = 0, off_z = 0, off_pia = 0, off_mean = 0, off_std = 0, off_values = 0,
          off_counter = 0, off_score = 0, off_eact = 0, off_eidx = 0, off_zbias = 0, ws_bytes = 0;
@@ -156,25 +199,6 @@ struct tdmpc2_planner {
   const int32_t* cur_task = nullptr;
   long long* prof = nullptr;
 };
-
-static int add_layer(tdmpc2_planner* p, int K, int N, bool has_ln) {
-  LayerHost l{};
-  l.K = K; l.Kpad = pad_to(K, kKch); l.N = N; l.Npad = pad_to(N, 128); l.has_ln = has_ln ? 1 : 0;
-  l.src_n = N; l.split_at = N; l.split_to = N;
-  int m = -1;
-  for (int i = 0; i < p->nmaps; ++i) if (p->map_kpad[i] == l.Kpad) m = i;
-  if (m < 0) {
-    if (p->nmaps == kMaxWMaps) return -1;
-    m = p->nmaps++;
-    p->map_kpad[m] = l.Kpad;
-    p->map_rows[m] = 0;
-  }
-  l.wmap = m;
-  l.wrow = p->map_rows[m];
-  p->map_rows[m] += 2 * l.Npad;
-  p->layers.push_back(l);
-  return static_cast<int>(p->layers.size()) - 1;
-}
 
 extern "C" int tdmpc2_abi_version(void) { return TDMPC2_B200_ABI_VERSION; }
 extern "C" const char* tdmpc2_last_error(void) { return g_err.c_str(); }
@@ -229,8 +253,13 @@ extern "C" int tdmpc2_planner_create(const tdmpc2_dims* dims, tdmpc2_planner** o
   p->nslots = num_sms;
   const int L = d.latent_dim, M = d.mlp_dim, A = d.action_dim, T = d.task_dim, B = d.num_bins;
   const int D = L + T + A;
-  bool ok = true;
-  auto add = [&](int K, int N, bool ln) { int i = add_layer(p, K, N, ln); if (i < 0) ok = false; return i; };
+  auto add = [&](int K, int N, bool ln) {
+    LayerHost l{};
+    l.K = K; l.Kpad = pad_to(K, kKch); l.N = N; l.Npad = pad_to(N, 128); l.has_ln = ln ? 1 : 0;
+    l.src_n = N; l.split_at = N; l.split_to = N;
+    p->layers.push_back(l);
+    return static_cast<int>(p->layers.size()) - 1;
+  };
   // encoder: mlp(obs+T, n_hidden*[enc_dim], L, act=SimNorm)  (layers.py:157-159); num_enc_layers == 0: the model has no
   // state encoder (pixel observations: tdmpc2_pixel_encode + tdmpc2_plan_prologue_latent supply the latent)
   p->num_enc = d.num_enc_layers == 0 ? 0 : n_hidden + 1;
@@ -243,14 +272,27 @@ extern "C" int tdmpc2_planner_create(const tdmpc2_dims* dims, tdmpc2_planner** o
     // pi head: rows [0, A) = mean logits, rows [A, 2A) = log_std logits, the latter moved to column pad32(A)
     const int Apad = pad_to(A, 32);
     const int i = add(M, Apad + A, false);
-    if (i >= 0) { p->layers[i].src_n = 2 * A; p->layers[i].split_at = A; p->layers[i].split_to = Apad; }
+    p->layers[i].src_n = 2 * A; p->layers[i].split_at = A; p->layers[i].split_to = Apad;
   }
   p->li_q = static_cast<int>(p->layers.size());
   for (int h = 0; h < d.num_q; ++h) { add(D, M, true); add(M, M, true); add(M, B, false); }
   // termination head: mlp(L+T, 2*[M], 1) on z_{t+1}  (world_model.py:28); appended so the other layer indices stay put
   p->li_term = -1;
   if (d.episodic) { p->li_term = static_cast<int>(p->layers.size()); add(L + T, M, true); add(M, M, true); add(M, 1, false); }
-  if (!ok) { delete p; return fail(TDMPC2_ERR_INVALID, "more than %d distinct padded input widths", kMaxWMaps); }
+
+  // ---- packed blob layout; the extra vectors sit between the per-layer vectors and the weight maps
+  const size_t emb_bytes = align_up(static_cast<size_t>(d.num_tasks) * std::max(T, 1) * 4, 256);
+  const size_t mask_bytes = align_up(static_cast<size_t>(d.num_tasks) * A * 4, 256);
+  const size_t disc_bytes = align_up(static_cast<size_t>(d.num_tasks) * (d.horizon + 1) * 4, 256);
+  const size_t bins_bytes = align_up(static_cast<size_t>(B) * 4, 256);
+  if (!layout_blob(p->layers, 0, emb_bytes + mask_bytes + disc_bytes + bins_bytes, p->lay)) {
+    delete p;
+    return fail(TDMPC2_ERR_INVALID, "more than %d distinct padded input widths", kMaxWMaps);
+  }
+  p->off_emb = p->lay.off_extra;
+  p->off_masks = p->off_emb + emb_bytes;
+  p->off_disc = p->off_masks + mask_bytes;
+  p->off_bins = p->off_disc + disc_bytes;
 
   p->KpadX = std::max(pad_to(D, kKch), pad_to(d.obs_dim + T, kKch));
   p->KpadH = std::max(pad_to(M, kKch), pad_to(d.enc_dim, kKch));
@@ -260,32 +302,9 @@ extern "C" int tdmpc2_planner_create(const tdmpc2_dims* dims, tdmpc2_planner** o
   while (p->Ppad < d.num_pi_trajs) p->Ppad <<= 1;
   p->tiles_per_env = (d.num_samples + kTileM - 1) / kTileM;
 
-  // ---- packed blob layout
-  size_t off = 0;
-  p->off_table = off; off = align_up(off + p->layers.size() * sizeof(LayerDev), 256);
-  p->off_absmax = off; off = align_up(off + p->layers.size() * sizeof(unsigned), 256);
-  for (auto& l : p->layers) {
-    l.off_bias = off; off = align_up(off + l.Npad * 4, 256);
-    l.off_g = off; off = align_up(off + l.Npad * 4, 256);
-    l.off_b = off; off = align_up(off + l.Npad * 4, 256);
-  }
-  p->off_emb = off; off = align_up(off + static_cast<size_t>(d.num_tasks) * std::max(T, 1) * 4, 256);
-  p->off_masks = off; off = align_up(off + static_cast<size_t>(d.num_tasks) * A * 4, 256);
-  p->off_disc = off; off = align_up(off + static_cast<size_t>(d.num_tasks) * (d.horizon + 1) * 4, 256);
-  p->off_bins = off; off = align_up(off + static_cast<size_t>(B) * 4, 256);
-  for (int m = 0; m < p->nmaps; ++m) {
-    off = align_up(off, 1024);
-    p->map_off[m] = off;
-    off += static_cast<size_t>(p->map_rows[m]) * p->map_kpad[m] * 2;
-  }
-  p->packed_bytes = align_up(off, 1024);
-  for (auto& l : p->layers) {
-    l.off_hi = p->map_off[l.wmap] + static_cast<size_t>(l.wrow) * l.Kpad * 2;
-    l.off_lo = l.off_hi + static_cast<size_t>(l.Npad) * l.Kpad * 2;
-  }
   // ---- workspace layout
   const size_t E = d.num_envs, H = d.horizon, N = d.num_samples, K = d.num_elites, P = d.num_pi_trajs;
-  off = 0;
+  size_t off = 0;
   p->off_X = off; off = align_up(off + static_cast<size_t>(p->nslots) * 2 * kTileM * p->KpadX * 2, 1024);
   p->off_H = off; off = align_up(off + static_cast<size_t>(p->nslots) * 2 * kTileM * p->KpadH * 2, 1024);
   p->off_raw = off; off = align_up(off + static_cast<size_t>(p->nslots) * kTileM * p->NpadMax * 4, 1024);
@@ -304,48 +323,10 @@ extern "C" int tdmpc2_planner_create(const tdmpc2_dims* dims, tdmpc2_planner** o
   p->off_zbias = off; off = align_up(off + 2 * E * static_cast<size_t>(p->zb_pitch) * 4, 256);
   p->ws_bytes = align_up(off, 1024);
 
-  // ---- target Q blob layout: table | absmax | per-layer vectors | one weight map per Kpad class of the online heads
+  // ---- target Q blob: copies of the online heads' layers, with weight maps of their own after the online ones
   TargetQ& tq = p->tq;
-  tq.base_map = p->nmaps;
-  bool tq_ok = true;
-  for (int h = 0; h < d.num_q && tq_ok; ++h)
-    for (int l = 0; l < 3; ++l) {
-      LayerHost t = p->layers[p->li_q + 3 * h + l];
-      int m = -1;
-      for (int i = 0; i < tq.nmaps; ++i) if (tq.map_kpad[i] == t.Kpad) m = i;
-      if (m < 0) {
-        if (tq.base_map + tq.nmaps == kMaxWMaps) { tq_ok = false; break; }
-        m = tq.nmaps++;
-        tq.map_kpad[m] = t.Kpad;
-        tq.map_rows[m] = 0;
-      }
-      t.wmap = tq.base_map + m;
-      t.wrow = tq.map_rows[m];
-      tq.map_rows[m] += 2 * t.Npad;
-      tq.layers.push_back(t);
-    }
-  if (tq_ok) {
-    off = 0;
-    tq.off_table = off; off = align_up(off + tq.layers.size() * sizeof(LayerDev), 256);
-    tq.off_absmax = off; off = align_up(off + tq.layers.size() * sizeof(unsigned), 256);
-    for (auto& l : tq.layers) {
-      l.off_bias = off; off = align_up(off + l.Npad * 4, 256);
-      l.off_g = off; off = align_up(off + l.Npad * 4, 256);
-      l.off_b = off; off = align_up(off + l.Npad * 4, 256);
-    }
-    for (int m = 0; m < tq.nmaps; ++m) {
-      off = align_up(off, 1024);
-      tq.map_off[m] = off;
-      off += static_cast<size_t>(tq.map_rows[m]) * tq.map_kpad[m] * 2;
-    }
-    tq.bytes = align_up(off, 1024);
-    for (auto& l : tq.layers) {
-      l.off_hi = tq.map_off[l.wmap - tq.base_map] + static_cast<size_t>(l.wrow) * l.Kpad * 2;
-      l.off_lo = l.off_hi + static_cast<size_t>(l.Npad) * l.Kpad * 2;
-    }
-  } else {
-    tq.layers.clear();
-  }
+  tq.layers.assign(p->layers.begin() + p->li_q, p->layers.begin() + p->li_q + 3 * d.num_q);
+  if (!layout_blob(tq.layers, p->lay.nmaps, 0, tq.lay)) tq.layers.clear();
   *out = p;
   return 0;
 }
@@ -353,7 +334,7 @@ extern "C" int tdmpc2_planner_create(const tdmpc2_dims* dims, tdmpc2_planner** o
 extern "C" void tdmpc2_planner_destroy(tdmpc2_planner* p) { delete p; }
 extern "C" int tdmpc2_planner_packed_bytes(const tdmpc2_planner* p, size_t* out) {
   if (!p || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
-  *out = p->packed_bytes;
+  *out = p->lay.bytes;
   return 0;
 }
 extern "C" int tdmpc2_planner_workspace_bytes(const tdmpc2_planner* p, size_t* out) {
@@ -411,8 +392,13 @@ static int make_map(EncodeTiledFn enc, CUtensorMap* m, void* base, uint64_t kpad
   return 0;
 }
 
-// Layer table (host part; inv_scale is filled by the pack kernel) of `layers`, whose offsets are relative to `blob`.
-static int write_layer_table(const std::vector<LayerHost>& layers, uint8_t* blob, size_t off_table) {
+// Binds `blob`, laid out by `lay`, to its TMA weight maps and writes its layer table (host part; inv_scale is filled by
+// the pack kernel).
+static int bind_blob(EncodeTiledFn enc, CUtensorMap* tmW, const std::vector<LayerHost>& layers, const BlobLayout& lay,
+                     uint8_t* blob) {
+  int rc;
+  for (int m = 0; m < lay.nmaps; ++m)
+    if ((rc = make_map(enc, &tmW[lay.base_map + m], blob + lay.map_off[m], lay.map_kpad[m], lay.map_rows[m]))) return rc;
   std::vector<LayerDev> tab(layers.size());
   for (size_t i = 0; i < tab.size(); ++i) {
     const LayerHost& l = layers[i];
@@ -425,7 +411,7 @@ static int write_layer_table(const std::vector<LayerHost>& layers, uint8_t* blob
     t.w_hi = reinterpret_cast<const __half*>(blob + l.off_hi);
     t.w_lo = reinterpret_cast<const __half*>(blob + l.off_lo);
   }
-  CUDA_TRY(cudaMemcpy(blob + off_table, tab.data(), tab.size() * sizeof(LayerDev), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(blob + lay.off_table, tab.data(), tab.size() * sizeof(LayerDev), cudaMemcpyHostToDevice));
   return 0;
 }
 
@@ -454,12 +440,9 @@ extern "C" int tdmpc2_planner_bind(tdmpc2_planner* p, void* packed, void* worksp
   int rc;
   if ((rc = make_map(enc, &B.tmX, p->ws + p->off_X, p->KpadX, static_cast<uint64_t>(p->nslots) * 2 * kTileM))) return rc;
   if ((rc = make_map(enc, &B.tmH, p->ws + p->off_H, p->KpadH, static_cast<uint64_t>(p->nslots) * 2 * kTileM))) return rc;
-  for (int m = 0; m < p->nmaps; ++m)
-    if ((rc = make_map(enc, &B.tmW[m], p->packed + p->map_off[m], p->map_kpad[m], p->map_rows[m]))) return rc;
+  if ((rc = bind_blob(enc, B.tmW, p->layers, p->lay, p->packed))) return rc;
 
-  if ((rc = write_layer_table(p->layers, p->packed, p->off_table))) return rc;
-
-  B.layers = reinterpret_cast<const LayerDev*>(p->packed + p->off_table);
+  B.layers = reinterpret_cast<const LayerDev*>(p->packed + p->lay.off_table);
   B.E = d.num_envs; B.N = d.num_samples; B.P = d.num_pi_trajs; B.Ppad = p->Ppad; B.K = d.num_elites; B.H = d.horizon;
   B.obs_dim = d.obs_dim; B.A = d.action_dim; B.Apad = pad_to(d.action_dim, 32); B.L = d.latent_dim; B.M = d.mlp_dim; B.T = d.task_dim; B.B = d.num_bins;
   B.num_q = d.num_q; B.simnorm = d.simnorm_dim; B.num_enc = p->num_enc;
@@ -492,12 +475,12 @@ extern "C" int tdmpc2_planner_bind(tdmpc2_planner* p, void* packed, void* worksp
   return 0;
 }
 
-// Pack Linear `lin` (head `head` of a stacked ensemble tensor) into layer li of `layers`, whose offsets are relative to `blob`.
-static int pack_layer(tdmpc2_planner* p, const std::vector<LayerHost>& layers, uint8_t* blob, size_t off_table, size_t off_absmax,
+// Pack Linear `lin` (head `head` of a stacked ensemble tensor) into layer li of `layers`, laid out in `blob` by `lay`.
+static int pack_layer(tdmpc2_planner* p, const std::vector<LayerHost>& layers, const BlobLayout& lay, uint8_t* blob,
                       int li, const tdmpc2_linear& lin, size_t head, cudaStream_t st) {
   const LayerHost& l = layers[li];
-  LayerDev* table = reinterpret_cast<LayerDev*>(blob + off_table);
-  unsigned* absmax = reinterpret_cast<unsigned*>(blob + off_absmax);
+  LayerDev* table = reinterpret_cast<LayerDev*>(blob + lay.off_table);
+  unsigned* absmax = reinterpret_cast<unsigned*>(blob + lay.off_absmax);
   if (!lin.weight || !lin.bias) return fail(TDMPC2_ERR_INVALID, "layer %d: null weight/bias", li);
   if (l.has_ln && (!lin.ln_weight || !lin.ln_bias)) return fail(TDMPC2_ERR_INVALID, "layer %d: missing LayerNorm tensors", li);
   const float* W = lin.weight + head * static_cast<size_t>(l.src_n) * l.K;
@@ -527,9 +510,9 @@ extern "C" int tdmpc2_pack_weights(tdmpc2_planner* p, const tdmpc2_weights* w, v
   if (d.task_dim > 0 && (!w->task_emb || !w->action_masks)) return fail(TDMPC2_ERR_INVALID, "multi-task model needs task_emb and action_masks");
   if (!w->discount_pow || !w->bins) return fail(TDMPC2_ERR_INVALID, "discount_pow and bins are required");
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
-  CUDA_TRY(cudaMemsetAsync(p->packed + p->off_absmax, 0, p->layers.size() * sizeof(unsigned), st));
+  CUDA_TRY(cudaMemsetAsync(p->packed + p->lay.off_absmax, 0, p->layers.size() * sizeof(unsigned), st));
   auto pack_one = [&](int li, const tdmpc2_linear& lin, size_t head) -> int {
-    return pack_layer(p, p->layers, p->packed, p->off_table, p->off_absmax, li, lin, head, st);
+    return pack_layer(p, p->layers, p->lay, p->packed, li, lin, head, st);
   };
   int rc;
   for (int i = 0; i < p->num_enc; ++i) if ((rc = pack_one(p->li_enc + i, w->enc[i], 0))) return rc;
@@ -574,34 +557,31 @@ struct LaunchCfg {
   LaunchCfg(tdmpc2_planner* p, int grid, size_t smem, cudaStream_t st);
 };
 
-template <class K>
-static int launch_big(tdmpc2_planner* p, K kernel, bool* attr_done, int grid, cudaStream_t st, const PlanParams& prm) {
-  if (!*attr_done) {     // > 48 KiB of dynamic shared memory needs the opt-in, once per kernel instantiation
+// Every plan_kernel launch.  The instantiation follows the engine and the kind of launch: planning, the rollout modes of
+// an episodic model (MODE_ITER / MODE_VALUE with the termination head), or row mode.  Row launches are not profiled.
+static int launch(tdmpc2_planner* p, const PlanParams& prm, void* stream_) {
+  using Kernel = void (*)(PlanParams);
+  static const Kernel kernels[2][3] = {
+      {plan_kernel<ENGINE_TC>, plan_kernel<ENGINE_TC, true>, plan_kernel<ENGINE_TC, false, true>},
+      {plan_kernel<ENGINE_SIMT>, plan_kernel<ENGINE_SIMT, true>, plan_kernel<ENGINE_SIMT, false, true>}};
+  const bool rows = prm.mode == MODE_ROWS;
+  const int kind = rows ? 2 : (p->d.episodic && (prm.mode == MODE_ITER || prm.mode == MODE_VALUE)) ? 1 : 0;
+  const int engine = p->engine == TDMPC2_ENGINE_SIMT ? 1 : 0;
+  const Kernel kernel = kernels[engine][kind];
+  bool& attr_done = p->attr_done[3 * engine + kind];
+  if (!attr_done) {     // > 48 KiB of dynamic shared memory needs the opt-in, once per kernel instantiation
     CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    *attr_done = true;
+    attr_done = true;
   }
-  LaunchCfg lc(p, grid, kSmemBytes, st);
-  CUDA_TRY(cudaLaunchKernelEx(&lc.cfg, kernel, prm));
+  PlanParams prm2 = prm;
+  prm2.prof = rows ? nullptr : p->prof;
+  prm2.prof_slots = p->nslots;
+  prm2.passes = p->passes;
+  LaunchCfg lc(p, std::min(prm.ntiles, p->nslots), kSmemBytes, static_cast<cudaStream_t>(stream_));
+  CUDA_TRY(cudaLaunchKernelEx(&lc.cfg, kernel, prm2));
   CUDA_TRY(cudaGetLastError());
   p->launches += 1;
   return 0;
-}
-
-static int launch_plan(tdmpc2_planner* p, const PlanParams& prm, int ntiles, cudaStream_t st) {
-  // episodic models: the rollout modes run the instantiations that carry the termination head
-  const bool epi = p->d.episodic && (prm.mode == MODE_ITER || prm.mode == MODE_VALUE);
-  const int grid = std::min(ntiles, p->nslots);
-  PlanParams prm2 = prm;
-  prm2.prof = p->prof;
-  prm2.prof_slots = p->nslots;
-  prm2.passes = p->passes;
-  bool* ad = p->attr_done;
-  if (p->engine == TDMPC2_ENGINE_SIMT) {
-    if (epi) return launch_big(p, plan_kernel<ENGINE_SIMT, true>, &ad[0], grid, st, prm2);
-    return launch_big(p, plan_kernel<ENGINE_SIMT>, &ad[1], grid, st, prm2);
-  }
-  if (epi) return launch_big(p, plan_kernel<ENGINE_TC, true>, &ad[2], grid, st, prm2);
-  return launch_big(p, plan_kernel<ENGINE_TC>, &ad[3], grid, st, prm2);
 }
 
 LaunchCfg::LaunchCfg(tdmpc2_planner* p, int grid, size_t smem, cudaStream_t st) {
@@ -667,7 +647,7 @@ static int prologue_impl(tdmpc2_planner* p, const float* obs, const float* z_in,
     prm.obs = obs;
     prm.mode = MODE_ENCODE;
     prm.ntiles = (d.num_envs + kTileM - 1) / kTileM;
-    if ((rc = launch_plan(p, prm, prm.ntiles, st))) return rc;
+    if ((rc = launch(p, prm, st))) return rc;
   } else {
     CUDA_TRY(cudaMemcpyAsync(p->base.z, z_in, static_cast<size_t>(d.num_envs) * d.latent_dim * 4, cudaMemcpyDeviceToDevice, st));
   }
@@ -685,7 +665,7 @@ static int prologue_impl(tdmpc2_planner* p, const float* obs, const float* z_in,
     prm.noise_prior = noise_prior;
     const int per = kTileM / p->Ppad;
     prm.ntiles = (d.num_envs + per - 1) / per;
-    if ((rc = launch_plan(p, prm, prm.ntiles, st))) return rc;
+    if ((rc = launch(p, prm, st))) return rc;
   }
   return 0;
 }
@@ -764,7 +744,7 @@ extern "C" int tdmpc2_plan_iter(tdmpc2_planner* p, const float* noise_r, const f
   prm.elite_idx_out = reinterpret_cast<long long*>(elite_idx_out);
   prm.ntiles = d.num_envs * p->tiles_per_env;
   prm.zb_kc0 = p->zb_kc0;
-  return launch_plan(p, prm, prm.ntiles, static_cast<cudaStream_t>(stream_));
+  return launch(p, prm, stream_);
 }
 
 // Declared non-parity throughput mode: the iteration generates its two large noise tensors itself (rng.cuh).
@@ -785,7 +765,7 @@ extern "C" int tdmpc2_plan_iter_rng(tdmpc2_planner* p, const uint64_t* rng_state
   prm.elite_idx_out = reinterpret_cast<long long*>(elite_idx_out);
   prm.ntiles = d.num_envs * p->tiles_per_env;
   prm.zb_kc0 = p->zb_kc0;
-  return launch_plan(p, prm, prm.ntiles, static_cast<cudaStream_t>(stream_));
+  return launch(p, prm, stream_);
 }
 // Diagnostics / tests: the normals of `ngroups` consecutive groups of one stream (4 per group).
 extern "C" int tdmpc2_debug_rng(const uint64_t* rng_state, uint32_t stream, uint64_t group0, int ngroups, float* out, void* stream_) {
@@ -840,7 +820,7 @@ extern "C" int tdmpc2_estimate_value(tdmpc2_planner* p, const float* z, const fl
   prm.z_rows = z; prm.actions_explicit = actions; prm.noise_pi = noise_pi; prm.qidx = qidx;
   prm.values_out = value_out;
   prm.ntiles = d.num_envs * p->tiles_per_env;
-  return launch_plan(p, prm, prm.ntiles, static_cast<cudaStream_t>(stream_));
+  return launch(p, prm, stream_);
 }
 
 extern "C" int tdmpc2_debug_layer(tdmpc2_planner* p, int layer, int mode, const float* x, int rows, float* y, void* stream_) {
@@ -854,30 +834,27 @@ extern "C" int tdmpc2_debug_layer(tdmpc2_planner* p, int layer, int mode, const 
   prm.mode = MODE_LAYER;
   prm.dbg_layer = layer; prm.dbg_mode = mode; prm.dbg_rows = rows; prm.dbg_x = x; prm.dbg_y = y;
   prm.ntiles = 1;
-  return launch_plan(p, prm, 1, static_cast<cudaStream_t>(stream_));
+  return launch(p, prm, stream_);
 }
 
 // ------------------------------------------------------------------------------------ target Q ensemble
 extern "C" int tdmpc2_planner_target_q_bytes(const tdmpc2_planner* p, size_t* out) {
   if (!p || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
-  if (p->tq.bytes == 0) return fail(TDMPC2_ERR_UNSUPPORTED, "the model's weight maps leave no room for the target Q maps (%d)", kMaxWMaps);
-  *out = p->tq.bytes;
+  if (p->tq.lay.bytes == 0) return fail(TDMPC2_ERR_UNSUPPORTED, "the model's weight maps leave no room for the target Q maps (%d)", kMaxWMaps);
+  *out = p->tq.lay.bytes;
   return 0;
 }
 
 extern "C" int tdmpc2_planner_bind_target_q(tdmpc2_planner* p, void* blob) {
   if (!p || !blob) return fail(TDMPC2_ERR_INVALID, "null argument");
   if (!p->bound) return fail(TDMPC2_ERR_STATE, "tdmpc2_planner_bind must be called first");
-  if (p->tq.bytes == 0) return fail(TDMPC2_ERR_UNSUPPORTED, "the model's weight maps leave no room for the target Q maps");
+  if (p->tq.lay.bytes == 0) return fail(TDMPC2_ERR_UNSUPPORTED, "the model's weight maps leave no room for the target Q maps");
   if (reinterpret_cast<uintptr_t>(blob) & 255) return fail(TDMPC2_ERR_INVALID, "buffers must be 256-byte aligned");
   TargetQ& tq = p->tq;
   EncodeTiledFn enc = encode_tiled_fn();
   if (!enc) return fail(TDMPC2_ERR_CUDA, "cuTensorMapEncodeTiled not available");
   int rc;
-  for (int m = 0; m < tq.nmaps; ++m)
-    if ((rc = make_map(enc, &p->base.tmW[tq.base_map + m], static_cast<uint8_t*>(blob) + tq.map_off[m], tq.map_kpad[m], tq.map_rows[m])))
-      return rc;
-  if ((rc = write_layer_table(tq.layers, static_cast<uint8_t*>(blob), tq.off_table))) return rc;
+  if ((rc = bind_blob(enc, p->base.tmW, tq.layers, tq.lay, static_cast<uint8_t*>(blob)))) return rc;
   tq.blob = static_cast<uint8_t*>(blob);
   tq.packed = false;
   return 0;
@@ -888,11 +865,11 @@ extern "C" int tdmpc2_pack_target_q(tdmpc2_planner* p, const tdmpc2_linear* targ
   if (!p->bound || !p->tq.blob) return fail(TDMPC2_ERR_STATE, "tdmpc2_planner_bind_target_q must be called first");
   TargetQ& tq = p->tq;
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
-  CUDA_TRY(cudaMemsetAsync(tq.blob + tq.off_absmax, 0, tq.layers.size() * sizeof(unsigned), st));
+  CUDA_TRY(cudaMemsetAsync(tq.blob + tq.lay.off_absmax, 0, tq.layers.size() * sizeof(unsigned), st));
   int rc;
   for (int h = 0; h < p->d.num_q; ++h)
     for (int l = 0; l < 3; ++l)
-      if ((rc = pack_layer(p, tq.layers, tq.blob, tq.off_table, tq.off_absmax, 3 * h + l, target_qs[l], h, st))) return rc;
+      if ((rc = pack_layer(p, tq.layers, tq.lay, tq.blob, 3 * h + l, target_qs[l], h, st))) return rc;
   CUDA_TRY(cudaGetLastError());
   tq.packed = true;
   return 0;
@@ -917,19 +894,9 @@ static PlanParams rows_params(tdmpc2_planner* p, int rop, int rows, const int32_
   prm.rop = rop;
   prm.rows = rows;
   prm.task = p->d.task_dim > 0 ? task : nullptr;
-  prm.rows_q = reinterpret_cast<const LayerDev*>(p->packed + p->off_table) + p->li_q;
+  prm.rows_q = reinterpret_cast<const LayerDev*>(p->packed + p->lay.off_table) + p->li_q;
   prm.ntiles = (rows + kTileM - 1) / kTileM;
   return prm;
-}
-
-static int launch_rows(tdmpc2_planner* p, const PlanParams& prm, void* stream_) {
-  const int grid = std::min(prm.ntiles, p->nslots);
-  PlanParams prm2 = prm;
-  prm2.prof = nullptr;
-  prm2.passes = p->passes;
-  cudaStream_t st = static_cast<cudaStream_t>(stream_);
-  if (p->engine == TDMPC2_ENGINE_SIMT) return launch_big(p, plan_kernel<ENGINE_SIMT, false, true>, &p->attr_done[4], grid, st, prm2);
-  return launch_big(p, plan_kernel<ENGINE_TC, false, true>, &p->attr_done[5], grid, st, prm2);
 }
 
 static int need_task(tdmpc2_planner* p, const int32_t* task) {
@@ -944,7 +911,7 @@ extern "C" int tdmpc2_wm_encode(tdmpc2_planner* p, const float* obs, const int32
   if (p->num_enc == 0) return fail(TDMPC2_ERR_STATE, "this planner was created without a state encoder (num_enc_layers = 0)");
   PlanParams prm = rows_params(p, ROP_ENCODE, rows, task);
   prm.rows_in = obs; prm.rows_out = z_out;
-  return launch_rows(p, prm, stream_);
+  return launch(p, prm, stream_);
 }
 
 static int rows_za(tdmpc2_planner* p, int rop, const float* z, const float* a, const int32_t* task, int rows, float* out, void* stream_) {
@@ -953,7 +920,7 @@ static int rows_za(tdmpc2_planner* p, int rop, const float* z, const float* a, c
   if (!z || !a || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
   PlanParams prm = rows_params(p, rop, rows, task);
   prm.rows_in = z; prm.rows_act = a; prm.rows_out = out;
-  return launch_rows(p, prm, stream_);
+  return launch(p, prm, stream_);
 }
 extern "C" int tdmpc2_wm_next(tdmpc2_planner* p, const float* z, const float* a, const int32_t* task, int rows, float* z_out, void* stream_) {
   return rows_za(p, ROP_NEXT, z, a, task, rows, z_out, stream_);
@@ -971,7 +938,7 @@ extern "C" int tdmpc2_wm_termination(tdmpc2_planner* p, const float* z, int rows
     return fail(TDMPC2_ERR_UNSUPPORTED, "termination needs an episodic single-task model");
   PlanParams prm = rows_params(p, ROP_TERM, rows, nullptr);
   prm.rows_in = z; prm.rows_out = out; prm.rows_flag = sigmoid ? 1 : 0;
-  return launch_rows(p, prm, stream_);
+  return launch(p, prm, stream_);
 }
 
 extern "C" int tdmpc2_wm_pi(tdmpc2_planner* p, const float* z, const int32_t* task, const float* eps, int rows, float* action_out,
@@ -982,14 +949,14 @@ extern "C" int tdmpc2_wm_pi(tdmpc2_planner* p, const float* z, const int32_t* ta
   PlanParams prm = rows_params(p, ROP_PI, rows, task);
   prm.rows_in = z; prm.rows_eps = eps;
   prm.rows_out = action_out; prm.rows_out2 = mean_out; prm.rows_out3 = log_std_out; prm.rows_out4 = log_prob_out;
-  return launch_rows(p, prm, stream_);
+  return launch(p, prm, stream_);
 }
 
 static int select_q(tdmpc2_planner* p, int target, PlanParams& prm) {
   if (!target) return 0;
   if (!p->tq.blob || !p->tq.packed)
     return fail(TDMPC2_ERR_STATE, "target Q op before tdmpc2_planner_bind_target_q + tdmpc2_pack_target_q");
-  prm.rows_q = reinterpret_cast<const LayerDev*>(p->tq.blob + p->tq.off_table);
+  prm.rows_q = reinterpret_cast<const LayerDev*>(p->tq.blob + p->tq.lay.off_table);
   return 0;
 }
 
@@ -1004,7 +971,7 @@ extern "C" int tdmpc2_wm_q(tdmpc2_planner* p, const float* z, const float* a, co
   if ((rc = select_q(p, target, prm))) return rc;
   prm.rows_in = z; prm.rows_act = a; prm.rows_out = out; prm.qidx = qidx;
   prm.rows_flag = return_type == TDMPC2_Q_AVG ? 1 : 0;
-  return launch_rows(p, prm, stream_);
+  return launch(p, prm, stream_);
 }
 
 extern "C" int tdmpc2_td_target(tdmpc2_planner* p, const float* next_z, const float* reward, const float* terminated,
@@ -1016,5 +983,5 @@ extern "C" int tdmpc2_td_target(tdmpc2_planner* p, const float* next_z, const fl
   if ((rc = select_q(p, 1, prm))) return rc;
   prm.rows_in = next_z; prm.rows_eps = eps; prm.qidx = qidx;
   prm.rows_reward = reward; prm.rows_term = terminated; prm.rows_out = out;
-  return launch_rows(p, prm, stream_);
+  return launch(p, prm, stream_);
 }

@@ -108,11 +108,9 @@ class TDMPC2(torch.nn.Module):
     @torch.no_grad()
     def _policy_action(self, obs, eval_mode=False, task=None, eps: Optional[torch.Tensor] = None):
         """The non-MPC branch of act() (tdmpc2.py:116-120): a = pi(encode(obs)), or its mean in eval_mode
-        (`info["mean"]` = tanh(mean), world_model.py:173).  Runs the encode + policy-prior kernel modes: trajectory 0,
-        step 0 of the prior rollout IS pi(encode(obs)) with noise eps (zero noise gives the mean)."""
+        (`info["mean"]` = tanh(mean), world_model.py:173).  Two row-mode launches, encode then pi with noise eps
+        (zero noise gives the mean); the planner's state is not touched."""
         cfg, E, dev = self.cfg, self.num_envs, self.device
-        if cfg.num_pi_trajs < 1:
-            raise NotImplementedError("the kernel policy path needs cfg.num_pi_trajs >= 1")
         rgb = cfg.get("obs", "state") == "rgb"
         obs = obs.to(dev, torch.float32)
         obs = (obs.reshape(E, *cfg.obs_shape["rgb"]) if rgb else obs.reshape(E, -1)).contiguous()
@@ -123,18 +121,18 @@ class TDMPC2(torch.nn.Module):
             taskv = torch.as_tensor(task, device=dev).reshape(-1).to(torch.int32)
             taskv = taskv.expand(E).contiguous() if taskv.numel() == 1 else taskv.contiguous()
         pl = self.planner
-        shift = None
         if rgb:                                                                     # ShiftAug's draw comes first (layers.py:55)
             shift = torch.randint(0, 7, (E, 2), device=dev, dtype=torch.float32, generator=self.generator)
-        noise = torch.zeros(E, cfg.horizon, cfg.num_pi_trajs, cfg.action_dim, device=dev)
-        if not eval_mode:
-            noise[:, 0, 0] = torch.randn(E, cfg.action_dim, device=dev, generator=self.generator) if eps is None else eps.to(dev)
-        ones, zeros = torch.ones(E, dtype=torch.uint8, device=dev), torch.zeros(E, cfg.horizon, cfg.action_dim, device=dev)
-        if rgb:
-            pl.prologue_latent(pl.encode_pixels(obs, shift), taskv, ones, zeros, noise)
+            z = pl.encode_pixels(obs, shift)
         else:
-            pl.prologue(obs, taskv, ones, zeros, noise)
-        return pl.get_state()["pi_actions"][:, 0, 0].clone()
+            z = pl.wm_encode(obs, taskv)
+        if eval_mode:
+            eps = torch.zeros(E, cfg.action_dim, device=dev)
+        elif eps is None:
+            eps = torch.randn(E, cfg.action_dim, device=dev, generator=self.generator)
+        else:
+            eps = eps.to(dev, torch.float32).expand(E, cfg.action_dim).contiguous()
+        return pl.wm_pi(z, taskv, eps)[0]
 
     @torch.no_grad()
     def _plan(self, obs, t0=False, eval_mode=False, task=None, noise: Optional[Noise] = None, return_trace=False):

@@ -2,7 +2,7 @@
 
 The planner's kernels read the weights straight from `state_dict()` (tdmpc2_b200/planner.py packs them into the
 kernel layout), so this class holds tensors, not a module tree.  Every forward of the planning path runs in the fused
-sm_90a kernels, including the non-MPC `act()` branch (TDMPC2.act -> the policy-prior kernel mode).  The reference's
+sm_90a kernels, including the non-MPC `act()` branch (TDMPC2.act -> row-mode encode and pi).  The reference's
 methods -- `encode`, `next`, `reward`, `termination`, `pi`, `Q` (common/world_model.py:103-216) -- exist with its
 signatures and shapes and run on the kernels' row mode (one launch per call, any [..., .] batch); `td_target` is
 TDMPC2._td_target's fused launch.  They use the owning agent's Planner, or a one-environment Planner of their own; the

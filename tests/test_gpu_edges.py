@@ -120,7 +120,7 @@ def test_agent_api_shapes_state_and_checkpoint(tmp_path):
 
 def test_non_mpc_act_runs_the_policy_through_the_kernels():
     """cfg.mpc = False (tdmpc2.py:116-120): act() = pi(encode(obs)) with noise, or tanh(mean) in eval_mode -- both come
-    from the encode + policy-prior kernel modes and must match the oracle's encode/pi (1e-5, like the prior test)."""
+    from the row-mode encode and pi launches and must match the oracle's encode/pi (1e-5, like the prior test)."""
     from oracle.plan_oracle import OracleModel
     from tdmpc2_b200.tdmpc2 import TDMPC2
     E = 3
