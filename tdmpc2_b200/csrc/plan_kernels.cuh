@@ -18,13 +18,14 @@
 //                 X / H / raw scratch, which is dead between launches.
 //
 // Every dense layer is `acc = A[128, Kpad] * W[Npad, Kpad]^T` with both operands stored as two fp16 planes (hi, lo;
-// x ~= hi + lo to ~22 bits).  The tensor-core engine (ENGINE_TC) streams 64-element K-chunks of both operands with TMA
-// (128-byte swizzle) through a 3-stage mbarrier ring (warp 16 = producer) into four consumer warpgroups, each of which
-// owns a 64 x 64 block of every 128 x 128 output block and runs wgmma (m64n64k16) A_lo*W_hi + A_hi*W_lo + A_hi*W_hi
-// per K-chunk into fresh fp32 registers; the K-chunk partials are added with round-to-nearest and the block goes to
-// an fp32 scratch row buffer in global memory.  The SIMT engine computes the same sums with FFMA on CUDA cores.  Both
-// engines then run the same row phases (warp per row): bias + LayerNorm + Mish / SimNorm, two-hot-inverse,
-// tanh-Gaussian sampling, and emit the next layer's fp16 planes.
+// x ~= hi + lo to ~22 bits).  A CTA is 384 threads (12 warps).  The tensor-core engine (ENGINE_TC) streams 64-element
+// K-chunks of both operands with TMA (128-byte swizzle) through a 3-stage mbarrier ring (warp 8 = producer, warps 9-11
+// idle during the GEMM) into two consumer warpgroups (warps 0-7), each of which owns 64 rows x all 128 columns of every
+// 128 x 128 output block and runs wgmma (m64n128k16) A_lo*W_hi + A_hi*W_lo + A_hi*W_hi per K-chunk into fresh fp32
+// registers; the K-chunk partials are added with round-to-nearest and the block goes to an fp32 scratch row buffer in
+// global memory.  The SIMT engine computes the same sums with FFMA on CUDA cores.  Both engines then run the same row
+// phases (all 12 warps, warp per row): bias + LayerNorm + Mish / SimNorm, two-hot-inverse, tanh-Gaussian sampling, and
+// emit the next layer's fp16 planes.
 //
 // Activations live in a per-CTA scratch slot (global memory: X planes +
 // one in-place hidden buffer, 0.56 MB per slot for the 5M model).
@@ -49,10 +50,10 @@ constexpr int kStageBytes = 6 * kAPlane;        // 96 KiB (the operand smem is k
 constexpr int kGStages = 3;
 constexpr int kGStageBytes = 4 * kAPlane;
 constexpr int kGNb = 128;                        // output columns per block (W rows per stage)
-constexpr int kGWarpGroups = 4;                  // consumer warps 0..15: warpgroup g owns rows 64 (g & 1).., columns 64 (g >> 1)..
-constexpr int kGProducerWarp = 4 * kGWarpGroups; // warp 16 issues the TMA loads
+constexpr int kGWarpGroups = 2;                  // consumer warps 0..7: warpgroup g owns rows 64 g.., all 128 columns
+constexpr int kGProducerWarp = 4 * kGWarpGroups; // warp 8 issues the TMA loads; warps 9..11 idle during the GEMM
 static_assert(kGStages * kGStageBytes <= kStages * kStageBytes, "operand smem layout");
-constexpr int kThreads = 576;                   // 18 warps; ptxas assigns 96 registers per thread (small spills)
+constexpr int kThreads = 384;                   // 12 warps: __launch_bounds__(384, 1) leaves ptxas 168 registers per thread
 constexpr int kWarps = kThreads / 32;
 constexpr int kMaxWMaps = 8;
 constexpr int kMaxHeadCols = 256;  // widest head output (2A or num_bins)
@@ -182,14 +183,6 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
-// Mish(x) = x * tanh(softplus(x)) (layers.py:103; softplus threshold 20).
-// tanh(log(1+e^x)) = n / (n + 2) with n = e^x (e^x + 2): one exp, one divide, no cancellation.
-__device__ __forceinline__ float mish_f(float x) {
-  if (x > 20.f) return x;
-  const float e = expf(x);
-  const float n = e * (e + 2.f);
-  return x * __fdiv_rn(n, n + 2.f);
-}
 __device__ __forceinline__ float symexp_f(float x) {   // math.py:50-55
   const float m = expf(fabsf(x)) - 1.f;
   return x > 0.f ? m : (x < 0.f ? -m : 0.f);
@@ -220,7 +213,7 @@ __device__ __forceinline__ float4 lds128(const float* p) {   // p must point int
 }
 // Diagnostics (cycle counters per role, clock stamps per layer of CTA 0) exist only in builds with -DTDMPC2_PROF
 // (tdmpc2_b200.build.build_variant("prof", ["TDMPC2_PROF=1"]), loaded through TDMPC2_B200_LIB): in the product build
-// they compile to nothing -- the 8 per-thread 64-bit counters alone cost 16 registers of a 96-register budget.
+// they compile to nothing -- the 8 per-thread 64-bit counters alone cost 16 registers of a 168-register budget.
 #ifdef TDMPC2_PROF
 constexpr bool kProf = true;
 #else
@@ -390,45 +383,45 @@ __device__ __forceinline__ void gemm_tc(const PlanParams& P, Ctx& c, const Layer
       }
     }
   } else if (c.warp < kGProducerWarp) {
-    const int wg = c.warp >> 2, t = threadIdx.x & 127;
-    const int r0 = (wg & 1) * 64, n0 = (wg >> 1) * 64;
-    const int row = r0 + (t >> 5) * 16 + ((t & 31) >> 2), col = n0 + 2 * (t & 3);
+    const int t = threadIdx.x & 127;
+    const int r0 = (c.warp >> 2) * 64;
+    const int row = r0 + (t >> 5) * 16 + ((t & 31) >> 2), col = 2 * (t & 3);
     float* rawbase = raw_ptr(P, c.slot);
     const uint32_t sbase = ptx::smem_u32(c.stage_base);
     for (int nb = 0; nb < nnb; ++nb) {
-      float sum[32];
+      float sum[64];
 #pragma unroll
-      for (int i = 0; i < 32; ++i) sum[i] = 0.f;
+      for (int i = 0; i < 64; ++i) sum[i] = 0.f;
       for (int kc = kc0; kc < kc1; ++kc) {
         const uint32_t s = c.ma_it % kGStages, ph = (c.ma_it / kGStages) & 1;
         const long long tw = prof_clock();
         ptx::mbar_wait(&c.g_full[s], ph);
         c.pf2 += prof_clock() - tw;
-        const uint32_t sa = sbase + s * kGStageBytes + r0 * 128, sw = sbase + s * kGStageBytes + 2 * kAPlane + n0 * 128;
-        float acc[32];
+        const uint32_t sa = sbase + s * kGStageBytes + r0 * 128, sw = sbase + s * kGStageBytes + 2 * kAPlane;
+        float acc[64];
 #pragma unroll
-        for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
         ptx::wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < kKch / 16; ++ks) {
           const uint64_t a_hi = ptx::make_sw128_kmajor_desc(sa + ks * 32), w_hi = ptx::make_sw128_kmajor_desc(sw + ks * 32);
           if (lo) {
-            ptx::wgmma_m64n64k16(acc, ptx::make_sw128_kmajor_desc(sa + kAPlane + ks * 32), w_hi);
-            ptx::wgmma_m64n64k16(acc, a_hi, ptx::make_sw128_kmajor_desc(sw + kAPlane + ks * 32));
+            ptx::wgmma_m64n128k16(acc, ptx::make_sw128_kmajor_desc(sa + kAPlane + ks * 32), w_hi);
+            ptx::wgmma_m64n128k16(acc, a_hi, ptx::make_sw128_kmajor_desc(sw + kAPlane + ks * 32));
           }
-          ptx::wgmma_m64n64k16(acc, a_hi, w_hi);
+          ptx::wgmma_m64n128k16(acc, a_hi, w_hi);
         }
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         __syncwarp();
         if (c.lane == 0) ptx::mbar_arrive(&c.g_empty[s]);     // this warp's reads of the stage are complete
 #pragma unroll
-        for (int i = 0; i < 32; ++i) sum[i] = __fadd_rn(sum[i], acc[i]);
+        for (int i = 0; i < 64; ++i) sum[i] = __fadd_rn(sum[i], acc[i]);
         ++c.ma_it;
       }
       float* o = rawbase + static_cast<size_t>(row) * P.NpadMax + nb * kGNb + col;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
+      for (int j = 0; j < 16; ++j) {
         __stcg(reinterpret_cast<float2*>(o + 8 * j), make_float2(sum[4 * j], sum[4 * j + 1]));
         __stcg(reinterpret_cast<float2*>(o + 8 * static_cast<size_t>(P.NpadMax) + 8 * j), make_float2(sum[4 * j + 2], sum[4 * j + 3]));
       }
@@ -495,9 +488,8 @@ __device__ __forceinline__ void gemm_simt(const PlanParams& P, Ctx& c, const Lay
 }
 
 // ------------------------------------------------------------------------------------ row phases (warp per row)
-__device__ __forceinline__ float ln_act_lane(float y, bool valid, int act) {
-  if (act == EPI_LN_MISH) return mish_f(y);
-  // SimNorm (layers.py:74-88): softmax over groups of 8 consecutive columns = 8 adjacent lanes.
+// SimNorm (layers.py:74-88) of one lane's column: softmax over groups of 8 consecutive columns = 8 adjacent lanes.
+__device__ __forceinline__ float simnorm_lane(float y, bool valid) {
   float m = valid ? y : -CUDART_INF_F;
   m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
   m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
@@ -510,11 +502,36 @@ __device__ __forceinline__ float ln_act_lane(float y, bool valid, int act) {
   return valid ? __fdiv_rn(e, t) : 0.f;
 }
 
-// LayerNorm (+ Mish | SimNorm) over raw rows; one warp per row, lane-strided columns (lane + 32 j).  The output pass
-// re-reads raw from L2; the statistics read it once (512-wide rows) or once per statistic (other widths).  The output
-// pass stays a compact loop: keeping the row in registers through it too raises the kernel's spills (248 B of spill
-// stores instead of 84 with ptxas for sm_90a).
-constexpr int kLnRegCols = 16;
+constexpr int kLnRegCols = 16;   // columns per lane of a 512-wide row
+constexpr int kLnBatch = 8;      // columns per lane that the output pass carries through activation and stores at once
+
+// Mish(x) = x * tanh(softplus(x)) (layers.py:103; softplus threshold 20) of a lane's batch of columns.
+// tanh(log(1+e^x)) = n / (n + 2) with n = e^x (e^x + 2): one exp, one divide, no cancellation.  Three passes over the
+// batch, so that its independent exp / divide chains overlap: a divide is a branch (its slow-path call), and a
+// column-at-a-time loop runs the chains one after another.  x > 20 returns x; what the other passes computed for it
+// (possibly inf / NaN) is discarded.
+__device__ __forceinline__ void mish_batch(float (&y)[kLnBatch]) {
+  float q[kLnBatch];
+#pragma unroll
+  for (int u = 0; u < kLnBatch; ++u) {
+    const float e = expf(y[u]);
+    q[u] = e * (e + 2.f);
+  }
+#pragma unroll
+  for (int u = 0; u < kLnBatch; ++u) q[u] = __fdiv_rn(q[u], q[u] + 2.f);
+#pragma unroll
+  for (int u = 0; u < kLnBatch; ++u) y[u] = y[u] > 20.f ? y[u] : y[u] * q[u];
+}
+
+// LayerNorm (+ Mish | SimNorm) over raw rows; one warp per row, lane-strided columns (lane + 32 j).  raw is written by
+// this kernel's GEMM and read with ld.global.cg; bias / gamma / beta are read-only for the kernel's lifetime and go
+// through the read-only path (__ldg).  The output pass works on batches of kLnBatch columns per lane: every load of a
+// batch is issued before its first store (the stores go through pointers that may alias raw as far as the compiler
+// knows), and the batch's activations are independent chains that overlap.
+//   - 512-wide rows (every hidden layer of the 5M model): raw is read once; the 16 values per lane stay in registers from
+//     the statistics through the output pass.
+//   - other widths: raw is read once per statistic and once in the output pass.
+// Every column's value is the same expression in the same order in both paths: same bits.
 __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const LayerRec& ly, const EpiArgs& ea) {
   const float* rawbase = raw_ptr(P, c.slot);
   const int N = ly.N;
@@ -527,51 +544,84 @@ __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const L
   const int ncolj = (N + 31) / 32;
   for (int r = c.warp; r < kTileM; r += kWarps) {
     const float* rr = rawbase + static_cast<size_t>(r) * P.NpadMax;
-    float mean, var;
+    const int orow = ea.rowmap ? ea.rowmap[r] : r;
+    // activation and stores of the batch y = columns lane + 32 (j0 + u); warp-uniform (SimNorm shuffles across lanes)
+    auto act_store = [&](float (&y)[kLnBatch], int j0) {
+      if (ea.kind == EPI_LN_MISH) {
+        mish_batch(y);
+      } else {
+#pragma unroll
+        for (int u = 0; u < kLnBatch; ++u)
+          if (j0 + u < ncolj) y[u] = simnorm_lane(y[u], c.lane + 32 * (j0 + u) < N);
+      }
+      if (dhi) {
+        __half* hi = dhi + static_cast<size_t>(r) * pitch + ea.dst_col0;
+        __half* lo = dlo + static_cast<size_t>(r) * pitch + ea.dst_col0;
+#pragma unroll
+        for (int u = 0; u < kLnBatch; ++u) {
+          const int col = c.lane + 32 * (j0 + u);
+          if (col < N) split_store(hi + col, lo + col, y[u]);
+        }
+      }
+      if (ea.out_f32 && orow >= 0) {
+        float* o = ea.out_f32 + static_cast<size_t>(orow) * ea.out_pitch;
+#pragma unroll
+        for (int u = 0; u < kLnBatch; ++u) {
+          const int col = c.lane + 32 * (j0 + u);
+          if (col < N) o[col] = y[u];
+        }
+      }
+    };
     if (N == 32 * kLnRegCols) {
-      // 512-wide rows (every hidden layer of the 5M model): mean and variance from ONE read of the row.  The loads are
-      // unconditional and all issued before the first use, so the row costs one L2 round trip instead of one per
-      // unrolled batch of each statistic's loop.  Same expressions in the same order as below: same bits.
+      // The loads are unconditional and all issued before the first use: the row costs one L2 round trip.
       float x[kLnRegCols];
 #pragma unroll
       for (int j = 0; j < kLnRegCols; ++j) x[j] = __ldcg(rr + c.lane + 32 * j);
       float s = 0.f;
 #pragma unroll
       for (int j = 0; j < kLnRegCols; ++j) {
-        x[j] = fmaf(x[j], inv_scale, bias[c.lane + 32 * j]);
+        x[j] = fmaf(x[j], inv_scale, __ldg(bias + c.lane + 32 * j));
         s += x[j];
       }
-      mean = warp_sum(s) * invN;
+      const float mean = warp_sum(s) * invN;
       float sq = 0.f;
 #pragma unroll
       for (int j = 0; j < kLnRegCols; ++j) {
         const float d = x[j] - mean;
         sq = fmaf(d, d, sq);
       }
-      var = warp_sum(sq) * invN;
+      const float var = warp_sum(sq) * invN;
+      const float rstd = 1.f / sqrtf(var + 1e-5f);   // nn.LayerNorm eps (layers.py:101)
+#pragma unroll
+      for (int j0 = 0; j0 < kLnRegCols; j0 += kLnBatch) {
+        float y[kLnBatch];
+#pragma unroll
+        for (int u = 0; u < kLnBatch; ++u) {
+          const int col = c.lane + 32 * (j0 + u);
+          y[u] = (x[j0 + u] - mean) * rstd * __ldg(lg + col) + __ldg(lb + col);
+        }
+        act_store(y, j0);
+      }
     } else {
       float s = 0.f;
-      for (int col = c.lane; col < N; col += 32) s += fmaf(__ldcg(rr + col), inv_scale, bias[col]);
-      mean = warp_sum(s) * invN;
+      for (int col = c.lane; col < N; col += 32) s += fmaf(__ldcg(rr + col), inv_scale, __ldg(bias + col));
+      const float mean = warp_sum(s) * invN;
       float sq = 0.f;
       for (int col = c.lane; col < N; col += 32) {
-        const float d = fmaf(__ldcg(rr + col), inv_scale, bias[col]) - mean;
+        const float d = fmaf(__ldcg(rr + col), inv_scale, __ldg(bias + col)) - mean;
         sq = fmaf(d, d, sq);
       }
-      var = warp_sum(sq) * invN;
-    }
-    const float rstd = 1.f / sqrtf(var + 1e-5f);   // nn.LayerNorm eps (layers.py:101)
-    const int orow = ea.rowmap ? ea.rowmap[r] : r;
-    for (int j = 0; j < ncolj; ++j) {
-      const int col = c.lane + 32 * j;
-      const bool valid = col < N;
-      float y = 0.f;
-      if (valid) y = (fmaf(__ldcg(rr + col), inv_scale, bias[col]) - mean) * rstd * lg[col] + lb[col];
-      y = ln_act_lane(y, valid, ea.kind);
-      if (valid) {
-        if (dhi) split_store(dhi + static_cast<size_t>(r) * pitch + ea.dst_col0 + col,
-                             dlo + static_cast<size_t>(r) * pitch + ea.dst_col0 + col, y);
-        if (ea.out_f32 && orow >= 0) ea.out_f32[static_cast<size_t>(orow) * ea.out_pitch + col] = y;
+      const float var = warp_sum(sq) * invN;
+      const float rstd = 1.f / sqrtf(var + 1e-5f);
+      for (int j0 = 0; j0 < ncolj; j0 += kLnBatch) {
+        float y[kLnBatch];
+#pragma unroll
+        for (int u = 0; u < kLnBatch; ++u) {
+          const int col = c.lane + 32 * (j0 + u);
+          y[u] = col < N ? (fmaf(__ldcg(rr + col), inv_scale, __ldg(bias + col)) - mean) * rstd * __ldg(lg + col) + __ldg(lb + col)
+                         : 0.f;
+        }
+        act_store(y, j0);
       }
     }
   }
@@ -1197,11 +1247,11 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
   }
 
   if (kProf && P.prof) {
-    // rows: 0 TMA producer (warp 16 lane 0), 1 consumer warpgroup 0 (thread 0), 2 consumer warpgroup 3 (thread 384),
-    //       3 idle warp 17 during the GEMM
+    // rows: 0 TMA producer (warp 8 lane 0), 1 consumer warpgroup 0 (thread 0), 2 consumer warpgroup 1 (thread 128),
+    //       3 idle warp 9 during the GEMM
     // cols: 0 stage-empty wait cycles, 1 cycles inside layers, 2 stage-full wait, 3 publish, 4 tile set-up, 5 whole kernel,
     //       6 action pass, 7 refit
-    const int who = (threadIdx.x == kGProducerWarp * 32) ? 0 : (threadIdx.x == 0) ? 1 : (threadIdx.x == 384) ? 2
+    const int who = (threadIdx.x == kGProducerWarp * 32) ? 0 : (threadIdx.x == 0) ? 1 : (threadIdx.x == 128) ? 2
                     : (threadIdx.x == (kGProducerWarp + 1) * 32) ? 3 : -1;
     if (who >= 0) {
       long long* o = P.prof + (static_cast<size_t>(blockIdx.x) * 4 + who) * 12;
