@@ -39,7 +39,8 @@ extern "C" {
                                        4: tdmpc2_planner_set_passes (declared non-parity fast mode), set_kseg, iter_engine;
                                        5: pixel encoder (tdmpc2_pixel_*), tdmpc2_plan_prologue_latent, dims.num_enc_layers = 0;
                                        6: tdmpc2_plan_iter_rng (declared non-parity in-kernel noise), tdmpc2_debug_rng;
-                                       7: world-model methods on a flat batch (tdmpc2_wm_*, tdmpc2_td_target), target Q blob */
+                                       7: world-model methods on a flat batch (tdmpc2_wm_*, tdmpc2_td_target), target Q blob;
+                                          later, additive: tdmpc2_pixel_encode_rows (old callers and bindings unaffected) */
 #define TDMPC2_MAX_ENC_LAYERS 8
 
 typedef enum tdmpc2_status {
@@ -202,6 +203,13 @@ int tdmpc2_pixel_encoder_workspace_bytes(const tdmpc2_pixel_encoder* e, size_t* 
  *   z_out [E, 16 * num_channels]; workspace: caller-owned, tdmpc2_pixel_encoder_workspace_bytes. */
 int tdmpc2_pixel_encode(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
                         const float* shift, const float* grid_base, float* z_out, void* stream);
+/* The same encoder over any number of frames, e.g. WorldModel.encode(obs[1:]) of _update (tdmpc2.py:262) on a
+ * [T, B, C, 64, 64] batch flattened by the caller: frames [rows, C, 64, 64], shift [rows, 2], z_out [rows, 16 * num_channels].
+ * One launch, the same workspace as tdmpc2_pixel_encode (its size does not depend on rows), no allocation and no host
+ * synchronisation (capturable in a CUDA graph).  z of a frame is bit-identical to tdmpc2_pixel_encode's for the same
+ * frame and shift.  rows < 1 or a null pointer: TDMPC2_ERR_INVALID. */
+int tdmpc2_pixel_encode_rows(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
+                             const float* shift, const float* grid_base, int64_t rows, float* z_out, void* stream);
 
 /* Replaces ONE pass of the loop tdmpc2.py:173-197 (sample, _estimate_value
  * :122-136, topk, MPPI weights, refit) for all E environments.

@@ -19,7 +19,7 @@ SYMBOLS = [
     "tdmpc2_abi_version", "tdmpc2_last_error", "tdmpc2_planner_create", "tdmpc2_planner_destroy",
     "tdmpc2_planner_packed_bytes", "tdmpc2_planner_workspace_bytes", "tdmpc2_planner_bind",
     "tdmpc2_planner_set_engine", "tdmpc2_planner_iter_engine", "tdmpc2_planner_set_l2_persist", "tdmpc2_planner_set_kseg", "tdmpc2_planner_set_head_kseg", "tdmpc2_planner_set_passes", "tdmpc2_pack_weights", "tdmpc2_plan_prologue", "tdmpc2_plan_prologue_latent",
-    "tdmpc2_pixel_encoder_create", "tdmpc2_pixel_encoder_destroy", "tdmpc2_pixel_encoder_workspace_bytes", "tdmpc2_pixel_encode", "tdmpc2_plan_iter", "tdmpc2_plan_iter_rng", "tdmpc2_debug_rng",
+    "tdmpc2_pixel_encoder_create", "tdmpc2_pixel_encoder_destroy", "tdmpc2_pixel_encoder_workspace_bytes", "tdmpc2_pixel_encode", "tdmpc2_pixel_encode_rows", "tdmpc2_plan_iter", "tdmpc2_plan_iter_rng", "tdmpc2_debug_rng",
     "tdmpc2_plan_epilogue", "tdmpc2_plan_get_state", "tdmpc2_estimate_value", "tdmpc2_debug_layer",
     "tdmpc2_planner_layer_count", "tdmpc2_planner_launch_count", "tdmpc2_planner_set_profile",
     "tdmpc2_planner_target_q_bytes", "tdmpc2_planner_bind_target_q", "tdmpc2_pack_target_q",
@@ -100,6 +100,7 @@ def load():
     lib.tdmpc2_pixel_encoder_destroy.restype = None
     lib.tdmpc2_pixel_encoder_workspace_bytes.argtypes = [vp, C.POINTER(C.c_size_t)]
     lib.tdmpc2_pixel_encode.argtypes = [vp, vp, C.POINTER(ConvWeights), vp, vp, vp, vp, vp]
+    lib.tdmpc2_pixel_encode_rows.argtypes = [vp, vp, C.POINTER(ConvWeights), vp, vp, vp, i64, vp, vp]
     lib.tdmpc2_plan_iter.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.tdmpc2_plan_iter_rng.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp]
     lib.tdmpc2_debug_rng.argtypes = [vp, C.c_uint32, C.c_uint64, C.c_int, vp, vp]

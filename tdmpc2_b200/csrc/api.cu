@@ -5,6 +5,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -684,6 +685,7 @@ extern "C" int tdmpc2_plan_prologue_latent(tdmpc2_planner* p, const float* z, co
 // ------------------------------------------------------------------------------------ pixel encoder (cfg.obs == 'rgb')
 struct tdmpc2_pixel_encoder {
   tdmpc2_pixel_dims d;
+  int num_sms = 0;                 // the persistent grid's width: one conv1 scratch slot per SM
   size_t ws_bytes = 0, smem = 0;
   bool attr_done = false;
 };
@@ -697,13 +699,22 @@ extern "C" int tdmpc2_pixel_encoder_create(const tdmpc2_pixel_dims* dims, tdmpc2
   int num_sms = 0;
   int rc = check_device(&num_sms);
   if (rc) return rc;
+  // shared memory: the activations of the larger phase (staged frame / conv2-4 maps), plus every layer's weights and bias
+  // next to its activations when they fit the opt-in maximum; otherwise the kernel stages them in chunks
+  const size_t stage = pix_stage_floats(d.in_channels), maps = pix_maps_floats(d.num_channels), nc = d.num_channels;
+  const size_t want = std::max({stage + nc * (d.in_channels * 49 + 1), maps + nc * (nc * 25 + 1), std::max(stage, maps)});
+  const size_t smem = std::min(want * 4, static_cast<size_t>(kPixMaxSmem));
+  const int cap1 = static_cast<int>(smem / 4) - static_cast<int>(stage), cap2 = static_cast<int>(smem / 4) - static_cast<int>(maps);
+  int occ = 0, icc1 = 0, icc2 = 0, icc3 = 0;
+  if (cap1 > 0) pix_chunk(d.in_channels, d.num_channels, 49, cap1, &occ, &icc1);
+  if (cap2 > 0) { pix_chunk(d.num_channels, d.num_channels, 25, cap2, &occ, &icc2); pix_chunk(d.num_channels, d.num_channels, 9, cap2, &occ, &icc3); }
+  if (std::max(stage, maps) * 4 > static_cast<size_t>(kPixMaxSmem) || icc1 < 1 || icc2 < 1 || icc3 < 1)
+    return fail(TDMPC2_ERR_INVALID, "pixel encoder: %d input channels do not fit shared memory", d.in_channels);
   tdmpc2_pixel_encoder* e = new tdmpc2_pixel_encoder();
   e->d = d;
-  e->ws_bytes = align_up(static_cast<size_t>(d.num_envs) * d.num_channels * kPixO1 * kPixO1 * 4, 256);
-  const size_t stage = static_cast<size_t>(d.in_channels) * kPixHW * kPixHW;
-  const size_t maps = static_cast<size_t>(d.num_channels) * (kPixO2 * kPixO2 + kPixO3 * kPixO3 + kPixO4 * kPixO4);
-  e->smem = std::max(stage, maps) * 4;
-  if (e->smem > 227 * 1024) { delete e; return fail(TDMPC2_ERR_INVALID, "pixel encoder: %d input channels do not fit shared memory", d.in_channels); }
+  e->num_sms = num_sms;
+  e->ws_bytes = align_up(static_cast<size_t>(num_sms) * d.num_channels * kPixO1 * kPixO1 * 4, 256);
+  e->smem = smem;
   *out = e;
   return 0;
 }
@@ -713,21 +724,43 @@ extern "C" int tdmpc2_pixel_encoder_workspace_bytes(const tdmpc2_pixel_encoder* 
   *out = e->ws_bytes;
   return 0;
 }
-extern "C" int tdmpc2_pixel_encode(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
-                                   const float* shift, const float* grid_base, float* z_out, void* stream_) {
-  if (!e || !workspace || !w || !frames || !shift || !grid_base || !z_out) return fail(TDMPC2_ERR_INVALID, "null argument");
+
+// One launch over `rows` frames: min(rows, SMs) CTAs, each looping over its frames with its own conv1 scratch slot.
+static int pixel_launch(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
+                        const float* shift, const float* grid_base, int64_t rows, float* z_out, void* stream_) {
+  if (!workspace || !w || !frames || !shift || !grid_base || !z_out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (rows < 1) return fail(TDMPC2_ERR_INVALID, "rows must be >= 1");
   for (int i = 0; i < 4; ++i) if (!w->weight[i] || !w->bias[i]) return fail(TDMPC2_ERR_INVALID, "pixel encoder: null conv weight");
   PixelParams P{};
   P.frames = frames; P.shift = shift; P.grid = grid_base; P.scratch = static_cast<float*>(workspace); P.z = z_out;
   for (int i = 0; i < 4; ++i) { P.w[i] = w->weight[i]; P.b[i] = w->bias[i]; }
-  P.E = e->d.num_envs; P.C = e->d.in_channels; P.nc = e->d.num_channels; P.simnorm = e->d.simnorm_dim;
+  P.rows = rows; P.C = e->d.in_channels; P.nc = e->d.num_channels; P.simnorm = e->d.simnorm_dim;
+  P.smem_floats = static_cast<int>(e->smem / 4);
   if (!e->attr_done) {
     CUDA_TRY(cudaFuncSetAttribute(pixel_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(e->smem)));
     e->attr_done = true;
   }
-  pixel_encode_kernel<<<P.E, kPixThreads, e->smem, static_cast<cudaStream_t>(stream_)>>>(P);
+  const int grid = static_cast<int>(std::min<int64_t>(rows, e->num_sms));
+  pixel_encode_kernel<<<grid, kPixThreads, e->smem, static_cast<cudaStream_t>(stream_)>>>(P);
   CUDA_TRY(cudaGetLastError());
   return 0;
+}
+
+extern "C" int tdmpc2_pixel_encode(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
+                                   const float* shift, const float* grid_base, float* z_out, void* stream_) {
+  if (!e) return fail(TDMPC2_ERR_INVALID, "null argument");
+  return pixel_launch(e, workspace, w, frames, shift, grid_base, e->d.num_envs, z_out, stream_);
+}
+
+extern "C" int tdmpc2_pixel_encode_rows(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w,
+                                        const float* frames, const float* shift, const float* grid_base, int64_t rows,
+                                        float* z_out, void* stream_) {
+  if (!e) {                        // an encoder exists only where a device does: report the missing device first
+    int n = 0;
+    const int rc = check_device(&n);
+    return rc ? rc : fail(TDMPC2_ERR_INVALID, "null pixel encoder");
+  }
+  return pixel_launch(e, workspace, w, frames, shift, grid_base, rows, z_out, stream_);
 }
 
 extern "C" int tdmpc2_plan_iter(tdmpc2_planner* p, const float* noise_r, const float* noise_pi, const int32_t* qidx,

@@ -136,6 +136,16 @@ def draw_noise(cfg: Config, num_envs: int, device, eval_mode: bool = False,
     return nz
 
 
+def draw_shifts(lead, device, generator: Optional[torch.Generator] = None) -> torch.Tensor:
+    """ShiftAug's random shifts (layers.py:55) for WorldModel.encode of pixel frames with leading shape `lead`: [B] -> one
+    randint(0, 7) draw of (B, 2); [T, B] -> T draws of (B, 2) in order of t, because the reference encodes a 5-D batch
+    slice by slice (world_model.py:110-111).  (x, y) pairs as fp32, shape [*lead, 2]."""
+    kw = dict(device=device, dtype=torch.float32, generator=generator)
+    if len(lead) == 1:
+        return torch.randint(0, 7, (lead[0], 2), **kw)
+    return torch.stack([torch.randint(0, 7, (lead[1], 2), **kw) for _ in range(lead[0])])
+
+
 def discount_table(cfg: Config, device) -> torch.Tensor:
     """[num_tasks, H+1] fp32: the running `discount` of tdmpc2.py:125-132 after t steps.
     Single-task: a Python float product (double) cast to fp32 when it multiplies
@@ -343,6 +353,23 @@ class Planner:
             _cabi.check(self.lib.tdmpc2_pixel_encode(self.pix, self.pix_ws.data_ptr(), C.byref(self._conv), _ptr(frames),
                                                      _ptr(shift), _ptr(self.pix_grid), _ptr(self.pix_z), self._stream()))
         return self.pix_z
+
+    def encode_pixel_rows(self, frames, shift) -> torch.Tensor:
+        """z = encode(obs) for any number of pixel frames in one launch: frames [R, C, 64, 64] (any dtype, values 0..255),
+        shift [R, 2] (x, y) -> a fresh z [R, L].  Bit-identical to encode_pixels for the same frame and shift."""
+        if self.pix is None or self._conv is None:
+            raise _cabi.CabiError("encode_pixel_rows needs a cfg.obs == 'rgb' planner with packed weights")
+        frames = frames.to(self.device, torch.float32).contiguous()      # ShiftAug's x.float() (layers.py:44)
+        shift = shift.to(self.device, torch.float32).contiguous()
+        R = frames.shape[0]
+        if frames.ndim != 4 or tuple(frames.shape[1:]) != (self.cfg.obs_shape["rgb"][0], 64, 64) or tuple(shift.shape) != (R, 2):
+            raise ValueError(f"frames must be [R, {self.cfg.obs_shape['rgb'][0]}, 64, 64] and shift [R, 2]; got "
+                             f"{tuple(frames.shape)} and {tuple(shift.shape)}")
+        z = self._rows_out(R, self.cfg.latent_dim)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_pixel_encode_rows(self.pix, self.pix_ws.data_ptr(), C.byref(self._conv), _ptr(frames),
+                                                          _ptr(shift), _ptr(self.pix_grid), R, _ptr(z), self._stream()))
+        return z
 
     def prologue_latent(self, z, task, t0, prev_mean, noise_prior) -> None:
         self._keep = [z, task, t0, prev_mean, noise_prior]

@@ -28,7 +28,7 @@ from typing import List, Optional
 import torch
 import torch.nn as nn
 
-from .planner import Planner
+from .planner import Planner, draw_shifts
 from .synth import QS_PREFIXES, synth_state_dict
 
 _LAYER_PARAM_NAMES = ("weight", "bias", "ln.weight", "ln.bias")
@@ -174,13 +174,30 @@ class WorldModel(nn.Module):
         t = torch.as_tensor(task, device=pl.device).reshape(-1).to(torch.int32)
         return t.expand(*lead).reshape(-1).contiguous()
 
-    def encode(self, obs, task):
-        """world_model.py:103-112 (state observations): obs [..., obs_dim] -> z [..., L]."""
+    def encode(self, obs, task, *, shift: Optional[torch.Tensor] = None):
+        """world_model.py:103-112: obs [..., obs_dim] -> z [..., L].  Pixel models (layers.py:36-59,136-150): frames
+        [B, C, 64, 64] -> z [B, L], or [T, B, C, 64, 64] -> z [T, B, L] in one launch; `shift` [..., 2] (x, y) (default:
+        ShiftAug's randint draws from the agent's generator, one (B, 2) draw per t, like the reference's slice loop)."""
         if self.cfg.get("obs", "state") == "rgb":
-            raise NotImplementedError("row-batched pixel encoding is not built: the pixel encoder is sized per environment")
+            return self._encode_rgb(obs, shift)
         pl = self._kernels()
         lead = obs.shape[:-1]
         return pl.wm_encode(self._rows(pl, obs), self._task_rows(pl, task, lead)).view(*lead, -1)
+
+    def _encode_rgb(self, obs, shift):
+        agent = self._agent() if self._agent is not None else None
+        if agent is None and self.tensor(self._keys[0]).device.type != "cuda":
+            raise NotImplementedError("pixel encoding runs on the sm_90a conv-encoder kernel: move the model to a CUDA "
+                                      "device (there is no CPU fallback)")
+        C_in = self.cfg.obs_shape["rgb"][0]
+        if obs.ndim not in (4, 5) or tuple(obs.shape[-3:]) != (C_in, 64, 64):
+            raise ValueError(f"pixel obs must be [B, {C_in}, 64, 64] or [T, B, {C_in}, 64, 64]; got {tuple(obs.shape)}")
+        pl = self._kernels()
+        lead = tuple(obs.shape[:-3])
+        shift = draw_shifts(lead, pl.device, self._generator()) if shift is None else torch.as_tensor(shift)
+        if tuple(shift.shape) != lead + (2,):
+            raise ValueError(f"shift must be {list(lead) + [2]}; got {tuple(shift.shape)}")
+        return pl.encode_pixel_rows(obs.reshape(-1, C_in, 64, 64), shift.reshape(-1, 2)).view(*lead, -1)
 
     def next(self, z, a, task):
         """world_model.py:114-121: z [..., L], a [..., A] -> z' [..., L]."""
