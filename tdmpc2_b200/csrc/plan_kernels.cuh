@@ -505,6 +505,34 @@ __device__ __forceinline__ float simnorm_lane(float y, bool valid) {
 constexpr int kLnRegCols = 16;   // columns per lane of a 512-wide row
 constexpr int kLnBatch = 8;      // columns per lane that the output pass carries through activation and stores at once
 
+// Row staging.  A row phase is latency-bound: a warp that loads a row when it starts on it waits for an L2 round trip
+// per row.  The operand ring is idle from the end of a GEMM (its __syncthreads: every TMA load has landed and been
+// consumed) to the next layer's first TMA load (after publish_planes' proxy fence and barrier), so each warp owns two
+// kStageCols-float buffers there.  While the warp works on row r from one, cp.async (L2 only, no registers held) copies
+// row r + kWarps of raw into the other.
+constexpr int kStageCols = 512;
+static_assert(kWarps * 2 * kStageCols * 4 <= kStages * kStageBytes, "row staging buffers");
+__device__ __forceinline__ float* row_stage(const Ctx& c, int i) {
+  return reinterpret_cast<float*>(c.stage_base) + (c.warp * 2 + (i & 1)) * kStageCols;
+}
+// copy columns [0, ncols) of raw row r to dst (ncols <= kStageCols, a multiple of 4; raw rows are 16-byte aligned and
+// written by the GEMM up to Npad) as one commit group
+__device__ __forceinline__ void stage_row(const PlanParams& P, const Ctx& c, int r, int ncols, float* dst) {
+  const float* src = raw_ptr(P, c.slot) + static_cast<size_t>(r) * P.NpadMax;
+  for (int q = 4 * c.lane; q < ncols; q += 4 * 32) ptx::cp_async_16(dst + q, src + q);
+  ptx::cp_async_commit();
+}
+// Iteration i of a warp's row loop (row r; row r was staged into buffer i by the previous iteration or before the loop):
+// stage row r + kWarps into buffer i + 1, wait for row r and make it visible to the whole warp.  The loop body must end
+// with __syncwarp() so that no lane still reads buffer i when iteration i + 1 refills it.
+__device__ __forceinline__ const float* stage_advance(const PlanParams& P, const Ctx& c, int r, int i, int ncols) {
+  if (r + kWarps < kTileM) stage_row(P, c, r + kWarps, ncols, row_stage(c, i + 1));
+  else ptx::cp_async_commit();   // an empty group: "all but the newest group" is then always row r
+  ptx::cp_async_wait<1>();
+  __syncwarp();
+  return row_stage(c, i);
+}
+
 // Mish(x) = x * tanh(softplus(x)) (layers.py:103; softplus threshold 20) of a lane's batch of columns.
 // tanh(log(1+e^x)) = n / (n + 2) with n = e^x (e^x + 2): one exp, one divide, no cancellation.  Three passes over the
 // batch, so that its independent exp / divide chains overlap: a divide is a branch (its slow-path call), and a
@@ -528,9 +556,11 @@ __device__ __forceinline__ void mish_batch(float (&y)[kLnBatch]) {
 // through the read-only path (__ldg).  The output pass works on batches of kLnBatch columns per lane: every load of a
 // batch is issued before its first store (the stores go through pointers that may alias raw as far as the compiler
 // knows), and the batch's activations are independent chains that overlap.
-//   - 512-wide rows (every hidden layer of the 5M model): raw is read once; the 16 values per lane stay in registers from
-//     the statistics through the output pass.
-//   - other widths: raw is read once per statistic and once in the output pass.
+//   - 512-wide rows (every hidden layer of the 5M model): raw is read once, through the staging buffers, so that the next
+//     row's copy overlaps this row's work; the 16 values per lane stay in registers from the statistics through the
+//     output pass.  (Holding the next row in registers instead spills it: the row phase shares the kernel's 168.)
+//   - other widths: raw is read once per statistic and once in the output pass.  (Statistics loads in guarded batches
+//     of kLnBatch were measured slower on c3's 1792-wide rows than these loops, which ptxas unrolls with unguarded loads.)
 // Every column's value is the same expression in the same order in both paths: same bits.
 __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const LayerRec& ly, const EpiArgs& ea) {
   const float* rawbase = raw_ptr(P, c.slot);
@@ -542,41 +572,42 @@ __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const L
   const float inv_scale = ly.inv_scale;
   const float* bias = ly.bias; const float* lg = ly.ln_g; const float* lb = ly.ln_b;
   const int ncolj = (N + 31) / 32;
-  for (int r = c.warp; r < kTileM; r += kWarps) {
-    const float* rr = rawbase + static_cast<size_t>(r) * P.NpadMax;
+  // activation and stores of row r's batch y = columns lane + 32 (j0 + u); warp-uniform (SimNorm shuffles across lanes)
+  auto act_store = [&](float (&y)[kLnBatch], int j0, int r) {
+    if (ea.kind == EPI_LN_MISH) {
+      mish_batch(y);
+    } else {
+#pragma unroll
+      for (int u = 0; u < kLnBatch; ++u)
+        if (j0 + u < ncolj) y[u] = simnorm_lane(y[u], c.lane + 32 * (j0 + u) < N);
+    }
+    if (dhi) {
+      __half* hi = dhi + static_cast<size_t>(r) * pitch + ea.dst_col0;
+      __half* lo = dlo + static_cast<size_t>(r) * pitch + ea.dst_col0;
+#pragma unroll
+      for (int u = 0; u < kLnBatch; ++u) {
+        const int col = c.lane + 32 * (j0 + u);
+        if (col < N) split_store(hi + col, lo + col, y[u]);
+      }
+    }
     const int orow = ea.rowmap ? ea.rowmap[r] : r;
-    // activation and stores of the batch y = columns lane + 32 (j0 + u); warp-uniform (SimNorm shuffles across lanes)
-    auto act_store = [&](float (&y)[kLnBatch], int j0) {
-      if (ea.kind == EPI_LN_MISH) {
-        mish_batch(y);
-      } else {
+    if (ea.out_f32 && orow >= 0) {
+      float* o = ea.out_f32 + static_cast<size_t>(orow) * ea.out_pitch;
 #pragma unroll
-        for (int u = 0; u < kLnBatch; ++u)
-          if (j0 + u < ncolj) y[u] = simnorm_lane(y[u], c.lane + 32 * (j0 + u) < N);
+      for (int u = 0; u < kLnBatch; ++u) {
+        const int col = c.lane + 32 * (j0 + u);
+        if (col < N) o[col] = y[u];
       }
-      if (dhi) {
-        __half* hi = dhi + static_cast<size_t>(r) * pitch + ea.dst_col0;
-        __half* lo = dlo + static_cast<size_t>(r) * pitch + ea.dst_col0;
-#pragma unroll
-        for (int u = 0; u < kLnBatch; ++u) {
-          const int col = c.lane + 32 * (j0 + u);
-          if (col < N) split_store(hi + col, lo + col, y[u]);
-        }
-      }
-      if (ea.out_f32 && orow >= 0) {
-        float* o = ea.out_f32 + static_cast<size_t>(orow) * ea.out_pitch;
-#pragma unroll
-        for (int u = 0; u < kLnBatch; ++u) {
-          const int col = c.lane + 32 * (j0 + u);
-          if (col < N) o[col] = y[u];
-        }
-      }
-    };
-    if (N == 32 * kLnRegCols) {
-      // The loads are unconditional and all issued before the first use: the row costs one L2 round trip.
+    }
+  };
+  if (N == 32 * kLnRegCols) {
+    // Rows arrive through the warp's staging buffers (see stage_row): row r + kWarps is copied while row r is computed.
+    stage_row(P, c, c.warp, N, row_stage(c, 0));
+    for (int r = c.warp, i = 0; r < kTileM; r += kWarps, ++i) {
+      const float* row = stage_advance(P, c, r, i, N);
       float x[kLnRegCols];
 #pragma unroll
-      for (int j = 0; j < kLnRegCols; ++j) x[j] = __ldcg(rr + c.lane + 32 * j);
+      for (int j = 0; j < kLnRegCols; ++j) x[j] = row[c.lane + 32 * j];
       float s = 0.f;
 #pragma unroll
       for (int j = 0; j < kLnRegCols; ++j) {
@@ -600,9 +631,13 @@ __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const L
           const int col = c.lane + 32 * (j0 + u);
           y[u] = (x[j0 + u] - mean) * rstd * __ldg(lg + col) + __ldg(lb + col);
         }
-        act_store(y, j0);
+        act_store(y, j0, r);
       }
-    } else {
+      __syncwarp();   // every lane has read buffer i before the next iteration refills it
+    }
+  } else {
+    for (int r = c.warp; r < kTileM; r += kWarps) {
+      const float* rr = rawbase + static_cast<size_t>(r) * P.NpadMax;
       float s = 0.f;
       for (int col = c.lane; col < N; col += 32) s += fmaf(__ldcg(rr + col), inv_scale, __ldg(bias + col));
       const float mean = warp_sum(s) * invN;
@@ -621,29 +656,39 @@ __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const L
           y[u] = col < N ? (fmaf(__ldcg(rr + col), inv_scale, __ldg(bias + col)) - mean) * rstd * __ldg(lg + col) + __ldg(lb + col)
                          : 0.f;
         }
-        act_store(y, j0);
+        act_store(y, j0, r);
       }
     }
   }
 }
 
-// Head output row -> smem row buffer: out[col] = raw*inv_scale + bias (plain Linear, no LN).
-__device__ __forceinline__ void head_row_to_smem(const PlanParams& P, Ctx& c, const LayerRec& ly, int r, float* buf) {
-  const float* rr = raw_ptr(P, c.slot) + static_cast<size_t>(r) * P.NpadMax;
-  for (int col = c.lane; col < ly.N; col += 32) buf[col] = fmaf(__ldcg(rr + col), ly.inv_scale, ly.bias[col]);
-  __syncwarp();
-}
+// A head row is at most kMaxHeadCols wide: kHeadRegCols columns per lane (lane + 32 j) fit in registers.
+constexpr int kHeadRegCols = kMaxHeadCols / 32;
+static_assert(kMaxHeadCols <= kStageCols, "a head row fits a staging buffer");
 
-// two_hot_inv (math.py:74-83): softmax over the bins, expectation under linspace(vmin,vmax,B), symexp.
-__device__ __forceinline__ float two_hot_inv_row(const PlanParams& P, Ctx& c, const float* buf) {
+// two_hot_inv (math.py:74-83): softmax over the bins, expectation under linspace(vmin,vmax,B), symexp.  y = the lane's
+// logits (columns lane + 32 j < B); per bin and per lane the same expressions in the same order as a strided loop.
+__device__ __forceinline__ float two_hot_inv_row(const PlanParams& P, Ctx& c, const float (&y)[kHeadRegCols]) {
+  float bin[kHeadRegCols];
+#pragma unroll
+  for (int j = 0; j < kHeadRegCols; ++j) bin[j] = c.lane + 32 * j < P.B ? __ldg(P.bins + c.lane + 32 * j) : 0.f;
   float m = -CUDART_INF_F;
-  for (int col = c.lane; col < P.B; col += 32) m = fmaxf(m, buf[col]);
+#pragma unroll
+  for (int j = 0; j < kHeadRegCols; ++j)
+    if (c.lane + 32 * j < P.B) m = fmaxf(m, y[j]);
   m = warp_max(m);
+  float e[kHeadRegCols];
   float s = 0.f;
-  for (int col = c.lane; col < P.B; col += 32) s += expf(buf[col] - m);
+#pragma unroll
+  for (int j = 0; j < kHeadRegCols; ++j) {
+    e[j] = expf(y[j] - m);
+    if (c.lane + 32 * j < P.B) s += e[j];
+  }
   s = warp_sum(s);
   float acc = 0.f;
-  for (int col = c.lane; col < P.B; col += 32) acc = fmaf(__fdiv_rn(expf(buf[col] - m), s), P.bins[col], acc);
+#pragma unroll
+  for (int j = 0; j < kHeadRegCols; ++j)
+    if (c.lane + 32 * j < P.B) acc = fmaf(__fdiv_rn(e[j], s), bin[j], acc);
   acc = warp_sum(acc);
   return symexp_f(acc);
 }
@@ -698,46 +743,68 @@ __device__ __forceinline__ void rows_pi(const PlanParams& P, Ctx& c, const float
   if (P.rows_out4 && row >= 0 && c.lane == 0) { P.rows_out4[2 * static_cast<size_t>(row)] = lp; P.rows_out4[2 * static_cast<size_t>(row) + 1] = sq; }
 }
 
+// Planning pi head (PRIOR / ITER / VALUE) for tile row r: the sampled action goes to the X action columns and, for the
+// policy prior, to pi_actions.
+__device__ __forceinline__ void pi_row(const PlanParams& P, Ctx& c, const EpiArgs& ea, const float* myrow, int r, __half* xhi, __half* xlo) {
+  const RowMap rm = map_row(P, ea.tile, r);
+  const int e = rm.env < 0 ? 0 : rm.env, idx = rm.env < 0 ? 0 : rm.idx;
+  const int task = P.task ? P.task[e] : 0;
+  for (int a = c.lane; a < P.A; a += 32) {
+    const float eps = ea.eps_base ? __ldcs(&ea.eps_base[(static_cast<size_t>(e) * ea.eps_rows + idx) * P.A + a])
+                                  : noise_pi_at(P, e, idx, a);        // eps_base == nullptr: in-kernel noise (ITER)
+    const float act = pi_action(P, myrow[a], myrow[P.Apad + a], eps, task, a);
+    const size_t o = static_cast<size_t>(r) * P.KpadX + P.L + P.T + a;
+    split_store(xhi + o, xlo + o, act);
+    if (ea.act_out && rm.env >= 0)
+      ea.act_out[((static_cast<size_t>(e) * P.H + ea.t_out) * P.P + idx) * P.A + a] = act;
+  }
+}
+
 template <bool EPISODIC, bool ROWS>
 __device__ __forceinline__ void rows_head(const PlanParams& P, Ctx& c, const LayerRec& ly, const EpiArgs& ea) {
   float* myrow = c.rowbuf + c.warp * kMaxHeadCols;
   __half* xhi = plane_ptr(P, c.slot, BUF_X, 0);
   __half* xlo = plane_ptr(P, c.slot, BUF_X, 1);
-  for (int r = c.warp; r < kTileM; r += kWarps) {
+  const int N = ly.N;
+  // Rows arrive through the warp's staging buffers like rows_ln_act's 512-wide rows.  Heads are at most kMaxHeadCols
+  // wide; only a diagnostic MODE_LAYER EPI_RAW row can be wider than a buffer, and it reads raw directly.
+  const bool staged = N <= kStageCols;
+  const int n4 = (N + 3) & ~3;
+  if (staged) stage_row(P, c, c.warp, n4, row_stage(c, 0));
+  for (int r = c.warp, i = 0; r < kTileM; r += kWarps, ++i) {
+    const float* row = staged ? stage_advance(P, c, r, i, n4) : raw_ptr(P, c.slot) + static_cast<size_t>(r) * P.NpadMax;
     if (ea.kind == EPI_RAW) {
       const int orow = ea.rowmap ? ea.rowmap[r] : r;
-      const float* rr = raw_ptr(P, c.slot) + static_cast<size_t>(r) * P.NpadMax;
       if (orow >= 0)
-        for (int col = c.lane; col < ly.N; col += 32) {
-          float v = fmaf(__ldcg(rr + col), ly.inv_scale, ly.bias[col]);
+        for (int col = c.lane; col < N; col += 32) {
+          float v = fmaf(row[col], ly.inv_scale, __ldg(ly.bias + col));
           if (ROWS && ea.head) v = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-v)));      // termination: sigmoid
           ea.out_f32[static_cast<size_t>(orow) * ea.out_pitch + col] = v;
         }
-      continue;
-    }
-    head_row_to_smem(P, c, ly, r, myrow);
-    if (EPISODIC && ea.kind == EPI_TERM) {
-      if (c.lane == 0) term_commit(c, r, myrow[0]);
-    } else if (ROWS && ea.kind == EPI_TWOHOT) {
-      const float v = two_hot_inv_row(P, c, myrow);
-      if (c.lane == 0) rows_commit(P, c, ea, r, v);
-    } else if (ROWS && ea.kind == EPI_PI) {
-      rows_pi(P, c, myrow, r, xhi, xlo);
-    } else if (ea.kind == EPI_TWOHOT) {
-      const float v = two_hot_inv_row(P, c, myrow);
-      if (c.lane == 0) head_commit<EPISODIC>(P, c, ea, r, v);
-    } else if (ea.kind == EPI_PI) {
-      const RowMap rm = map_row(P, ea.tile, r);
-      const int e = rm.env < 0 ? 0 : rm.env, idx = rm.env < 0 ? 0 : rm.idx;
-      const int task = P.task ? P.task[e] : 0;
-      for (int a = c.lane; a < P.A; a += 32) {
-        const float eps = ea.eps_base ? __ldcs(&ea.eps_base[(static_cast<size_t>(e) * ea.eps_rows + idx) * P.A + a])
-                                      : noise_pi_at(P, e, idx, a);        // eps_base == nullptr: in-kernel noise (ITER)
-        const float act = pi_action(P, myrow[a], myrow[P.Apad + a], eps, task, a);
-        const size_t o = static_cast<size_t>(r) * P.KpadX + P.L + P.T + a;
-        split_store(xhi + o, xlo + o, act);
-        if (ea.act_out && rm.env >= 0)
-          ea.act_out[((static_cast<size_t>(e) * P.H + ea.t_out) * P.P + idx) * P.A + a] = act;
+    } else {
+      // out[col] = raw * inv_scale + bias (plain Linear, no LN), the lane's columns lane + 32 j in registers
+      float y[kHeadRegCols];
+#pragma unroll
+      for (int j = 0; j < kHeadRegCols; ++j) {
+        const int col = c.lane + 32 * j;
+        y[j] = col < N ? fmaf(row[col], ly.inv_scale, __ldg(ly.bias + col)) : 0.f;
+      }
+      if (EPISODIC && ea.kind == EPI_TERM) {
+        if (c.lane == 0) term_commit(c, r, y[0]);
+      } else if (ea.kind == EPI_TWOHOT) {
+        const float v = two_hot_inv_row(P, c, y);
+        if (c.lane == 0) {
+          if (ROWS) rows_commit(P, c, ea, r, v);
+          else head_commit<EPISODIC>(P, c, ea, r, v);
+        }
+      } else if (ea.kind == EPI_PI) {
+        // the pi head reads its mean and log_std columns (a, Apad + a) through the warp's smem row buffer
+#pragma unroll
+        for (int j = 0; j < kHeadRegCols; ++j)
+          if (c.lane + 32 * j < N) myrow[c.lane + 32 * j] = y[j];
+        __syncwarp();
+        if (ROWS) rows_pi(P, c, myrow, r, xhi, xlo);
+        else pi_row(P, c, ea, myrow, r, xhi, xlo);
       }
     }
     __syncwarp();

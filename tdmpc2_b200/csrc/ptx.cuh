@@ -79,6 +79,16 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void* p, size_t bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;\n" ::"l"(a0), "r"(static_cast<uint32_t>(a1 - a0)) : "memory");
 }
 
+// ------------------------------------------------------------------ cp.async (per-thread asynchronous copies)
+// 16 bytes global -> shared through L2 only (.cg); completion is tracked per thread in commit groups.
+__device__ __forceinline__ void cp_async_16(void* smem_dst, const void* gsrc) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+// wait until at most N of this thread's committed groups are still pending
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
+
 // ------------------------------------------------------------------ wgmma
 // Shared-memory matrix descriptor (sm_90 wgmma), K-major operand, 128-byte swizzle, tile rows of 64 fp16 (128 B),
 // 8-row swizzle atoms 1024 B apart (SBO):
