@@ -61,6 +61,18 @@ CASES = {
     # refits dominated by one elite and clamped to min_std -- branches the init-scale cases never reach
     "tiny_sharp": ("tiny", {}, 18, True, 1.0,
                    [(True, False, None, 530), (False, False, None, 531), (False, True, None, 532)]),
+    # corners of the shape envelope tdmpc2_planner_create accepts (tests/test_gpu_shape_envelope.py): an odd L + T (the
+    # scalar action pass), a one-dimensional task action space and two-bin heads
+    "tiny_mt_t5": ("tiny-mt", {"task_dim": 5, "action_dims": [5, 1, 4, 2], "num_bins": 2, "vmin": -3, "vmax": 3}, 19, True, 60.0,
+                   [(True, False, 1, 540), (False, False, 1, 541), (False, True, 3, 542), (True, False, 0, 543)]),
+    # 256-column heads (pad32(128) + 128 and num_bins = 256) on a latent of one SimNorm group
+    "tiny_wide_heads": ("tiny", {"action_dim": 128, "num_bins": 256, "latent_dim": 8}, 20, True, 1.0,
+                        [(True, False, None, 550), (False, False, None, 551), (False, True, None, 552)]),
+    # LayerNorm rows one past 512, a latent that is not a multiple of 32, scratch pitches set by the encoder
+    # (obs_dim + T > L + T + A, enc_dim > mlp_dim) and a full 128-trajectory prior tile
+    "tiny_odd_widths": ("tiny", {"mlp_dim": 513, "latent_dim": 40, "enc_dim": 600, "obs_dim": 700, "num_pi_trajs": 128,
+                                 "num_samples": 256}, 21, True, 1.0,
+                        [(True, False, None, 560), (False, False, None, 561), (False, True, None, 562)]),
 }
 TRAINED = {"tiny_sharp": ("sharp", 218)}     # name -> (trained_scale level, seed)
 OBS_SCALE = {"tiny_sharp": 30.0}

@@ -133,6 +133,10 @@ CASES = {
     "tiny_mt_wm": ("tiny-mt", {}, 22, 122, 60.0, 3, 50, 610),     # per-row tasks; emb_scale 60 exercises max_norm
     "tiny_episodic_wm": ("tiny", {"episodic": True}, 23, 123, 1.0, 3, 50, 620),
     "c1_dog5m_wm": ("c1", {}, 24, 124, 1.0, 3, 10, 630),           # 512-wide rows: the register LayerNorm path
+    # corners of the shape envelope: an odd L + T and a one-dimensional task action space; 256-column heads on a latent
+    # of one SimNorm group (a few rows each: tests/test_gpu_shape_envelope.py compares 200-row batches with the oracle)
+    "tiny_mt_t5_wm": ("tiny-mt", {"task_dim": 5, "action_dims": [5, 1, 4, 2]}, 26, 126, 60.0, 1, 6, 650),
+    "tiny_wide_heads_wm": ("tiny", {"action_dim": 128, "num_bins": 256, "latent_dim": 8}, 27, 127, 1.0, 1, 2, 660),
 }
 # Trained-scale cases (same fields), kept apart from CASES because fixed fp32 tolerances do not apply to them:
 # TRAINED gives the synth.trained_scale (level, seed) applied after the target blend -- peaked two-hot heads with values

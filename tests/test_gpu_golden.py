@@ -9,7 +9,7 @@ from helpers import load_golden, stable_positions, boundary_separated
 pytestmark = pytest.mark.gpu
 
 CASES = ["tiny", "tiny_mt", "c1_dog5m", "c3_humanoid48m_e1", "c4_mt80_317m_e1", "tiny_episodic", "c1_dog5m_episodic", "tiny_rgb",
-         "tiny_nopi", "tiny_h1", "tiny_knobs"]
+         "tiny_nopi", "tiny_h1", "tiny_knobs", "tiny_mt_t5", "tiny_wide_heads", "tiny_odd_widths"]
 # A termination decision flips a trajectory value by O(1): samples whose termination logit lies within this margin
 # of the 0.5 boundary (by the oracle, which is bit-identical to the reference) are not compared.
 TERM_MARGIN = 2e-5

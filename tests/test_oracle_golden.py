@@ -7,6 +7,7 @@ from oracle.plan_oracle import draw_noise, plan_oracle
 from helpers import load_golden, stable_positions, boundary_separated
 
 CASES = ["tiny", "tiny_mt", "c1_dog5m", "tiny_episodic", "c1_dog5m_episodic", "tiny_rgb", "tiny_nopi", "tiny_h1", "tiny_knobs",
+         "tiny_mt_t5", "tiny_wide_heads", "tiny_odd_widths",
          pytest.param("c3_humanoid48m_e1", marks=pytest.mark.slow),
          pytest.param("c4_mt80_317m_e1", marks=pytest.mark.slow)]
 
