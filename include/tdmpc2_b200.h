@@ -40,7 +40,8 @@ extern "C" {
                                        5: pixel encoder (tdmpc2_pixel_*), tdmpc2_plan_prologue_latent, dims.num_enc_layers = 0;
                                        6: tdmpc2_plan_iter_rng (declared non-parity in-kernel noise), tdmpc2_debug_rng;
                                        7: world-model methods on a flat batch (tdmpc2_wm_*, tdmpc2_td_target), target Q blob;
-                                          later, additive: tdmpc2_pixel_encode_rows (old callers and bindings unaffected) */
+                                          later, additive: tdmpc2_pixel_encode_rows (old callers and bindings unaffected);
+                                          later, additive: agent.update_pi (tdmpc2_pi_loss_*, tdmpc2_pi_grads) */
 #define TDMPC2_MAX_ENC_LAYERS 8
 
 typedef enum tdmpc2_status {
@@ -287,6 +288,35 @@ int tdmpc2_wm_q(tdmpc2_planner* p, const float* z, const float* a, const int32_t
  * reward, terminated [rows, 1]. */
 int tdmpc2_td_target(tdmpc2_planner* p, const float* next_z, const float* reward, const float* terminated,
                      const int32_t* task, const float* eps, const int32_t* qidx, int rows, float* out, void* stream);
+
+/* ---- agent.update_pi (tdmpc2.py:208-239) ------------------------------------------------------------------------
+ * The policy loss of a [T, B] batch of latents zs (rows = T B, row r = t B + b):
+ *   action = pi(zs) with eps [rows, A]; q = Q(zs, action, 'avg') of the ONLINE heads qidx[0], qidx[1] (detached: the Q
+ *   weights get no gradient, the action does); loss = mean_t rho^t mean_b -(entropy_coef scaled_entropy + q / scale).
+ * forward: one launch of the fused row kernel.  It writes action_out [rows, A], q_out [rows, 1], log_prob_out [rows, 2]
+ * (as tdmpc2_wm_pi's) and the caller-owned tape [tape_bytes] the backward reads.  dropout_mask: NULL (eval mode) or
+ * [num_q, rows, mlp_dim] = the train-mode Dropout(cfg.dropout) scale mask / (1 - p) of Q layer 0 (layers.py:104-108),
+ * head h's rows at h rows mlp_dim; applied to the pre-LayerNorm output.
+ * backward: from the tape, the same eps / qidx / dropout_mask and task, the fp32 state-dict tensors w->pi, w->qs, and
+ * scale [1] (device memory: RunningScale.value), ADDS dL/dparameter to grads (like autograd accumulates .grad):
+ * _pi.{0,1,2}.weight / .bias, _pi.{0,1}.ln.weight / .ln.bias, and for multi-task models _task_emb.weight.grad (pi's and
+ * both Q heads' layer-0 inputs).  Reductions over rows run in a fixed order: repeated calls give identical bits.
+ * workspace: caller-owned, workspace_bytes(rows).  No allocation, no host synchronisation (capturable). */
+typedef struct tdmpc2_pi_grads {
+  float* weight[3];
+  float* bias[3];
+  float* ln_weight[2];
+  float* ln_bias[2];
+  float* task_emb;         /* [num_tasks, T]; NULL for single-task models */
+} tdmpc2_pi_grads;
+int tdmpc2_pi_loss_tape_bytes(const tdmpc2_planner* p, int rows, size_t* out);
+int tdmpc2_pi_loss_workspace_bytes(const tdmpc2_planner* p, int rows, size_t* out);
+int tdmpc2_pi_loss_forward(tdmpc2_planner* p, const float* z, const int32_t* task, const float* eps, const int32_t* qidx,
+                           const float* dropout_mask, int rows, float* tape, float* action_out, float* q_out,
+                           float* log_prob_out, void* stream);
+int tdmpc2_pi_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* z, const int32_t* task,
+                            const float* eps, const int32_t* qidx, const float* dropout_mask, int T, int B, const float* scale,
+                            float entropy_coef, float rho, const tdmpc2_pi_grads* grads, void* workspace, void* stream);
 
 /* Diagnostics: y[rows, out] = act(LN(x W^T + b)) for ONE packed layer, through
  * the same fused kernels (rows <= 128).  layer index: 0.. = enc, then dynamics

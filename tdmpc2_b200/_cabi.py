@@ -24,7 +24,8 @@ SYMBOLS = [
     "tdmpc2_planner_layer_count", "tdmpc2_planner_launch_count", "tdmpc2_planner_set_profile",
     "tdmpc2_planner_target_q_bytes", "tdmpc2_planner_bind_target_q", "tdmpc2_pack_target_q",
     "tdmpc2_wm_encode", "tdmpc2_wm_next", "tdmpc2_wm_reward", "tdmpc2_wm_termination", "tdmpc2_wm_pi", "tdmpc2_wm_q",
-    "tdmpc2_td_target",
+    "tdmpc2_td_target", "tdmpc2_pi_loss_tape_bytes", "tdmpc2_pi_loss_workspace_bytes", "tdmpc2_pi_loss_forward",
+    "tdmpc2_pi_loss_backward",
 ]
 
 
@@ -53,6 +54,11 @@ class PixelDims(C.Structure):
 
 class ConvWeights(C.Structure):
     _fields_ = [("weight", C.c_void_p * 4), ("bias", C.c_void_p * 4)]
+
+
+class PiGrads(C.Structure):
+    _fields_ = [("weight", C.c_void_p * 3), ("bias", C.c_void_p * 3), ("ln_weight", C.c_void_p * 2),
+                ("ln_bias", C.c_void_p * 2), ("task_emb", C.c_void_p)]
 
 
 class CabiError(RuntimeError):
@@ -122,6 +128,11 @@ def load():
     lib.tdmpc2_wm_pi.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
     lib.tdmpc2_wm_q.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]
     lib.tdmpc2_td_target.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_int, vp, vp]
+    lib.tdmpc2_pi_loss_tape_bytes.argtypes = [vp, C.c_int, C.POINTER(C.c_size_t)]
+    lib.tdmpc2_pi_loss_workspace_bytes.argtypes = [vp, C.c_int, C.POINTER(C.c_size_t)]
+    lib.tdmpc2_pi_loss_forward.argtypes = [vp, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
+    lib.tdmpc2_pi_loss_backward.argtypes = [vp, C.POINTER(Weights), vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, C.c_float,
+                                            C.c_float, C.POINTER(PiGrads), vp, vp]
     for s in SYMBOLS:
         f = getattr(lib, s)
         if f.restype is C.c_int and s not in ("tdmpc2_abi_version", "tdmpc2_planner_layer_count"):

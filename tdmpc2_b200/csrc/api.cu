@@ -16,6 +16,7 @@
 
 #include "../../include/tdmpc2_b200.h"
 #include "plan_kernels.cuh"
+#include "grad_kernels.cuh"
 #include "pixel_encoder.cuh"
 
 using namespace tdmpc2;
@@ -1017,4 +1018,175 @@ extern "C" int tdmpc2_td_target(tdmpc2_planner* p, const float* next_z, const fl
   prm.rows_in = next_z; prm.rows_eps = eps; prm.qidx = qidx;
   prm.rows_reward = reward; prm.rows_term = terminated; prm.rows_out = out;
   return launch(p, prm, stream_);
+}
+
+// ------------------------------------------------------------------------------------ agent.update_pi (ROP_PI_LOSS + grad_kernels.cuh)
+static PiTape planner_tape(const tdmpc2_planner* p) {
+  return pi_tape(p->d.mlp_dim, p->d.action_dim, pad_to(p->d.action_dim, 32), p->d.num_bins);
+}
+
+// Workspace of the backward, in floats: the per-row gradients of every layer it walks through, and the split-K
+// partials of the dW reductions (nsplit row blocks, summed in order by pl_reduce).
+struct PiWs {
+  size_t dl, gq, gq2, dxq, dlog, gp, gp2, dyn, dy, hb, xb, dxe, part, floats;
+  int nsplit;
+};
+static PiWs pi_ws(const tdmpc2_planner* p, int rows) {
+  const tdmpc2_dims& d = p->d;
+  const size_t R = rows, M = d.mlp_dim, nb = d.num_bins, TA = d.task_dim + d.action_dim, LT = d.latent_dim + d.task_dim;
+  PiWs w;
+  w.nsplit = std::max(1, std::min(8, rows / 256));
+  size_t off = 0;
+  auto take = [&](size_t n) { const size_t o = off; off += (n + 63) / 64 * 64; return o; };
+  w.dl = take(2 * R * nb); w.gq = take(2 * R * M); w.gq2 = take(2 * R * M); w.dxq = take(2 * R * TA);
+  w.dlog = take(R * 2 * d.action_dim); w.gp = take(R * M); w.gp2 = take(R * M); w.dyn = take(R * M); w.dy = take(R * M);
+  w.hb = take(R * M); w.xb = take(R * LT); w.dxe = take(R * TA);
+  w.part = take(static_cast<size_t>(w.nsplit) * M * std::max({M, LT, static_cast<size_t>(2 * d.action_dim)}));
+  w.floats = off;
+  return w;
+}
+
+extern "C" int tdmpc2_pi_loss_tape_bytes(const tdmpc2_planner* p, int rows, size_t* out) {
+  if (!p || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (rows < 1) return fail(TDMPC2_ERR_INVALID, "rows must be >= 1");
+  *out = static_cast<size_t>(rows) * planner_tape(p).pitch * 4;
+  return 0;
+}
+
+extern "C" int tdmpc2_pi_loss_workspace_bytes(const tdmpc2_planner* p, int rows, size_t* out) {
+  if (!p || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (rows < 1) return fail(TDMPC2_ERR_INVALID, "rows must be >= 1");
+  *out = pi_ws(p, rows).floats * 4;
+  return 0;
+}
+
+extern "C" int tdmpc2_pi_loss_forward(tdmpc2_planner* p, const float* z, const int32_t* task, const float* eps,
+                                      const int32_t* qidx, const float* dropout_mask, int rows, float* tape, float* action_out,
+                                      float* q_out, float* log_prob_out, void* stream_) {
+  int rc = rows_ready(p, rows);
+  if (rc || (rc = need_task(p, task))) return rc;
+  if (!z || !eps || !qidx || !tape || !action_out || !q_out || !log_prob_out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  PlanParams prm = rows_params(p, ROP_PI_LOSS, rows, task);
+  prm.rows_in = z; prm.rows_eps = eps; prm.qidx = qidx; prm.rows_flag = 1;       // 'avg' of the online pair
+  prm.rows_tape = tape; prm.rows_act_out = action_out; prm.rows_out = q_out; prm.rows_out4 = log_prob_out;
+  prm.rows_drop = dropout_mask;
+  return launch(p, prm, stream_);
+}
+
+static int gemm(const GemmArgs& g, int batch, cudaStream_t st) {
+  const dim3 grid((g.n + kGBN - 1) / kGBN, (g.m + kGBM - 1) / kGBM, batch * g.nsplit);
+  gemm_f32<<<grid, 256, 0, st>>>(g);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int tdmpc2_pi_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* z,
+                                       const int32_t* task, const float* eps, const int32_t* qidx, const float* dropout_mask,
+                                       int T, int B, const float* scale, float entropy_coef, float rho,
+                                       const tdmpc2_pi_grads* gr, void* workspace, void* stream_) {
+  if (T < 1 || B < 1) {
+    int n = 0;
+    const int rc = check_device(&n);
+    return rc ? rc : fail(TDMPC2_ERR_INVALID, "T and B must be >= 1");
+  }
+  if (static_cast<long long>(T) * B > 0x7fffffff) return fail(TDMPC2_ERR_INVALID, "T * B too large");
+  const int R = T * B;
+  int rc = rows_ready(p, R);
+  if (rc || (rc = need_task(p, task))) return rc;
+  if (!w || !tape || !z || !eps || !qidx || !scale || !gr || !workspace) return fail(TDMPC2_ERR_INVALID, "null argument");
+  for (int i = 0; i < 3; ++i) {
+    if (!w->pi[i].weight || !w->qs[i].weight || !gr->weight[i] || !gr->bias[i]) return fail(TDMPC2_ERR_INVALID, "null weight or gradient");
+    if (i < 2 && (!w->pi[i].ln_weight || !w->qs[i].ln_weight || !w->qs[i].ln_bias || !w->pi[i].ln_bias || !gr->ln_weight[i] ||
+                  !gr->ln_bias[i]))
+      return fail(TDMPC2_ERR_INVALID, "null LayerNorm tensor or gradient");
+  }
+  const tdmpc2_dims& d = p->d;
+  if (d.task_dim > 0 && !gr->task_emb) return fail(TDMPC2_ERR_INVALID, "multi-task model needs the task-embedding gradient");
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  const PiTape tp = planner_tape(p);
+  const PiWs L = pi_ws(p, R);
+  float* ws = static_cast<float*>(workspace);
+  const long long M = d.mlp_dim, nb = d.num_bins, A = d.action_dim, Tq = d.task_dim, TA = Tq + A, Lz = d.latent_dim;
+  const long long LT = Lz + Tq, D = Lz + Tq + A;
+  float *dl = ws + L.dl, *gq = ws + L.gq, *gq2 = ws + L.gq2, *dxq = ws + L.dxq, *dlog = ws + L.dlog, *gp = ws + L.gp,
+        *gp2 = ws + L.gp2, *dyn = ws + L.dyn, *dy = ws + L.dy, *hb = ws + L.hb, *xb = ws + L.xb, *dxe = ws + L.dxe,
+        *part = ws + L.part;
+  const dim3 rows8((R + 7) / 8), rows8x2((R + 7) / 8, 2);
+  const int* task_rows = d.task_dim > 0 ? task : nullptr;
+  auto colsum = [&](const float* src, long long n, long long ld, float* dst) -> int {
+    pl_colsum<<<static_cast<int>((n + 127) / 128), 128, 0, st>>>(src, R, static_cast<int>(n), ld, dst);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+  };
+  // dst += src^T x [rows, n] over the rows, in nsplit row blocks summed in order
+  auto dweight = [&](const float* src, long long m, const float* x, long long n, long long ldx, float* dst) -> int {
+    GemmArgs g{src, 1, m, 0, x, ldx, 1, 0, nullptr, part, n, 0, m * n, static_cast<int>(m), static_cast<int>(n), R, L.nsplit};
+    int rc2 = gemm(g, 1, st);
+    if (rc2) return rc2;
+    pl_reduce<<<static_cast<int>((m * n + 255) / 256), 256, 0, st>>>(part, L.nsplit, m * n, m * n, dst);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+  };
+  LnBackArgs lb{};
+  lb.tape = tape; lb.pitch = tp.pitch; lb.rows = R; lb.N = static_cast<int>(M); lb.ld = M;
+
+  // ---- the two Q heads: two-hot inverse -> layer 2 -> LN/Mish 1 -> layer 1 -> LN/Mish/dropout 0 -> [emb | a] columns
+  pl_q_head_back<<<rows8x2, 256, 0, st>>>(tape, tp.pitch, tp.q[0] + 2 * static_cast<int>(M), tp.q[1] + 2 * static_cast<int>(M), R,
+                                          static_cast<int>(nb), p->base.bins, scale, B, T, rho, dl);
+  CUDA_TRY(cudaGetLastError());
+  if ((rc = gemm(GemmArgs{dl, nb, 1, R * nb, w->qs[2].weight, M, 1, nb * M, qidx, gq, M, R * M, 0,
+                          R, static_cast<int>(M), static_cast<int>(nb), 1}, 2, st))) return rc;
+  lb.off = tp.q[0] + static_cast<int>(M); lb.off_z = tp.q[1] - tp.q[0]; lb.g = gq; lb.out = gq; lb.g_z = R * M;
+  lb.gamma = w->qs[1].ln_weight; lb.beta = w->qs[1].ln_bias; lb.hsel = qidx;
+  pl_ln_back<<<rows8x2, 256, 0, st>>>(lb);
+  CUDA_TRY(cudaGetLastError());
+  if ((rc = gemm(GemmArgs{gq, M, 1, R * M, w->qs[1].weight, M, 1, M * M, qidx, gq2, M, R * M, 0,
+                          R, static_cast<int>(M), static_cast<int>(M), 1}, 2, st))) return rc;
+  lb.off = tp.q[0]; lb.g = gq2; lb.out = gq2; lb.gamma = w->qs[0].ln_weight; lb.beta = w->qs[0].ln_bias; lb.drop = dropout_mask;
+  pl_ln_back<<<rows8x2, 256, 0, st>>>(lb);
+  CUDA_TRY(cudaGetLastError());
+  if ((rc = gemm(GemmArgs{gq2, M, 1, R * M, w->qs[0].weight + Lz, D, 1, M * D, qidx, dxq, TA, R * TA, 0,
+                          R, static_cast<int>(TA), static_cast<int>(M), 1}, 2, st))) return rc;
+
+  // ---- the tanh-Gaussian head, then pi layers 2 -> 0 with their parameter gradients
+  PiHeadArgs ph{};
+  ph.tape = tape; ph.pitch = tp.pitch; ph.off_h = tp.pih; ph.Apad = pad_to(d.action_dim, 32);
+  ph.eps = eps; ph.task = task_rows; ph.masks = p->base.masks;
+  ph.da_q = dxq; ph.da_ld = TA; ph.da_z = R * TA; ph.a_off = static_cast<int>(Tq);
+  ph.log_std_min = d.log_std_min; ph.log_std_dif = d.log_std_dif; ph.entropy_coef = entropy_coef; ph.rho = rho; ph.scale = scale;
+  ph.rows = R; ph.A = d.action_dim; ph.Bsz = B; ph.Tsz = T; ph.dlog = dlog;
+  pl_pi_head_back<<<rows8, 256, 0, st>>>(ph);
+  CUDA_TRY(cudaGetLastError());
+  if ((rc = gemm(GemmArgs{dlog, 2 * A, 1, 0, w->pi[2].weight, M, 1, 0, nullptr, gp, M, 0, 0,
+                          R, static_cast<int>(M), static_cast<int>(2 * A), 1}, 1, st))) return rc;
+  lb.off = tp.pi1; lb.off_z = 0; lb.g = gp; lb.out = gp; lb.g_z = 0; lb.gamma = w->pi[1].ln_weight; lb.beta = w->pi[1].ln_bias;
+  lb.hsel = nullptr; lb.drop = nullptr; lb.dyn = dyn; lb.dy = dy; lb.h = hb;
+  pl_ln_back<<<rows8, 256, 0, st>>>(lb);                       // gp <- dL/dpre of pi.1; hb <- pi.1's activation
+  CUDA_TRY(cudaGetLastError());
+  if ((rc = colsum(dyn, M, M, gr->ln_weight[1])) || (rc = colsum(dy, M, M, gr->ln_bias[1]))) return rc;
+  if ((rc = dweight(dlog, 2 * A, hb, M, M, gr->weight[2])) || (rc = colsum(dlog, 2 * A, 2 * A, gr->bias[2]))) return rc;
+  if ((rc = gemm(GemmArgs{gp, M, 1, 0, w->pi[1].weight, M, 1, 0, nullptr, gp2, M, 0, 0,
+                          R, static_cast<int>(M), static_cast<int>(M), 1}, 1, st))) return rc;
+  lb.off = tp.pi0; lb.g = gp2; lb.out = gp2; lb.gamma = w->pi[0].ln_weight; lb.beta = w->pi[0].ln_bias;
+  pl_ln_back<<<rows8, 256, 0, st>>>(lb);                       // gp2 <- dL/dpre of pi.0; hb <- pi.0's activation
+  CUDA_TRY(cudaGetLastError());
+  if ((rc = colsum(dyn, M, M, gr->ln_weight[0])) || (rc = colsum(dy, M, M, gr->ln_bias[0]))) return rc;
+  if ((rc = dweight(gp, M, hb, M, M, gr->weight[1])) || (rc = colsum(gp, M, M, gr->bias[1]))) return rc;
+  const float* x = z;
+  if (Tq > 0) {
+    pl_gather_x<<<static_cast<int>((R * LT + 255) / 256), 256, 0, st>>>(z, p->base.emb, task, R, static_cast<int>(Lz),
+                                                                       static_cast<int>(Tq), xb);
+    CUDA_TRY(cudaGetLastError());
+    x = xb;
+  }
+  if ((rc = dweight(gp2, M, x, LT, LT, gr->weight[0])) || (rc = colsum(gp2, M, M, gr->bias[0]))) return rc;
+  if (Tq > 0) {
+    // the embedding enters pi.0's and both Q heads' layer-0 inputs: dL/demb of each row, scattered by task in row order
+    if ((rc = gemm(GemmArgs{gp2, M, 1, 0, w->pi[0].weight + Lz, LT, 1, 0, nullptr, dxe, TA, 0, 0,
+                            R, static_cast<int>(Tq), static_cast<int>(M), 1}, 1, st))) return rc;
+    pl_emb_grad<<<static_cast<int>((d.num_tasks * Tq + 127) / 128), 128, 0, st>>>(dxe, dxq, dxq + R * TA, TA, task, R, d.num_tasks,
+                                                                                static_cast<int>(Tq), gr->task_emb);
+    CUDA_TRY(cudaGetLastError());
+  }
+  return 0;
 }

@@ -64,7 +64,9 @@ constexpr int kSmemBytes = kStages * kStageBytes + kSmemCtrl + kSmemRowBuf + kSm
 
 enum Mode { MODE_ENCODE = 0, MODE_PRIOR = 1, MODE_ITER = 2, MODE_VALUE = 3, MODE_LAYER = 4, MODE_ROWS = 5 };
 // MODE_ROWS: which world-model method a launch runs (PlanParams::rop)
-enum RowOp { ROP_ENCODE = 0, ROP_NEXT = 1, ROP_REWARD = 2, ROP_TERM = 3, ROP_PI = 4, ROP_Q_ALL = 5, ROP_Q_PAIR = 6, ROP_TD = 7 };
+// ROP_PI_LOSS: agent.update_pi's forward (pi, then the online Q pair's average on pi's action) writing a tape
+enum RowOp { ROP_ENCODE = 0, ROP_NEXT = 1, ROP_REWARD = 2, ROP_TERM = 3, ROP_PI = 4, ROP_Q_ALL = 5, ROP_Q_PAIR = 6, ROP_TD = 7,
+             ROP_PI_LOSS = 8 };
 enum Engine { ENGINE_TC = 0, ENGINE_SIMT = 1 };
 // X = [z | emb | a] input planes; H = hidden planes.  ONE hidden buffer is enough: a layer's epilogue only runs after
 // every MMA of its GEMM has consumed the A operand, so layer 1 overwrites its own input in place.
@@ -136,8 +138,28 @@ struct PlanParams {
   float* rows_out;                 // z' / logits [rows, .]; Q all [num_q, rows, B]; pi action [rows, A]; Q pair / TD [rows]
   float* rows_out2;                // ROP_PI: tanh(mean) [rows, A]
   float* rows_out3;                // ROP_PI: log_std [rows, A]
-  float* rows_out4;                // ROP_PI: [rows, 2] = (gaussian log-prob, sum of the squash terms)
+  float* rows_out4;                // ROP_PI / ROP_PI_LOSS: [rows, 2] = (gaussian log-prob, sum of the squash terms)
+  // ROP_PI_LOSS (rows_out = q [rows], rows_flag = 1)
+  float* rows_tape;                // [rows, tape.pitch]: see PiTape
+  float* rows_act_out;             // action [rows, A]
+  const float* rows_drop;          // Q layer 0 dropout scale (mask / (1 - p)) [num_q, rows, M], or nullptr (eval mode)
 };
+
+// The tape of ROP_PI_LOSS, per row (fp32 offsets): the pre-LayerNorm rows of pi.0 and pi.1 [M], the pi head's logits
+// [Apad + A] (log_std logits at column Apad, as in the kernel's head row), then for each selected Q head u the
+// pre-LayerNorm rows of its layers 0 (after dropout) and 1 [M] and its logits [B]; the action [A] and q [1] last.
+// The backward (grad_kernels.cuh) recomputes every LayerNorm / Mish value from it.
+struct PiTape {
+  int pi0, pi1, pih, q[2], act, qv, pitch;
+};
+__host__ __device__ inline PiTape pi_tape(int M, int A, int Apad, int B) {
+  PiTape t;
+  t.pi0 = 0; t.pi1 = M; t.pih = 2 * M;
+  t.q[0] = t.pih + Apad + A; t.q[1] = t.q[0] + 2 * M + B;
+  t.act = t.q[1] + 2 * M + B; t.qv = t.act + A;
+  t.pitch = (t.qv + 1 + 3) & ~3;
+  return t;
+}
 
 // The layer table lives in global memory; role loops are full of asm volatile(... "memory") (TMA issue, mbarrier waits,
 // fences), each of which would force the compiler to re-read any field it needs afterwards -- a dependent global load
@@ -170,6 +192,8 @@ struct EpiArgs {
   int eps_rows;
   float* act_out;           // PI: optional pi_actions output
   int t_out;
+  float* tape;              // MODE_ROWS ROP_PI_LOSS: this layer's tape segment of output row 0 (row pitch P.tape pitch)
+  const float* drop;        // MODE_ROWS ROP_PI_LOSS, Q layer 0: dropout scale of output row 0 (row pitch N), or nullptr
 };
 
 // ------------------------------------------------------------------------------------ small math
@@ -562,6 +586,9 @@ __device__ __forceinline__ void mish_batch(float (&y)[kLnBatch]) {
 //   - other widths: raw is read once per statistic and once in the output pass.  (Statistics loads in guarded batches
 //     of kLnBatch were measured slower on c3's 1792-wide rows than these loops, which ptxas unrolls with unguarded loads.)
 // Every column's value is the same expression in the same order in both paths: same bits.
+// ROWS (ROP_PI_LOSS): the pre-LayerNorm value is multiplied by the dropout scale ea.drop (Q layer 0, train mode) and
+// stored to the tape ea.tape; compiled out of the planning instantiations.
+template <bool ROWS>
 __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const LayerRec& ly, const EpiArgs& ea) {
   const float* rawbase = raw_ptr(P, c.slot);
   const int N = ly.N;
@@ -608,11 +635,19 @@ __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const L
       float x[kLnRegCols];
 #pragma unroll
       for (int j = 0; j < kLnRegCols; ++j) x[j] = row[c.lane + 32 * j];
+      const bool live = ROWS && ea.rowmap[r] >= 0;
+      const float* drow = live && ea.drop ? ea.drop + static_cast<size_t>(ea.rowmap[r]) * N : nullptr;
       float s = 0.f;
 #pragma unroll
       for (int j = 0; j < kLnRegCols; ++j) {
         x[j] = fmaf(x[j], inv_scale, __ldg(bias + c.lane + 32 * j));
+        if (ROWS && drow) x[j] *= drow[c.lane + 32 * j];
         s += x[j];
+      }
+      if (ROWS && live && ea.tape) {
+        float* trow = ea.tape + static_cast<size_t>(ea.rowmap[r]) * pi_tape(P.M, P.A, P.Apad, P.B).pitch;
+#pragma unroll
+        for (int j = 0; j < kLnRegCols; ++j) trow[c.lane + 32 * j] = x[j];
       }
       const float mean = warp_sum(s) * invN;
       float sq = 0.f;
@@ -634,6 +669,43 @@ __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const L
         act_store(y, j0, r);
       }
       __syncwarp();   // every lane has read buffer i before the next iteration refills it
+    }
+  } else if (ROWS && (ea.drop || ea.tape)) {
+    // other widths with a dropout scale or a tape (ROP_PI_LOSS; kept apart so that the planning path's code is untouched):
+    // the statistics pass tapes the pre-LayerNorm row, the later passes recompute it.  Padding rows have neither.
+    for (int r = c.warp; r < kTileM; r += kWarps) {
+      const float* rr = rawbase + static_cast<size_t>(r) * P.NpadMax;
+      const int orow = ea.rowmap[r];
+      const float* drow = ea.drop && orow >= 0 ? ea.drop + static_cast<size_t>(orow) * N : nullptr;
+      float* trow = ea.tape && orow >= 0 ? ea.tape + static_cast<size_t>(orow) * pi_tape(P.M, P.A, P.Apad, P.B).pitch : nullptr;
+      float s = 0.f;
+      for (int col = c.lane; col < N; col += 32) {
+        float v = fmaf(__ldcg(rr + col), inv_scale, __ldg(bias + col));
+        if (drow) v *= drow[col];
+        if (trow) trow[col] = v;
+        s += v;
+      }
+      const float mean = warp_sum(s) * invN;
+      auto pre = [&](int col) {
+        const float v = fmaf(__ldcg(rr + col), inv_scale, __ldg(bias + col));
+        return drow ? v * drow[col] : v;
+      };
+      float sq = 0.f;
+      for (int col = c.lane; col < N; col += 32) {
+        const float d = pre(col) - mean;
+        sq = fmaf(d, d, sq);
+      }
+      const float var = warp_sum(sq) * invN;
+      const float rstd = 1.f / sqrtf(var + 1e-5f);
+      for (int j0 = 0; j0 < ncolj; j0 += kLnBatch) {
+        float y[kLnBatch];
+#pragma unroll
+        for (int u = 0; u < kLnBatch; ++u) {
+          const int col = c.lane + 32 * (j0 + u);
+          y[u] = col < N ? (pre(col) - mean) * rstd * __ldg(lg + col) + __ldg(lb + col) : 0.f;
+        }
+        act_store(y, j0, r);
+      }
     }
   } else {
     for (int r = c.warp; r < kTileM; r += kWarps) {
@@ -710,6 +782,10 @@ __device__ __forceinline__ void rows_commit(const PlanParams& P, Ctx& c, const E
     P.rows_out[row] = __fadd_rn(P.rows_reward[row], __fmul_rn(__fmul_rn(disc, __fsub_rn(1.f, P.rows_term[row])), q));
   } else {
     P.rows_out[row] = q;
+    if (P.rows_tape) {
+      const PiTape tp = pi_tape(P.M, P.A, P.Apad, P.B);
+      P.rows_tape[static_cast<size_t>(row) * tp.pitch + tp.qv] = q;
+    }
   }
 }
 
@@ -736,6 +812,10 @@ __device__ __forceinline__ void rows_pi(const PlanParams& P, Ctx& c, const float
       P.rows_out[ro] = act;
       P.rows_out2[ro] = tanhf(mu);
       P.rows_out3[ro] = ls;
+    }
+    if (P.rows_tape && row >= 0) {
+      P.rows_act_out[static_cast<size_t>(row) * P.A + a] = act;
+      P.rows_tape[static_cast<size_t>(row) * pi_tape(P.M, P.A, P.Apad, P.B).pitch + pi_tape(P.M, P.A, P.Apad, P.B).act + a] = act;
     }
   }
   lp = warp_sum(lp);
@@ -789,6 +869,12 @@ __device__ __forceinline__ void rows_head(const PlanParams& P, Ctx& c, const Lay
         const int col = c.lane + 32 * j;
         y[j] = col < N ? fmaf(row[col], ly.inv_scale, __ldg(ly.bias + col)) : 0.f;
       }
+      if (ROWS && ea.tape && c.rowenv[r] >= 0) {      // ROP_PI_LOSS: the head's logits go to the tape
+        float* t = ea.tape + static_cast<size_t>(c.rowenv[r]) * pi_tape(P.M, P.A, P.Apad, P.B).pitch;
+#pragma unroll
+        for (int j = 0; j < kHeadRegCols; ++j)
+          if (c.lane + 32 * j < N) t[c.lane + 32 * j] = y[j];
+      }
       if (EPISODIC && ea.kind == EPI_TERM) {
         if (c.lane == 0) term_commit(c, r, y[0]);
       } else if (ea.kind == EPI_TWOHOT) {
@@ -832,7 +918,7 @@ __device__ __forceinline__ void run_layer(const PlanParams& P, Ctx& c, const Lay
   if (ENGINE == ENGINE_TC) gemm_tc(P, c, ly, srcbuf, kc0);
   else gemm_simt(P, c, ly, srcbuf, kc0);
   if (threadIdx.x == 0) TDMPC2_TRACE(P, c, 3);
-  if (is_ln) rows_ln_act(P, c, ly, ea);
+  if (is_ln) rows_ln_act<ROWS>(P, c, ly, ea);
   else rows_head<EPISODIC, ROWS>(P, c, ly, ea);
   c.pf1 += prof_clock() - tl;
   const long long tp = prof_clock();
@@ -1107,7 +1193,7 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
     //   ITER   : per t: [a_t -> X] rew.0-2, dyn.0-2 [, term.0-2 if EPISODIC] ; then pi.0-2, q_a.0-2, q_b.0-2
     int nsteps;
     if (ROWS) nsteps = P.rop == ROP_ENCODE ? P.num_enc : P.rop == ROP_Q_ALL ? 3 * P.num_q : P.rop == ROP_Q_PAIR ? 6
-                     : P.rop == ROP_TD ? 9 : 3;
+                     : (P.rop == ROP_TD || P.rop == ROP_PI_LOSS) ? 9 : 3;
     else if (P.mode == MODE_LAYER) nsteps = 1;
     else if (P.mode == MODE_ENCODE) nsteps = P.num_enc;
     else if (P.mode == MODE_PRIOR) nsteps = 6 * (P.H - 1) + 3;
@@ -1119,6 +1205,7 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
       EpiArgs ea;
       ea.kind = EPI_LN_MISH; ea.dstbuf = -1; ea.dst_col0 = 0; ea.out_f32 = nullptr; ea.out_pitch = 0; ea.rowmap = nullptr;
       ea.head = 0; ea.disc = 0.f; ea.tile = tile; ea.eps_base = nullptr; ea.eps_rows = 0; ea.act_out = nullptr; ea.t_out = 0;
+      ea.tape = nullptr; ea.drop = nullptr;
       int li, src;
       int kc0 = 0;                       // first K-chunk of the GEMM and bias vector: the shared-latent fold (PlanParams::zbias)
       const float* bias_ov = nullptr;
@@ -1143,14 +1230,22 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
         } else if (P.rop == ROP_TERM) {
           li = P.li_term + l;
           if (last) { ea.kind = EPI_RAW; ea.out_f32 = P.rows_out; ea.out_pitch = 1; ea.head = P.rows_flag; }
-        } else if (P.rop == ROP_PI || (P.rop == ROP_TD && sidx < 3)) {
+        } else if (P.rop == ROP_PI || ((P.rop == ROP_TD || P.rop == ROP_PI_LOSS) && sidx < 3)) {
           li = P.li_pi + l;
           if (last) ea.kind = EPI_PI;
+          if (P.rop == ROP_PI_LOSS) {
+            const PiTape tp = pi_tape(P.M, P.A, P.Apad, P.B);
+            ea.tape = P.rows_tape + (l == 0 ? tp.pi0 : l == 1 ? tp.pi1 : tp.pih);
+          }
         } else {
-          const int u = P.rop == ROP_TD ? sidx / 3 - 1 : sidx / 3;     // head slot
+          const int u = (P.rop == ROP_TD || P.rop == ROP_PI_LOSS) ? sidx / 3 - 1 : sidx / 3;     // head slot
           const int h = P.rop == ROP_Q_ALL ? u : P.qidx[u];
           lyt = P.rows_q;
           li = 3 * h + l;
+          if (P.rop == ROP_PI_LOSS) {
+            ea.tape = P.rows_tape + pi_tape(P.M, P.A, P.Apad, P.B).q[u] + l * P.M;
+            if (l == 0 && P.rows_drop) ea.drop = P.rows_drop + static_cast<size_t>(h) * P.rows * P.M;
+          }
           if (last && P.rop == ROP_Q_ALL) {
             ea.kind = EPI_RAW; ea.out_f32 = P.rows_out + static_cast<size_t>(h) * P.rows * P.B; ea.out_pitch = P.B;
           } else if (last) {

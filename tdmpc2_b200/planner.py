@@ -245,6 +245,7 @@ class Planner:
         self._graph_launches = 0
         self.target_blob = None      # target Q ensemble (tdmpc2_planner_bind_target_q), allocated by the first target op
         self.target_version = None
+        self._tables = None          # discount powers and two-hot bins (pack)
 
     def __del__(self):
         try:
@@ -327,13 +328,16 @@ class Planner:
             emb, masks = f("_task_emb.weight"), f("_action_masks")
             keep.extend([emb, masks])
             W.task_emb, W.action_masks = _ptr(emb), _ptr(masks)
-        disc = discount_table(cfg, self.device)
-        bins = torch.linspace(cfg.vmin, cfg.vmax, cfg.num_bins, device=self.device, dtype=torch.float32)  # math.py:80
-        keep.extend([disc, bins])
+        if self._tables is None:      # built once: torch.tensor() of host values is a synchronising copy
+            self._tables = (discount_table(cfg, self.device),
+                            torch.linspace(cfg.vmin, cfg.vmax, cfg.num_bins, device=self.device, dtype=torch.float32))  # math.py:80
+        disc, bins = self._tables
         W.discount_pow, W.bins = _ptr(disc), _ptr(bins)
         with torch.cuda.device(self.device):
-            _cabi.check(self.lib.tdmpc2_pack_weights(self.h, C.byref(W), self._stream()))
-            torch.cuda.current_stream(self.device).synchronize()   # `keep` tensors may be freed afterwards
+            stream = torch.cuda.current_stream(self.device)
+            _cabi.check(self.lib.tdmpc2_pack_weights(self.h, C.byref(W), stream.cuda_stream))
+            for t in keep:            # `keep` tensors may be freed now: their memory is not reused before the pack ran
+                t.record_stream(stream)
 
     # ------------------------------------------------------------------ hot path
     def prologue(self, obs, task, t0, prev_mean, noise_prior) -> None:
@@ -630,6 +634,43 @@ class Planner:
             _cabi.check(self.lib.tdmpc2_td_target(self.h, _ptr(next_z), _ptr(reward), _ptr(terminated), _ptr(task),
                                                   _ptr(eps), _ptr(qidx), R, _ptr(out), self._stream()))
         return out
+
+    def pi_loss_forward(self, z, task, eps, qidx, drop):
+        """update_pi's forward on z [rows, L]: -> tape, action [rows, A], q [rows, 1], [rows, 2] = (gaussian log-prob,
+        sum of the squash terms).  drop: Q layer 0's dropout scale [num_q, rows, M] or None."""
+        R = z.shape[0]
+        nb = C.c_size_t()
+        _cabi.check(self.lib.tdmpc2_pi_loss_tape_bytes(self.h, R, C.byref(nb)))
+        tape = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        act, q, lp = self._rows_out(R, self.cfg.action_dim), self._rows_out(R, 1), self._rows_out(R, 2)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_pi_loss_forward(self.h, _ptr(z), _ptr(task), _ptr(eps), _ptr(qidx), _ptr(drop), R,
+                                                        _ptr(tape), _ptr(act), _ptr(q), _ptr(lp), self._stream()))
+        return tape, act, q, lp
+
+    def pi_loss_backward(self, tensor, tape, z, task, eps, qidx, drop, T, B, scale, entropy_coef, rho, grads, emb_grad):
+        """Adds dL/dparameter of update_pi's loss to `grads` (the 10 `_pi.*` .grad tensors by state-dict key) and, for
+        multi-task models, to `emb_grad`.  `tensor(key)` returns the model's fp32 tensor of a state-dict key."""
+        W = _cabi.Weights()
+        for i in range(3):
+            for pfx, dst in (("_pi", W.pi), ("_Qs.params", W.qs)):
+                k = f"{pfx}.{i}"
+                ln = i < 2
+                dst[i] = _cabi.Linear(_ptr(tensor(k + ".weight")), _ptr(tensor(k + ".bias")),
+                                      _ptr(tensor(k + ".ln.weight")) if ln else None, _ptr(tensor(k + ".ln.bias")) if ln else None)
+        G = _cabi.PiGrads()
+        for i in range(3):
+            G.weight[i], G.bias[i] = _ptr(grads[f"_pi.{i}.weight"]), _ptr(grads[f"_pi.{i}.bias"])
+            if i < 2:
+                G.ln_weight[i], G.ln_bias[i] = _ptr(grads[f"_pi.{i}.ln.weight"]), _ptr(grads[f"_pi.{i}.ln.bias"])
+        G.task_emb = _ptr(emb_grad)
+        nb = C.c_size_t()
+        _cabi.check(self.lib.tdmpc2_pi_loss_workspace_bytes(self.h, max(1, T * B), C.byref(nb)))
+        ws = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_pi_loss_backward(self.h, C.byref(W), _ptr(tape), _ptr(z), _ptr(task), _ptr(eps),
+                                                         _ptr(qidx), _ptr(drop), T, B, _ptr(scale), float(entropy_coef),
+                                                         float(rho), C.byref(G), _ptr(ws), self._stream()))
 
     def estimate_value(self, z, actions, task, noise_pi, qidx):
         """z [E,N,L], actions [E,H,N,A], noise_pi [E,N,A], qidx [E,2] int32 -> [E,N]."""

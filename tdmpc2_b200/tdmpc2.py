@@ -5,9 +5,9 @@ Drop-in for the inference half of the reference class `TDMPC2`
 `._prev_mean`, `.discount`, `.load()`, `.save()`, `.act()`, `.plan`, `._plan()`,
 `._estimate_value()`, `._td_target()` keep their names, argument meaning and return shapes, so
 `evaluate.py:57-80` of the reference runs unchanged on it (INTEGRATION.md), and so does the
-no-grad block of `_update` (`model.encode` + `_td_target`, tdmpc2.py:259-264).
-Gradients (`update`, optimisers, RunningScale) are out of scope (SURVEY.md 2.1 #1b);
-call `sync_weights()` after changing the model's parameters (incl. the target Q update).
+no-grad block of `_update` (`model.encode` + `_td_target`, tdmpc2.py:259-264), and the policy update
+`update_pi` (tdmpc2.py:208-239) with its `scale` (RunningScale) and `pi_optim`.  The world model's losses and
+optimiser are out of scope; call `sync_weights()` after changing the model's parameters (incl. the target Q update).
 
 New: an environments axis.  `obs [E, obs_dim]`, `t0 [E]`, `task [E]` plan E
 independent environments in one call; E == 1 (1-D obs) is the reference API.
@@ -22,6 +22,7 @@ import torch
 
 from .config import Config, get_discount
 from .planner import Noise, Planner, draw_noise
+from .scale import RunningScale
 from .world_model import WorldModel, convert_legacy_checkpoint
 
 
@@ -49,6 +50,11 @@ class TDMPC2(torch.nn.Module):
         self._use_graph = bool(cfg.get("cuda_graph", True))   # replay the launch chain as one CUDA graph (cfg.compile's role)
         # one environment: interleave the reference-order noise draws with the launches instead (TDMPC2_B200_E1_GRAPH=1: A/B knob)
         self._e1_interleaved = bool(cfg.get("e1_interleaved", True)) and os.environ.get("TDMPC2_B200_E1_GRAPH", "0") in ("", "0")
+        # the policy update (tdmpc2.py:26-30,41): Adam over the `_pi.*` parameters, and the running Q scale
+        self.scale = RunningScale(cfg, self.device)
+        self._pi_keys = [k for k in self.model.keys() if k.startswith("_pi.")]
+        self.pi_optim = torch.optim.Adam([self.model.tensor(k) for k in self._pi_keys], lr=cfg.lr, eps=1e-5,
+                                         capturable=self.device.type == "cuda")
 
     # ------------------------------------------------------------------ planner plumbing
     @property
@@ -186,6 +192,76 @@ class TDMPC2(torch.nn.Module):
         self._prev_mean.copy_(new_mean.reshape(self._prev_mean.shape))           # tdmpc2.py:205
         out = action[0] if E == 1 else action
         return (out, trace) if return_trace else out
+
+    def update_pi(self, zs, task, *, eps=None, qidx=None, dropout_mask=None):
+        """tdmpc2.py:208-239 on the kernels: one forward launch (pi, then the online Q pair's average, writing a tape) and
+        the backward chain of grad_kernels.cuh, which ADDS the gradients to `.grad` of the `_pi.*` parameters (and of
+        `_task_emb.weight` in multi-task models) as autograd would; then torch's clip_grad_norm_ and pi_optim.step().
+        zs [T, B, L] (detached), task [B] | int | None.  Draws from self.generator in the reference's order: eps
+        ([T, B, A], pi's randn_like), then in train mode (`self.model.training`, as inside _update) the dropout masks of
+        Q layer 0 -- one [T B, mlp_dim] draw per head for all num_q heads (the reference's vmap dropout stream is not
+        replayed bit for bit) -- then qidx (randperm(num_q)[:2]).  `eps`, `qidx`, `dropout_mask` ([num_q, T, B,
+        mlp_dim] of mask / (1 - p) values) pass them explicitly.  Returns the reference's info dict."""
+        cfg, dev = self.cfg, self.device
+        if dev.type != "cuda":
+            raise RuntimeError("update_pi runs on the sm_90a kernels: the agent needs a CUDA device (there is no CPU fallback)")
+        pl = self.planner
+        if zs.ndim != 3 or zs.shape[-1] != cfg.latent_dim or zs.shape[0] < 1 or zs.shape[1] < 1:
+            raise ValueError(f"zs must be [T, B, {cfg.latent_dim}]; got {tuple(zs.shape)}")
+        if cfg.multitask and task is None:
+            raise ValueError("multi-task model needs `task`")
+        T, B = int(zs.shape[0]), int(zs.shape[1])
+        R, A, M, g = T * B, cfg.action_dim, cfg.mlp_dim, self.generator
+        z = zs.detach().to(dev, torch.float32).reshape(R, -1).contiguous()
+        eps = (torch.randn(T, B, A, device=dev, generator=g) if eps is None else torch.as_tensor(eps, device=dev))
+        if tuple(eps.shape) != (T, B, A):
+            raise ValueError(f"eps must be [{T}, {B}, {A}]; got {tuple(eps.shape)}")
+        eps = eps.to(torch.float32).reshape(R, A).contiguous()
+        drop = None
+        if dropout_mask is not None:
+            drop = torch.as_tensor(dropout_mask, device=dev)
+            if tuple(drop.shape) != (cfg.num_q, T, B, M):
+                raise ValueError(f"dropout_mask must be [{cfg.num_q}, {T}, {B}, {M}]; got {tuple(drop.shape)}")
+            drop = drop.to(torch.float32).contiguous()
+        elif self.model.training and cfg.dropout > 0:       # nn.Dropout(cfg.dropout) of Q layer 0 (layers.py:104-108)
+            keep = 1.0 - cfg.dropout
+            drop = torch.empty(cfg.num_q, R, M, device=dev).bernoulli_(keep, generator=g).div_(keep)
+        if qidx is None:
+            qidx = torch.randperm(cfg.num_q, device=dev, generator=g)[:2]
+        qidx = torch.as_tensor(qidx, device=dev).reshape(-1)
+        if qidx.numel() != 2:
+            raise ValueError(f"qidx must hold 2 head indices; got {qidx.numel()}")
+        qidx = qidx.to(torch.int32).contiguous()
+        taskv = self.model._task_rows(pl, task, (T, B))
+
+        tape, _, q, lp = pl.pi_loss_forward(z, taskv, eps, qidx, drop)
+        log_prob, log_pi = lp[:, :1], lp[:, :1] - lp[:, 1:]                 # world_model.py:166-176
+        size = float(A) if taskv is None else self.model.tensor("_action_masks").sum(-1)[taskv.long()].unsqueeze(-1)
+        entropy = (-log_pi).view(T, B, 1)
+        scaled_entropy = (-log_pi * (log_prob * size / (log_pi + 1e-8))).view(T, B, 1)
+        qs = q.view(T, B, 1)
+        self.scale.update(qs[0])
+        qs = self.scale(qs)
+        rho = torch.pow(cfg.rho, torch.arange(T, device=dev))
+        pi_loss = (-(cfg.entropy_coef * scaled_entropy + qs).mean(dim=(1, 2)) * rho).mean()
+
+        params = [self.model.tensor(k) for k in self._pi_keys]
+        for p in params:
+            if p.grad is None:
+                p.grad = torch.zeros_like(p)
+        emb = None
+        if cfg.multitask:
+            emb = self.model.tensor("_task_emb.weight")
+            if emb.grad is None:
+                emb.grad = torch.zeros_like(emb)
+        pl.pi_loss_backward(self.model.tensor, tape, z, taskv, eps, qidx, drop, T, B, self.scale.value, cfg.entropy_coef,
+                            cfg.rho, {k: p.grad for k, p in zip(self._pi_keys, params)}, None if emb is None else emb.grad)
+        pi_grad_norm = torch.nn.utils.clip_grad_norm_(params, cfg.grad_clip_norm)
+        self.pi_optim.step()
+        self.pi_optim.zero_grad(set_to_none=True)
+        self.sync_weights()
+        return {"pi_loss": pi_loss.detach(), "pi_grad_norm": pi_grad_norm, "pi_entropy": entropy,
+                "pi_scaled_entropy": scaled_entropy, "pi_scale": self.scale.value}
 
     @torch.no_grad()
     def _td_target(self, next_z, reward, terminated, task, *, eps=None, qidx=None):
