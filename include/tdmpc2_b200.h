@@ -41,7 +41,8 @@ extern "C" {
                                        6: tdmpc2_plan_iter_rng (declared non-parity in-kernel noise), tdmpc2_debug_rng;
                                        7: world-model methods on a flat batch (tdmpc2_wm_*, tdmpc2_td_target), target Q blob;
                                           later, additive: tdmpc2_pixel_encode_rows (old callers and bindings unaffected);
-                                          later, additive: agent.update_pi (tdmpc2_pi_loss_*, tdmpc2_pi_grads) */
+                                          later, additive: agent.update_pi (tdmpc2_pi_loss_*, tdmpc2_pi_grads),
+                                          agent._update (tdmpc2_wm_loss_*, tdmpc2_wm_grads) */
 #define TDMPC2_MAX_ENC_LAYERS 8
 
 typedef enum tdmpc2_status {
@@ -317,6 +318,51 @@ int tdmpc2_pi_loss_forward(tdmpc2_planner* p, const float* z, const int32_t* tas
 int tdmpc2_pi_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* z, const int32_t* task,
                             const float* eps, const int32_t* qidx, const float* dropout_mask, int T, int B, const float* scale,
                             float entropy_coef, float rho, const tdmpc2_pi_grads* grads, void* workspace, void* stream);
+
+/* ---- agent._update: the world model's loss (tdmpc2.py:259-313), state observations ------------------------------
+ * forward: the latent rollout of a [H + 1, B] batch (row r of a [H, B] batch is t B + b), as row launches that also
+ * write the caller-owned tape [tape_bytes] (the pre-LayerNorm row of every LayerNorm layer, DESIGN section 4.4):
+ *   encode(obs0 [B, obs_dim]) -> zs[0]; next(zs[t], action[t]) -> zs[t + 1] for t < H, written in place into
+ *   zs [H + 1, B, L]; Q 'all' on (zs[:H], action) with dropout_mask (NULL: eval mode; else [num_q, H B, mlp_dim] of
+ *   mask / (1 - p) on each head's layer 0) -> q_logits [num_q, H B, num_bins]; reward(zs[:H], action) -> reward_logits
+ *   [H B, num_bins]; episodic models: termination(zs[1:]) -> term_logits [H B] (else NULL).
+ *   task: NULL (single-task) or [H B] per-row task indices.  Pixel models (no state encoder): TDMPC2_ERR_UNSUPPORTED.
+ * backward: from the tape, the forward's inputs and outputs, next_z [H, B, L] (encode(obs[1:])), reward / td_target /
+ *   terminated [H B] and the loss coefficients, ADDS dL/dparameter of
+ *     consistency * sum_t rho^t mse(zs[t+1], next_z[t]) / H + reward * sum_t rho^t soft_ce(reward logits, r_t).mean() / H
+ *     + value * sum_{t,q} rho^t soft_ce(Q_q logits, td_t).mean() / (H num_q) + termination * bce(term logits, terminated)
+ *   to grads (encoder, dynamics, reward, termination, the stacked Q heads, and the task embedding through every layer-0
+ *   input), like autograd accumulates .grad.  fp32 FFMA on the fp32 tensors w; reductions over rows in a fixed order
+ *   (repeated calls give identical bits); no allocation, no host synchronisation.  workspace: workspace_bytes(H, B). */
+typedef struct tdmpc2_linear_grad {
+  float* weight;
+  float* bias;
+  float* ln_weight;        /* NULL for a plain Linear (an MLP's layer 2) */
+  float* ln_bias;
+} tdmpc2_linear_grad;
+typedef struct tdmpc2_wm_grads {
+  int32_t num_enc;
+  tdmpc2_linear_grad enc[TDMPC2_MAX_ENC_LAYERS];
+  tdmpc2_linear_grad dynamics[3];
+  tdmpc2_linear_grad reward[3];
+  tdmpc2_linear_grad termination[3];   /* episodic models */
+  tdmpc2_linear_grad qs[3];            /* [num_q] leading dim, like _Qs.params.* */
+  float* task_emb;                     /* [num_tasks, T]; NULL for single-task models */
+} tdmpc2_wm_grads;
+typedef struct tdmpc2_wm_loss_coefs {
+  float consistency, reward, value, termination, rho;
+  float vmin, vmax, bin_size;          /* two_hot's range and bin width (math.py:58-71) */
+} tdmpc2_wm_loss_coefs;
+int tdmpc2_wm_loss_tape_bytes(const tdmpc2_planner* p, int H, int B, size_t* out);
+int tdmpc2_wm_loss_workspace_bytes(const tdmpc2_planner* p, int H, int B, size_t* out);
+int tdmpc2_wm_loss_forward(tdmpc2_planner* p, const float* obs0, const float* action, const int32_t* task,
+                           const float* dropout_mask, int H, int B, float* zs, float* q_logits, float* reward_logits,
+                           float* term_logits, float* tape, void* stream);
+int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* obs0,
+                            const float* action, const int32_t* task, const float* dropout_mask, int H, int B,
+                            const float* zs, const float* q_logits, const float* reward_logits, const float* term_logits,
+                            const float* next_z, const float* reward, const float* td_target, const float* terminated,
+                            const tdmpc2_wm_loss_coefs* coefs, const tdmpc2_wm_grads* grads, void* workspace, void* stream);
 
 /* Diagnostics: y[rows, out] = act(LN(x W^T + b)) for ONE packed layer, through
  * the same fused kernels (rows <= 128).  layer index: 0.. = enc, then dynamics

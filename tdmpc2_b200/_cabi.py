@@ -25,7 +25,8 @@ SYMBOLS = [
     "tdmpc2_planner_target_q_bytes", "tdmpc2_planner_bind_target_q", "tdmpc2_pack_target_q",
     "tdmpc2_wm_encode", "tdmpc2_wm_next", "tdmpc2_wm_reward", "tdmpc2_wm_termination", "tdmpc2_wm_pi", "tdmpc2_wm_q",
     "tdmpc2_td_target", "tdmpc2_pi_loss_tape_bytes", "tdmpc2_pi_loss_workspace_bytes", "tdmpc2_pi_loss_forward",
-    "tdmpc2_pi_loss_backward",
+    "tdmpc2_pi_loss_backward", "tdmpc2_wm_loss_tape_bytes", "tdmpc2_wm_loss_workspace_bytes", "tdmpc2_wm_loss_forward",
+    "tdmpc2_wm_loss_backward",
 ]
 
 
@@ -59,6 +60,19 @@ class ConvWeights(C.Structure):
 class PiGrads(C.Structure):
     _fields_ = [("weight", C.c_void_p * 3), ("bias", C.c_void_p * 3), ("ln_weight", C.c_void_p * 2),
                 ("ln_bias", C.c_void_p * 2), ("task_emb", C.c_void_p)]
+
+
+class LinearGrad(C.Structure):
+    _fields_ = [("weight", C.c_void_p), ("bias", C.c_void_p), ("ln_weight", C.c_void_p), ("ln_bias", C.c_void_p)]
+
+
+class WmGrads(C.Structure):
+    _fields_ = [("num_enc", C.c_int32), ("enc", LinearGrad * MAX_ENC_LAYERS), ("dynamics", LinearGrad * 3),
+                ("reward", LinearGrad * 3), ("termination", LinearGrad * 3), ("qs", LinearGrad * 3), ("task_emb", C.c_void_p)]
+
+
+class WmLossCoefs(C.Structure):
+    _fields_ = [(n, C.c_float) for n in ("consistency", "reward", "value", "termination", "rho", "vmin", "vmax", "bin_size")]
 
 
 class CabiError(RuntimeError):
@@ -133,6 +147,11 @@ def load():
     lib.tdmpc2_pi_loss_forward.argtypes = [vp, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
     lib.tdmpc2_pi_loss_backward.argtypes = [vp, C.POINTER(Weights), vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, C.c_float,
                                             C.c_float, C.POINTER(PiGrads), vp, vp]
+    lib.tdmpc2_wm_loss_tape_bytes.argtypes = [vp, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
+    lib.tdmpc2_wm_loss_workspace_bytes.argtypes = [vp, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
+    lib.tdmpc2_wm_loss_forward.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
+    lib.tdmpc2_wm_loss_backward.argtypes = [vp, C.POINTER(Weights), vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp,
+                                            vp, vp, C.POINTER(WmLossCoefs), C.POINTER(WmGrads), vp, vp]
     for s in SYMBOLS:
         f = getattr(lib, s)
         if f.restype is C.c_int and s not in ("tdmpc2_abi_version", "tdmpc2_planner_layer_count"):

@@ -46,7 +46,8 @@ _DEFAULTS: Dict[str, Any] = dict(
     latent_dim=512, task_dim=0, num_q=5, dropout=0.01, simnorm_dim=8,
     # discount heuristic (config.yaml:28-30)
     discount_denom=5, discount_min=0.95, discount_max=0.995,
-    # training keys (config.yaml:10-22); rho and grad_clip_norm are read by agent.update_pi
+    # training keys (config.yaml:10-22), read by agent._update / agent.update_pi
+    reward_coef=0.1, value_coef=0.1, termination_coef=1, consistency_coef=20,
     lr=3e-4, enc_lr_scale=0.3, tau=0.01, rho=0.5, grad_clip_norm=20, batch_size=256, seed=1, compile=False,
     # filled in by make_cfg
     multitask=False, tasks=None, obs_shape=None, action_dim=None, action_dims=None,

@@ -1069,7 +1069,7 @@ extern "C" int tdmpc2_pi_loss_forward(tdmpc2_planner* p, const float* z, const i
   PlanParams prm = rows_params(p, ROP_PI_LOSS, rows, task);
   prm.rows_in = z; prm.rows_eps = eps; prm.qidx = qidx; prm.rows_flag = 1;       // 'avg' of the online pair
   prm.rows_tape = tape; prm.rows_act_out = action_out; prm.rows_out = q_out; prm.rows_out4 = log_prob_out;
-  prm.rows_drop = dropout_mask;
+  prm.rows_drop = dropout_mask; prm.tape_pitch = planner_tape(p).pitch;
   return launch(p, prm, stream_);
 }
 
@@ -1187,6 +1187,344 @@ extern "C" int tdmpc2_pi_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* 
     pl_emb_grad<<<static_cast<int>((d.num_tasks * Tq + 127) / 128), 128, 0, st>>>(dxe, dxq, dxq + R * TA, TA, task, R, d.num_tasks,
                                                                                 static_cast<int>(Tq), gr->task_emb);
     CUDA_TRY(cudaGetLastError());
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------ agent._update (row-op tapes + grad_kernels.cuh)
+// The forward's tape (floats): one segment per row op, each [rows, pitch] of the pre-LayerNorm rows of its LayerNorm
+// layers in layer order -- encoder [B, (n_enc - 1) enc_dim + L]; dynamics [H B, 2 M + L] (step t's rows at t B);
+// reward [H B, 2 M]; Q 'all' [H B, 2 M num_q] (head h's layers 0, 1 at (2 h + l) M, layer 0 after dropout);
+// termination [H B, 2 M] (episodic).
+struct WmTape {
+  int p_enc, p_dyn, p_rew, p_q, p_term;
+  size_t enc, dyn, rew, q, term, floats;
+};
+static size_t take64(size_t& off, size_t n) { const size_t o = off; off += (n + 63) / 64 * 64; return o; }
+static WmTape wm_tape(const tdmpc2_planner* p, int H, int B) {
+  const tdmpc2_dims& d = p->d;
+  const size_t R = static_cast<size_t>(H) * B;
+  WmTape t;
+  t.p_enc = (p->num_enc - 1) * d.enc_dim + d.latent_dim;
+  t.p_dyn = 2 * d.mlp_dim + d.latent_dim; t.p_rew = 2 * d.mlp_dim; t.p_q = 2 * d.mlp_dim * d.num_q; t.p_term = 2 * d.mlp_dim;
+  size_t off = 0;
+  t.enc = take64(off, static_cast<size_t>(B) * t.p_enc);
+  t.dyn = take64(off, R * t.p_dyn);
+  t.rew = take64(off, R * t.p_rew);
+  t.q = take64(off, R * t.p_q);
+  t.term = d.episodic ? take64(off, R * t.p_term) : 0;
+  t.floats = off;
+  return t;
+}
+
+// Workspace of the backward (floats; ints for the head index array).
+struct WmWs {
+  size_t dlr, dlq, dlt, gA, gB, dyn, dy, hb, dxr, dxq, dxt, dxd, xa, dz, dp2, dyn2, dy2, dp1, dyn1, dy1, h1, dp0, dyn0, dy0,
+      h0, ea, eb, edyn, edy, eh, ex, exe, zero, part, iota, floats;
+  int nsplit;
+};
+static WmWs wm_ws(const tdmpc2_planner* p, int H, int B) {
+  const tdmpc2_dims& d = p->d;
+  const size_t R = static_cast<size_t>(H) * B, M = d.mlp_dim, L = d.latent_dim, T = d.task_dim, nb = d.num_bins, nq = d.num_q;
+  const size_t LT = L + T, D = L + T + d.action_dim, E = d.enc_dim, EL = std::max(E, L), OT = d.obs_dim + T;
+  WmWs w;
+  w.nsplit = std::max(1, std::min(8, static_cast<int>(R / 256)));
+  size_t off = 0;
+  w.dlr = take64(off, R * nb); w.dlq = take64(off, nq * R * nb); w.dlt = take64(off, R);
+  w.gA = take64(off, nq * R * M); w.gB = take64(off, nq * R * M); w.dyn = take64(off, nq * R * M); w.dy = take64(off, nq * R * M);
+  w.hb = take64(off, nq * R * M);
+  w.dxr = take64(off, R * LT); w.dxq = take64(off, nq * R * LT); w.dxt = take64(off, R * L); w.dxd = take64(off, R * LT);
+  w.xa = take64(off, R * D); w.dz = take64(off, B * L);
+  w.dp2 = take64(off, R * L); w.dyn2 = take64(off, R * L); w.dy2 = take64(off, R * L);
+  w.dp1 = take64(off, R * M); w.dyn1 = take64(off, R * M); w.dy1 = take64(off, R * M); w.h1 = take64(off, R * M);
+  w.dp0 = take64(off, R * M); w.dyn0 = take64(off, R * M); w.dy0 = take64(off, R * M); w.h0 = take64(off, R * M);
+  w.ea = take64(off, B * EL); w.eb = take64(off, B * EL); w.edyn = take64(off, B * EL); w.edy = take64(off, B * EL);
+  w.eh = take64(off, B * EL); w.ex = take64(off, B * OT); w.exe = take64(off, B * LT);
+  w.zero = take64(off, R * LT);
+  w.part = take64(off, static_cast<size_t>(w.nsplit) * std::max({M, L, E, nb}) * std::max({M, D, E, OT}));
+  w.iota = take64(off, nq);
+  w.floats = off;
+  return w;
+}
+
+static int wm_dims_ok(const tdmpc2_planner* p, int H, int B) {
+  if (H < 1 || B < 1) return fail(TDMPC2_ERR_INVALID, "H and B must be >= 1");
+  if (static_cast<long long>(H + 1) * B > 0x7fffffff) return fail(TDMPC2_ERR_INVALID, "H * B too large");
+  if (p->num_enc == 0) return fail(TDMPC2_ERR_UNSUPPORTED, "the world-model loss needs a state encoder (the conv encoder's backward is not built)");
+  return 0;
+}
+
+extern "C" int tdmpc2_wm_loss_tape_bytes(const tdmpc2_planner* p, int H, int B, size_t* out) {
+  if (!p || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  int rc = wm_dims_ok(p, H, B);
+  if (rc) return rc;
+  *out = wm_tape(p, H, B).floats * 4;
+  return 0;
+}
+
+extern "C" int tdmpc2_wm_loss_workspace_bytes(const tdmpc2_planner* p, int H, int B, size_t* out) {
+  if (!p || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  int rc = wm_dims_ok(p, H, B);
+  if (rc) return rc;
+  *out = wm_ws(p, H, B).floats * 4;
+  return 0;
+}
+
+extern "C" int tdmpc2_wm_loss_forward(tdmpc2_planner* p, const float* obs0, const float* action, const int32_t* task,
+                                      const float* dropout_mask, int H, int B, float* zs, float* q_logits, float* reward_logits,
+                                      float* term_logits, float* tape, void* stream_) {
+  int rc = rows_ready(p, B);
+  if (rc || (rc = wm_dims_ok(p, H, B)) || (rc = need_task(p, task))) return rc;
+  if (!obs0 || !action || !zs || !q_logits || !reward_logits || !tape) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (p->d.episodic && !term_logits) return fail(TDMPC2_ERR_INVALID, "episodic model needs term_logits");
+  const tdmpc2_dims& d = p->d;
+  const int R = H * B;
+  const size_t L = d.latent_dim, A = d.action_dim;
+  const WmTape tp = wm_tape(p, H, B);
+  PlanParams prm = rows_params(p, ROP_ENCODE, B, task);
+  prm.rows_in = obs0; prm.rows_out = zs; prm.rows_tape = tape + tp.enc; prm.tape_pitch = tp.p_enc;
+  if ((rc = launch(p, prm, stream_))) return rc;
+  for (int t = 0; t < H; ++t) {
+    const size_t r0 = static_cast<size_t>(t) * B;
+    prm = rows_params(p, ROP_NEXT, B, task ? task + r0 : nullptr);
+    prm.rows_in = zs + r0 * L; prm.rows_act = action + r0 * A; prm.rows_out = zs + (r0 + B) * L;
+    prm.rows_tape = tape + tp.dyn + r0 * tp.p_dyn; prm.tape_pitch = tp.p_dyn;
+    if ((rc = launch(p, prm, stream_))) return rc;
+  }
+  prm = rows_params(p, ROP_Q_ALL, R, task);
+  prm.rows_in = zs; prm.rows_act = action; prm.rows_out = q_logits;
+  prm.rows_tape = tape + tp.q; prm.tape_pitch = tp.p_q; prm.rows_drop = dropout_mask;
+  if ((rc = launch(p, prm, stream_))) return rc;
+  prm = rows_params(p, ROP_REWARD, R, task);
+  prm.rows_in = zs; prm.rows_act = action; prm.rows_out = reward_logits; prm.rows_tape = tape + tp.rew; prm.tape_pitch = tp.p_rew;
+  if ((rc = launch(p, prm, stream_))) return rc;
+  if (d.episodic) {
+    prm = rows_params(p, ROP_TERM, R, nullptr);
+    prm.rows_in = zs + static_cast<size_t>(B) * L; prm.rows_out = term_logits; prm.rows_flag = 0;
+    prm.rows_tape = tape + tp.term; prm.tape_pitch = tp.p_term;
+    if ((rc = launch(p, prm, stream_))) return rc;
+  }
+  return 0;
+}
+
+static bool lin_ok(const tdmpc2_linear& l, bool ln) { return l.weight && l.bias && (!ln || (l.ln_weight && l.ln_bias)); }
+static bool grad_ok(const tdmpc2_linear_grad& g, bool ln) { return g.weight && g.bias && (!ln || (g.ln_weight && g.ln_bias)); }
+
+extern "C" int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* obs0,
+                                       const float* action, const int32_t* task, const float* dropout_mask, int H, int B,
+                                       const float* zs, const float* q_logits, const float* reward_logits, const float* term_logits,
+                                       const float* next_z, const float* reward, const float* td_target, const float* terminated,
+                                       const tdmpc2_wm_loss_coefs* cf, const tdmpc2_wm_grads* gr, void* workspace, void* stream_) {
+  int rc = rows_ready(p, B);
+  if (rc || (rc = wm_dims_ok(p, H, B)) || (rc = need_task(p, task))) return rc;
+  const tdmpc2_dims& d = p->d;
+  if (!w || !tape || !obs0 || !action || !zs || !q_logits || !reward_logits || !next_z || !reward || !td_target || !cf || !gr ||
+      !workspace)
+    return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (d.episodic && (!term_logits || !terminated)) return fail(TDMPC2_ERR_INVALID, "episodic model needs term_logits and terminated");
+  if (w->num_enc != p->num_enc || gr->num_enc != p->num_enc) return fail(TDMPC2_ERR_INVALID, "num_enc differs from the planner's");
+  for (int i = 0; i < p->num_enc; ++i)
+    if (!lin_ok(w->enc[i], true) || !grad_ok(gr->enc[i], true)) return fail(TDMPC2_ERR_INVALID, "null encoder tensor or gradient");
+  for (int i = 0; i < 3; ++i) {
+    if (!lin_ok(w->dynamics[i], true) || !lin_ok(w->reward[i], i < 2) || !lin_ok(w->qs[i], i < 2) || !grad_ok(gr->dynamics[i], true) ||
+        !grad_ok(gr->reward[i], i < 2) || !grad_ok(gr->qs[i], i < 2))
+      return fail(TDMPC2_ERR_INVALID, "null weight or gradient");
+    if (d.episodic && (!lin_ok(w->termination[i], i < 2) || !grad_ok(gr->termination[i], i < 2)))
+      return fail(TDMPC2_ERR_INVALID, "null termination weight or gradient");
+  }
+  if (d.task_dim > 0 && !gr->task_emb) return fail(TDMPC2_ERR_INVALID, "multi-task model needs the task-embedding gradient");
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  const WmTape tp = wm_tape(p, H, B);
+  const WmWs W = wm_ws(p, H, B);
+  float* ws = static_cast<float*>(workspace);
+  const int R = H * B, nq = d.num_q;
+  const long long M = d.mlp_dim, nb = d.num_bins, A = d.action_dim, Tq = d.task_dim, Lz = d.latent_dim, E = d.enc_dim;
+  const long long LT = Lz + Tq, D = Lz + Tq + A, OT = d.obs_dim + Tq;
+  const float fH = static_cast<float>(H), fB = static_cast<float>(B);
+  float* X = ws + W.xa;
+  int* iota = reinterpret_cast<int*>(ws + W.iota);
+  auto ok = [&]() -> int { CUDA_TRY(cudaGetLastError()); return 0; };
+  auto colsum = [&](const float* src, int rows, long long n, long long ld, float* dst) -> int {
+    pl_colsum<<<static_cast<int>((n + 127) / 128), 128, 0, st>>>(src, rows, static_cast<int>(n), ld, dst);
+    return ok();
+  };
+  // dst [m, n] += src^T x over `rows` rows (src [rows, m], x [rows, n] with row pitch ldx), split-K partials summed in order
+  auto dweight = [&](const float* src, long long m, const float* x, long long n, long long ldx, int rows, float* dst) -> int {
+    GemmArgs g{src, 1, m, 0, x, ldx, 1, 0, nullptr, ws + W.part, n, 0, m * n, static_cast<int>(m), static_cast<int>(n), rows, W.nsplit};
+    int rc2 = gemm(g, 1, st);
+    if (rc2) return rc2;
+    pl_reduce<<<static_cast<int>((m * n + 255) / 256), 256, 0, st>>>(ws + W.part, W.nsplit, m * n, m * n, dst);
+    return ok();
+  };
+  // out [rows, n] = g [rows, k] W[:, :n] (W [k, ldw]), batched over `batch` heads (g, out strides; W by bsel)
+  auto dinput = [&](const float* g, long long k, const float* Wt, long long ldw, long long w_z, const int* bsel, int batch,
+                    long long n, float* out, long long ldo, long long o_z, int rows) -> int {
+    return gemm(GemmArgs{g, k, 1, static_cast<long long>(rows) * k, Wt, ldw, 1, w_z, bsel, out, ldo, o_z, 0, rows,
+                         static_cast<int>(n), static_cast<int>(k), 1}, batch, st);
+  };
+  // the three layers of a head MLP (NormedLinear 0, 1 and a plain Linear 2) from dL/dlogits dl [batch, R, nout]: parameter
+  // gradients of every layer (layer 0's input x0 [R, K0], row pitch ld0) and dX [batch, R, nx] of layer 0's first nx
+  // input columns (ld ldx)
+  auto head_back = [&](const float* dl, long long nout, const tdmpc2_linear* lw, const tdmpc2_linear_grad* lg, int batch,
+                       const float* tape_seg, int pitch, long long off_z, const float* drop, const float* x0, long long K0,
+                       long long ld0, long long nx, float* dx, long long ldx) -> int {
+    int rc2;
+    float *gA = ws + W.gA, *gB = ws + W.gB, *dyn = ws + W.dyn, *dy = ws + W.dy, *hb = ws + W.hb;
+    const long long RM = static_cast<long long>(R) * M;
+    const int* hs = batch > 1 ? iota : nullptr;
+    if ((rc2 = dinput(dl, nout, lw[2].weight, M, nout * M, hs, batch, M, gA, M, RM, R))) return rc2;
+    LnBackArgs lb{};
+    lb.tape = tape_seg; lb.pitch = pitch; lb.rows = R; lb.N = static_cast<int>(M); lb.ld = M; lb.off_z = off_z; lb.g_z = RM;
+    lb.o_z = RM; lb.hsel = hs; lb.dyn = dyn; lb.dy = dy; lb.h = hb;
+    lb.off = static_cast<int>(M); lb.g = gA; lb.out = gA; lb.gamma = lw[1].ln_weight; lb.beta = lw[1].ln_bias;
+    pl_ln_back<<<dim3((R + 7) / 8, batch), 256, 0, st>>>(lb);
+    if ((rc2 = ok())) return rc2;
+    for (int h = 0; h < batch; ++h) {
+      const long long o = h * RM;
+      if ((rc2 = colsum(dyn + o, R, M, M, lg[1].ln_weight + h * M)) || (rc2 = colsum(dy + o, R, M, M, lg[1].ln_bias + h * M)) ||
+          (rc2 = dweight(dl + h * R * nout, nout, hb + o, M, M, R, lg[2].weight + h * nout * M)) ||
+          (rc2 = colsum(dl + h * R * nout, R, nout, nout, lg[2].bias + h * nout)))
+        return rc2;
+    }
+    if ((rc2 = dinput(gA, M, lw[1].weight, M, M * M, hs, batch, M, gB, M, RM, R))) return rc2;
+    lb.off = 0; lb.g = gB; lb.out = gB; lb.gamma = lw[0].ln_weight; lb.beta = lw[0].ln_bias; lb.drop = drop;
+    pl_ln_back<<<dim3((R + 7) / 8, batch), 256, 0, st>>>(lb);
+    if ((rc2 = ok())) return rc2;
+    for (int h = 0; h < batch; ++h) {
+      const long long o = h * RM;
+      if ((rc2 = colsum(dyn + o, R, M, M, lg[0].ln_weight + h * M)) || (rc2 = colsum(dy + o, R, M, M, lg[0].ln_bias + h * M)) ||
+          (rc2 = dweight(gA + o, M, hb + o, M, M, R, lg[1].weight + h * M * M)) || (rc2 = colsum(gA + o, R, M, M, lg[1].bias + h * M)) ||
+          (rc2 = dweight(gB + o, M, x0, K0, ld0, R, lg[0].weight + h * M * K0)) || (rc2 = colsum(gB + o, R, M, M, lg[0].bias + h * M)))
+        return rc2;
+    }
+    return dinput(gB, M, lw[0].weight, K0, M * K0, hs, batch, nx, dx, ldx, static_cast<long long>(R) * ldx, R);
+  };
+
+  pl_iota<<<1, 32 * ((nq + 31) / 32), 0, st>>>(iota, nq);
+  if ((rc = ok())) return rc;
+  // X = [zs[:H] | emb | action]: the layer-0 input of the dynamics, reward and Q heads (z columns first)
+  pl_gather_xa<<<static_cast<int>((R * D + 255) / 256), 256, 0, st>>>(zs, p->base.emb, task, action, R, static_cast<int>(Lz),
+                                                                     static_cast<int>(Tq), static_cast<int>(A), X);
+  if ((rc = ok())) return rc;
+
+  // ---- 1. the heads, all H B rows at once: Q (batched over heads), reward, termination
+  pl_soft_ce_back<<<dim3((R + 7) / 8, nq), 256, 0, st>>>(q_logits, static_cast<long long>(R) * nb, R, static_cast<int>(nb), td_target,
+                                                         cf->vmin, cf->vmax, cf->bin_size, cf->value / (fH * nq * fB), cf->rho, B,
+                                                         ws + W.dlq);
+  if ((rc = ok())) return rc;
+  if ((rc = head_back(ws + W.dlq, nb, w->qs, gr->qs, nq, tape + tp.q, tp.p_q, 2 * M, dropout_mask, X, D, D, LT, ws + W.dxq, LT)))
+    return rc;
+  pl_soft_ce_back<<<dim3((R + 7) / 8, 1), 256, 0, st>>>(reward_logits, 0, R, static_cast<int>(nb), reward, cf->vmin, cf->vmax,
+                                                        cf->bin_size, cf->reward / (fH * fB), cf->rho, B, ws + W.dlr);
+  if ((rc = ok())) return rc;
+  if ((rc = head_back(ws + W.dlr, nb, w->reward, gr->reward, 1, tape + tp.rew, tp.p_rew, 0, nullptr, X, D, D, LT, ws + W.dxr, LT)))
+    return rc;
+  if (d.episodic) {
+    pl_bce_back<<<(R + 255) / 256, 256, 0, st>>>(term_logits, terminated, R, cf->termination / (fH * fB), ws + W.dlt);
+    if ((rc = ok())) return rc;
+    // termination reads [z_{t+1}] alone: its layer-0 input is zs[1:], a contiguous [R, L] block
+    if ((rc = head_back(ws + W.dlt, 1, w->termination, gr->termination, 1, tape + tp.term, tp.p_term, 0, nullptr,
+                        zs + static_cast<size_t>(B) * Lz, Lz, Lz, Lz, ws + W.dxt, Lz)))
+      return rc;
+  }
+
+  // ---- 2. back through time: dz_t, then dynamics step t - 1 (layers 2 -> 0) to its [z | emb] input columns
+  DzArgs za{};
+  za.zs = zs; za.next_z = next_z; za.dxq = ws + W.dxq; za.q_z = static_cast<long long>(R) * LT; za.nq = nq; za.dxr = ws + W.dxr;
+  za.dxd = ws + W.dxd; za.ld = LT; za.dxt = d.episodic ? ws + W.dxt : nullptr; za.ldt = Lz;
+  za.cons = cf->consistency * 2.f / (fH * fB * static_cast<float>(Lz)); za.rho = cf->rho; za.H = H; za.Bsz = B;
+  za.L = static_cast<int>(Lz); za.dz = ws + W.dz;
+  const int dz_blocks = static_cast<int>((B * Lz + 255) / 256), b8 = (B + 7) / 8;
+  for (int t = H; t >= 1; --t) {
+    za.t = t;
+    pl_dz_step<<<dz_blocks, 256, 0, st>>>(za);
+    if ((rc = ok())) return rc;
+    const size_t r0 = static_cast<size_t>(t - 1) * B;
+    const float* tseg = tape + tp.dyn + r0 * tp.p_dyn;
+    LnBackArgs lb{};
+    lb.tape = tseg; lb.pitch = tp.p_dyn; lb.rows = B; lb.off = static_cast<int>(2 * M); lb.N = static_cast<int>(Lz); lb.ld = Lz;
+    lb.g = ws + W.dz; lb.out = ws + W.dp2 + r0 * Lz; lb.gamma = w->dynamics[2].ln_weight; lb.beta = w->dynamics[2].ln_bias;
+    lb.dyn = ws + W.dyn2 + r0 * Lz; lb.dy = ws + W.dy2 + r0 * Lz;
+    pl_ln_simnorm_back<<<b8, 256, 0, st>>>(lb, d.simnorm_dim);
+    if ((rc = ok())) return rc;
+    if ((rc = dinput(ws + W.dp2 + r0 * Lz, Lz, w->dynamics[2].weight, M, 0, nullptr, 1, M, ws + W.dp1 + r0 * M, M, 0, B))) return rc;
+    lb.off = static_cast<int>(M); lb.N = static_cast<int>(M); lb.ld = M; lb.g = lb.out = ws + W.dp1 + r0 * M;
+    lb.gamma = w->dynamics[1].ln_weight; lb.beta = w->dynamics[1].ln_bias;
+    lb.dyn = ws + W.dyn1 + r0 * M; lb.dy = ws + W.dy1 + r0 * M; lb.h = ws + W.h1 + r0 * M;
+    pl_ln_back<<<b8, 256, 0, st>>>(lb);
+    if ((rc = ok())) return rc;
+    if ((rc = dinput(ws + W.dp1 + r0 * M, M, w->dynamics[1].weight, M, 0, nullptr, 1, M, ws + W.dp0 + r0 * M, M, 0, B))) return rc;
+    lb.off = 0; lb.g = lb.out = ws + W.dp0 + r0 * M; lb.gamma = w->dynamics[0].ln_weight; lb.beta = w->dynamics[0].ln_bias;
+    lb.dyn = ws + W.dyn0 + r0 * M; lb.dy = ws + W.dy0 + r0 * M; lb.h = ws + W.h0 + r0 * M;
+    pl_ln_back<<<b8, 256, 0, st>>>(lb);
+    if ((rc = ok())) return rc;
+    if ((rc = dinput(ws + W.dp0 + r0 * M, M, w->dynamics[0].weight, D, 0, nullptr, 1, LT, ws + W.dxd + r0 * LT, LT, 0, B))) return rc;
+  }
+  za.t = 0;
+  pl_dz_step<<<dz_blocks, 256, 0, st>>>(za);
+  if ((rc = ok())) return rc;
+
+  // ---- 3. the dynamics' parameter gradients: one reduction over all H B taped rows per layer
+  const tdmpc2_linear_grad* gd = gr->dynamics;
+  if ((rc = dweight(ws + W.dp2, Lz, ws + W.h1, M, M, R, gd[2].weight)) || (rc = colsum(ws + W.dp2, R, Lz, Lz, gd[2].bias)) ||
+      (rc = colsum(ws + W.dyn2, R, Lz, Lz, gd[2].ln_weight)) || (rc = colsum(ws + W.dy2, R, Lz, Lz, gd[2].ln_bias)) ||
+      (rc = dweight(ws + W.dp1, M, ws + W.h0, M, M, R, gd[1].weight)) || (rc = colsum(ws + W.dp1, R, M, M, gd[1].bias)) ||
+      (rc = colsum(ws + W.dyn1, R, M, M, gd[1].ln_weight)) || (rc = colsum(ws + W.dy1, R, M, M, gd[1].ln_bias)) ||
+      (rc = dweight(ws + W.dp0, M, X, D, D, R, gd[0].weight)) || (rc = colsum(ws + W.dp0, R, M, M, gd[0].bias)) ||
+      (rc = colsum(ws + W.dyn0, R, M, M, gd[0].ln_weight)) || (rc = colsum(ws + W.dy0, R, M, M, gd[0].ln_bias)))
+    return rc;
+
+  // ---- 4. dz_0 through the encoder: the SimNorm layer, then the Mish layers down to layer 0 (input [obs | emb])
+  {
+    const int ne = p->num_enc;
+    float *cur = ws + W.ea, *nxt = ws + W.eb;
+    LnBackArgs lb{};
+    lb.tape = tape + tp.enc; lb.pitch = tp.p_enc; lb.rows = B; lb.off = static_cast<int>((ne - 1) * E); lb.N = static_cast<int>(Lz);
+    lb.ld = Lz; lb.g = ws + W.dz; lb.out = cur; lb.gamma = w->enc[ne - 1].ln_weight; lb.beta = w->enc[ne - 1].ln_bias;
+    lb.dyn = ws + W.edyn; lb.dy = ws + W.edy;
+    pl_ln_simnorm_back<<<b8, 256, 0, st>>>(lb, d.simnorm_dim);
+    if ((rc = ok())) return rc;
+    if ((rc = colsum(ws + W.edyn, B, Lz, Lz, gr->enc[ne - 1].ln_weight)) || (rc = colsum(ws + W.edy, B, Lz, Lz, gr->enc[ne - 1].ln_bias)) ||
+        (rc = colsum(cur, B, Lz, Lz, gr->enc[ne - 1].bias)))
+      return rc;
+    long long n_cur = Lz;
+    for (int i = ne - 2; i >= 0; --i) {
+      if ((rc = dinput(cur, n_cur, w->enc[i + 1].weight, E, 0, nullptr, 1, E, nxt, E, 0, B))) return rc;
+      LnBackArgs le{};
+      le.tape = tape + tp.enc; le.pitch = tp.p_enc; le.rows = B; le.off = static_cast<int>(i * E); le.N = static_cast<int>(E); le.ld = E;
+      le.g = le.out = nxt; le.gamma = w->enc[i].ln_weight; le.beta = w->enc[i].ln_bias;
+      le.dyn = ws + W.edyn; le.dy = ws + W.edy; le.h = ws + W.eh;
+      pl_ln_back<<<b8, 256, 0, st>>>(le);
+      if ((rc = ok())) return rc;
+      if ((rc = dweight(cur, n_cur, ws + W.eh, E, E, B, gr->enc[i + 1].weight)) ||
+          (rc = colsum(ws + W.edyn, B, E, E, gr->enc[i].ln_weight)) || (rc = colsum(ws + W.edy, B, E, E, gr->enc[i].ln_bias)) ||
+          (rc = colsum(nxt, B, E, E, gr->enc[i].bias)))
+        return rc;
+      std::swap(cur, nxt);
+      n_cur = E;
+    }
+    const float* xe = obs0;
+    if (Tq > 0) {
+      pl_gather_x<<<static_cast<int>((B * OT + 255) / 256), 256, 0, st>>>(obs0, p->base.emb, task, B, d.obs_dim, static_cast<int>(Tq),
+                                                                         ws + W.ex);
+      if ((rc = ok())) return rc;
+      xe = ws + W.ex;
+    }
+    if ((rc = dweight(cur, n_cur, xe, OT, OT, B, gr->enc[0].weight))) return rc;
+    if (Tq > 0) {
+      // ---- 5. the task embedding: encoder layer 0, dynamics layer 0, reward layer 0, each Q head's layer 0, in order
+      if ((rc = dinput(cur, n_cur, w->enc[0].weight + d.obs_dim, OT, 0, nullptr, 1, Tq, ws + W.exe + Lz, LT, 0, B))) return rc;
+      CUDA_TRY(cudaMemsetAsync(ws + W.zero, 0, static_cast<size_t>(R) * LT * 4, st));
+      const float* z0 = ws + W.zero;
+      const dim3 eg(static_cast<int>((d.num_tasks * Tq + 127) / 128));
+      pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.exe + Lz, z0, z0, LT, task, B, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
+      pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.dxd + Lz, z0, z0, LT, task, R, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
+      pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.dxr + Lz, z0, z0, LT, task, R, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
+      for (int h = 0; h < nq; ++h)
+        pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.dxq + h * static_cast<long long>(R) * LT + Lz, z0, z0, LT, task, R, d.num_tasks,
+                                        static_cast<int>(Tq), gr->task_emb);
+      if ((rc = ok())) return rc;
+    }
   }
   return 0;
 }

@@ -145,6 +145,7 @@ struct LnBackArgs {
   const float* drop;                                        // dropout scale [heads, rows, N] or nullptr
   float* dyn; float* dy; float* h;                          // [rows, ld] or nullptr
   int rows, N;
+  long long o_z;                                            // batch stride of dyn / dy / h (0: shared by every batch)
 };
 __global__ void __launch_bounds__(256) pl_ln_back(const LnBackArgs a) {
   const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, u = blockIdx.y;
@@ -170,7 +171,7 @@ __global__ void __launch_bounds__(256) pl_ln_back(const LnBackArgs a) {
     const float dy = g[j] * (t + y * sg * (1.f - t * t));
     const float dn = dy * gm[j];
     s1 += dn; s2 = fmaf(dn, n, s2);
-    const size_t o = static_cast<size_t>(r) * a.ld + j;
+    const size_t o = u * a.o_z + static_cast<size_t>(r) * a.ld + j;
     if (a.dyn) { a.dyn[o] = dy * n; a.dy[o] = dy; }
     if (a.h) a.h[o] = y > 20.f ? y : y * t;
     out[j] = dn;                 // dn parked in out until the row's two sums are known (out may alias g: g[j] is read)
@@ -261,6 +262,142 @@ __global__ void pl_emb_grad(const float* __restrict__ s0, const float* __restric
   for (int r = 0; r < rows; ++r)
     if (task[r] == t) v += (s0[r * ld + cc] + s1[r * ld + cc]) + s2[r * ld + cc];
   dst[i] += v;
+}
+
+// ------------------------------------------------------------------------------------ agent._update (world-model loss)
+// The backward of the reference's _update loss (tdmpc2.py:259-313) from the tapes of the row ops ENCODE / NEXT / REWARD /
+// Q_ALL / TERM (api.cu, tdmpc2_wm_loss_backward): the heads' row gradients below, then the generic GEMM / LayerNorm
+// kernels above through the heads, back through time over the dynamics, and through the encoder.
+
+// Soft cross-entropy backward (math.py:33-37, 58-71) per row r and batch u = blockIdx.y (Q head, or the reward head):
+//   tw = two_hot(target_r); dl = w_r (softmax(l) sum(tw) - tw), w_r = coef rho^(r / Bsz)
+// two_hot as the reference computes it in fp32: symlog, clamp to [vmin, vmax], divide by bin_size, floor, and the lower
+// bin's neighbour at (idx + 1) % nb.
+__global__ void __launch_bounds__(256) pl_soft_ce_back(const float* __restrict__ logits, long long l_z, int rows, int nb,
+                                                       const float* __restrict__ target, float vmin, float vmax, float bin_size,
+                                                       float coef, float rho, int Bsz, float* __restrict__ dl) {
+  const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, u = blockIdx.y;
+  if (r >= rows) return;
+  const float* l = logits + u * l_z + static_cast<size_t>(r) * nb;
+  const float y = target[r];
+  const float sl = copysignf(logf(1.f + fabsf(y)), y);                                // sign(x) log(1 + |x|)
+  const float x = fminf(fmaxf(sl, vmin), vmax);
+  const float pos = (x - vmin) / bin_size;
+  const float fidx = floorf(pos);
+  const float off = pos - fidx;
+  const int i0 = static_cast<int>(fidx), i1 = (i0 + 1) % nb;
+  const float sum_tw = (1.f - off) + off;
+  float m = -INFINITY;
+  for (int i = lane; i < nb; i += 32) m = fmaxf(m, l[i]);
+  m = pl_warp_max(m);
+  float den = 0.f;
+  for (int i = lane; i < nb; i += 32) den += expf(l[i] - m);
+  den = pl_warp_sum(den);
+  const float w = coef * powf(rho, static_cast<float>(r / Bsz));
+  float* o = dl + u * l_z + static_cast<size_t>(r) * nb;
+  for (int i = lane; i < nb; i += 32) {
+    const float tw = i == i0 ? 1.f - off : i == i1 ? off : 0.f;
+    o[i] = w * (expf(l[i] - m) / den * sum_tw - tw);
+  }
+}
+
+// BCE-with-logits backward (mean over rows): dl = coef (sigmoid(l) - y)
+__global__ void pl_bce_back(const float* __restrict__ l, const float* __restrict__ y, int rows, float coef, float* __restrict__ dl) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  dl[r] = coef * (1.f / (1.f + expf(-l[r])) - y[r]);
+}
+
+// LayerNorm + SimNorm backward of the encoder's / the dynamics' last layer, per row r (a.hsel, a.drop unused).  From the
+// tape's pre row: n = LayerNorm(pre), y = gamma n + beta, s = softmax of y over groups of V columns.  g = dL/ds:
+//   dy = s (g - sum_grp s g); dn = dy gamma; dpre = rstd (dn - mean(dn) - n mean(dn n)) -> out (may alias g)
+// Each lane owns whole groups (lane + 32 k), so the group sums stay in the lane.
+__global__ void __launch_bounds__(256) pl_ln_simnorm_back(const LnBackArgs a, int V) {
+  const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= a.rows) return;
+  const float* pre = a.tape + static_cast<size_t>(r) * a.pitch + a.off;
+  const float* g = a.g + static_cast<size_t>(r) * a.ld;
+  float* out = a.out + static_cast<size_t>(r) * a.ld;
+  const float invN = 1.f / static_cast<float>(a.N);
+  float s = 0.f;
+  for (int j = lane; j < a.N; j += 32) s += pre[j];
+  const float mean = pl_warp_sum(s) * invN;
+  float sq = 0.f;
+  for (int j = lane; j < a.N; j += 32) { const float d = pre[j] - mean; sq = fmaf(d, d, sq); }
+  const float rstd = 1.f / sqrtf(pl_warp_sum(sq) * invN + 1e-5f);
+  float s1 = 0.f, s2 = 0.f;
+  for (int c0 = lane * V; c0 < a.N; c0 += 32 * V) {
+    float mx = -INFINITY;
+    for (int j = c0; j < c0 + V; ++j) mx = fmaxf(mx, fmaf((pre[j] - mean) * rstd, a.gamma[j], a.beta[j]));
+    float den = 0.f, sg = 0.f;
+    for (int j = c0; j < c0 + V; ++j) {
+      const float e = expf(fmaf((pre[j] - mean) * rstd, a.gamma[j], a.beta[j]) - mx);
+      den += e; sg = fmaf(e, g[j], sg);
+    }
+    sg /= den;
+    for (int j = c0; j < c0 + V; ++j) {
+      const float n = (pre[j] - mean) * rstd;
+      const float sm = expf(fmaf(n, a.gamma[j], a.beta[j]) - mx) / den;
+      const float dy = sm * (g[j] - sg);
+      const float dn = dy * a.gamma[j];
+      s1 += dn; s2 = fmaf(dn, n, s2);
+      const size_t o = static_cast<size_t>(r) * a.ld + j;
+      if (a.dyn) { a.dyn[o] = dy * n; a.dy[o] = dy; }
+      out[j] = dn;
+    }
+  }
+  s1 = pl_warp_sum(s1) * invN;
+  s2 = pl_warp_sum(s2) * invN;
+  __syncwarp();
+  for (int c0 = lane * V; c0 < a.N; c0 += 32 * V)
+    for (int j = c0; j < c0 + V; ++j) out[j] = rstd * (out[j] - s1 - (pre[j] - mean) * rstd * s2);
+}
+
+// dL/dz_t [Bsz, L] of rollout step t (row r = t Bsz + b of the [H, Bsz] head batches):
+//   consistency (t >= 1): cons rho^(t-1) (z_t - next_z_{t-1})      (cons = coef 2 / (H Bsz L))
+//   + the Q heads' dX (t < H, heads in order) + the reward head's (t < H) + the termination head's (t >= 1, rows of
+//   z_1..z_H) + dynamics step t's (t < H); dX of the heads and dynamics carry ld columns, z first.
+struct DzArgs {
+  const float* zs; const float* next_z;
+  const float* dxq; long long q_z; int nq; const float* dxr; const float* dxd; long long ld;
+  const float* dxt; long long ldt;
+  float cons, rho;
+  int t, H, Bsz, L;
+  float* dz;
+};
+__global__ void pl_dz_step(const DzArgs a) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.Bsz * a.L) return;
+  const int b = i / a.L, c = i % a.L;
+  float v = 0.f;
+  if (a.t >= 1) {
+    const size_t zi = (static_cast<size_t>(a.t) * a.Bsz + b) * a.L + c, ni = (static_cast<size_t>(a.t - 1) * a.Bsz + b) * a.L + c;
+    v = a.cons * powf(a.rho, static_cast<float>(a.t - 1)) * (a.zs[zi] - a.next_z[ni]);
+  }
+  if (a.t < a.H) {
+    const size_t row = static_cast<size_t>(a.t) * a.Bsz + b;
+    for (int q = 0; q < a.nq; ++q) v += a.dxq[q * a.q_z + row * a.ld + c];
+    v += a.dxr[row * a.ld + c];
+    v += a.dxd[row * a.ld + c];
+  }
+  if (a.t >= 1 && a.dxt) v += a.dxt[(static_cast<size_t>(a.t - 1) * a.Bsz + b) * a.ldt + c];
+  a.dz[i] = v;
+}
+
+// x[r] = [z_r | emb_{task[r]} | a_r]: the input of dynamics / reward / Q layer 0 (T == 0: no embedding columns)
+__global__ void pl_gather_xa(const float* __restrict__ z, const float* __restrict__ emb, const int* __restrict__ task,
+                             const float* __restrict__ act, int rows, int L, int T, int A, float* __restrict__ x) {
+  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  const int D = L + T + A;
+  if (i >= static_cast<long long>(rows) * D) return;
+  const int r = static_cast<int>(i / D), c = static_cast<int>(i % D);
+  x[i] = c < L ? z[static_cast<size_t>(r) * L + c]
+       : c < L + T ? emb[static_cast<size_t>(task[r]) * T + c - L] : act[static_cast<size_t>(r) * A + c - L - T];
+}
+
+__global__ void pl_iota(int* __restrict__ dst, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = i;
 }
 
 }  // namespace tdmpc2

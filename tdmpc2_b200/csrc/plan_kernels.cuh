@@ -143,6 +143,10 @@ struct PlanParams {
   float* rows_tape;                // [rows, tape.pitch]: see PiTape
   float* rows_act_out;             // action [rows, A]
   const float* rows_drop;          // Q layer 0 dropout scale (mask / (1 - p)) [num_q, rows, M], or nullptr (eval mode)
+  // Row pitch (floats) of rows_tape.  ROP_PI_LOSS: PiTape::pitch.  ROP_ENCODE / NEXT / REWARD / TERM / Q_ALL with a
+  // non-null rows_tape (agent._update's forward): the pre-LayerNorm rows of every LayerNorm layer of the launch, see
+  // WmTape in api.cu; Q_ALL also applies rows_drop to each head's layer 0 then.
+  int tape_pitch;
 };
 
 // The tape of ROP_PI_LOSS, per row (fp32 offsets): the pre-LayerNorm rows of pi.0 and pi.1 [M], the pi head's logits
@@ -645,7 +649,7 @@ __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const L
         s += x[j];
       }
       if (ROWS && live && ea.tape) {
-        float* trow = ea.tape + static_cast<size_t>(ea.rowmap[r]) * pi_tape(P.M, P.A, P.Apad, P.B).pitch;
+        float* trow = ea.tape + static_cast<size_t>(ea.rowmap[r]) * P.tape_pitch;
 #pragma unroll
         for (int j = 0; j < kLnRegCols; ++j) trow[c.lane + 32 * j] = x[j];
       }
@@ -677,7 +681,7 @@ __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const L
       const float* rr = rawbase + static_cast<size_t>(r) * P.NpadMax;
       const int orow = ea.rowmap[r];
       const float* drow = ea.drop && orow >= 0 ? ea.drop + static_cast<size_t>(orow) * N : nullptr;
-      float* trow = ea.tape && orow >= 0 ? ea.tape + static_cast<size_t>(orow) * pi_tape(P.M, P.A, P.Apad, P.B).pitch : nullptr;
+      float* trow = ea.tape && orow >= 0 ? ea.tape + static_cast<size_t>(orow) * P.tape_pitch : nullptr;
       float s = 0.f;
       for (int col = c.lane; col < N; col += 32) {
         float v = fmaf(__ldcg(rr + col), inv_scale, __ldg(bias + col));
@@ -784,7 +788,7 @@ __device__ __forceinline__ void rows_commit(const PlanParams& P, Ctx& c, const E
     P.rows_out[row] = q;
     if (P.rows_tape) {
       const PiTape tp = pi_tape(P.M, P.A, P.Apad, P.B);
-      P.rows_tape[static_cast<size_t>(row) * tp.pitch + tp.qv] = q;
+      P.rows_tape[static_cast<size_t>(row) * P.tape_pitch + tp.qv] = q;
     }
   }
 }
@@ -815,7 +819,7 @@ __device__ __forceinline__ void rows_pi(const PlanParams& P, Ctx& c, const float
     }
     if (P.rows_tape && row >= 0) {
       P.rows_act_out[static_cast<size_t>(row) * P.A + a] = act;
-      P.rows_tape[static_cast<size_t>(row) * pi_tape(P.M, P.A, P.Apad, P.B).pitch + pi_tape(P.M, P.A, P.Apad, P.B).act + a] = act;
+      P.rows_tape[static_cast<size_t>(row) * P.tape_pitch + pi_tape(P.M, P.A, P.Apad, P.B).act + a] = act;
     }
   }
   lp = warp_sum(lp);
@@ -870,7 +874,7 @@ __device__ __forceinline__ void rows_head(const PlanParams& P, Ctx& c, const Lay
         y[j] = col < N ? fmaf(row[col], ly.inv_scale, __ldg(ly.bias + col)) : 0.f;
       }
       if (ROWS && ea.tape && c.rowenv[r] >= 0) {      // ROP_PI_LOSS: the head's logits go to the tape
-        float* t = ea.tape + static_cast<size_t>(c.rowenv[r]) * pi_tape(P.M, P.A, P.Apad, P.B).pitch;
+        float* t = ea.tape + static_cast<size_t>(c.rowenv[r]) * P.tape_pitch;
 #pragma unroll
         for (int j = 0; j < kHeadRegCols; ++j)
           if (c.lane + 32 * j < N) t[c.lane + 32 * j] = y[j];
@@ -1218,18 +1222,24 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
         ea.rowmap = rowenv;
         const bool last = P.rop == ROP_ENCODE ? sidx == P.num_enc - 1 : l == 2;
         if (!last) { ea.kind = EPI_LN_MISH; ea.dstbuf = BUF_H1; }
+        // agent._update's forward (rows_tape non-null): every LayerNorm layer tapes its pre-LayerNorm row at the layer's
+        // column offset (encoder: hidden layers enc_dim wide, the SimNorm layer last; MLPs: layers 0 and 1 M wide)
         if (P.rop == ROP_ENCODE) {
           li = P.li_enc + sidx;
           if (last) { ea.kind = EPI_LN_SIMNORM; ea.out_f32 = P.rows_out; ea.out_pitch = P.L; }
+          if (P.rows_tape) ea.tape = P.rows_tape + sidx * LY[P.li_enc].N;
         } else if (P.rop == ROP_NEXT) {
           li = P.li_dyn + l;
           if (last) { ea.kind = EPI_LN_SIMNORM; ea.out_f32 = P.rows_out; ea.out_pitch = P.L; }
+          if (P.rows_tape) ea.tape = P.rows_tape + l * P.M;
         } else if (P.rop == ROP_REWARD) {
           li = P.li_rew + l;
           if (last) { ea.kind = EPI_RAW; ea.out_f32 = P.rows_out; ea.out_pitch = P.B; }
+          else if (P.rows_tape) ea.tape = P.rows_tape + l * P.M;
         } else if (P.rop == ROP_TERM) {
           li = P.li_term + l;
           if (last) { ea.kind = EPI_RAW; ea.out_f32 = P.rows_out; ea.out_pitch = 1; ea.head = P.rows_flag; }
+          else if (P.rows_tape) ea.tape = P.rows_tape + l * P.M;
         } else if (P.rop == ROP_PI || ((P.rop == ROP_TD || P.rop == ROP_PI_LOSS) && sidx < 3)) {
           li = P.li_pi + l;
           if (last) ea.kind = EPI_PI;
@@ -1244,6 +1254,10 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
           li = 3 * h + l;
           if (P.rop == ROP_PI_LOSS) {
             ea.tape = P.rows_tape + pi_tape(P.M, P.A, P.Apad, P.B).q[u] + l * P.M;
+            if (l == 0 && P.rows_drop) ea.drop = P.rows_drop + static_cast<size_t>(h) * P.rows * P.M;
+          }
+          if (P.rop == ROP_Q_ALL && P.rows_tape && !last) {
+            ea.tape = P.rows_tape + (2 * h + l) * P.M;
             if (l == 0 && P.rows_drop) ea.drop = P.rows_drop + static_cast<size_t>(h) * P.rows * P.M;
           }
           if (last && P.rop == ROP_Q_ALL) {

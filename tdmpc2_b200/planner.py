@@ -577,8 +577,10 @@ class Planner:
                     t += [f(pfx + ".ln.weight"), f(pfx + ".ln.bias")]
                 keep.extend(t)
                 lins[i] = _cabi.Linear(*[x.data_ptr() for x in t])
-            _cabi.check(self.lib.tdmpc2_pack_target_q(self.h, lins, self._stream()))
-            torch.cuda.current_stream(self.device).synchronize()   # `keep` tensors may be freed afterwards
+            stream = torch.cuda.current_stream(self.device)
+            _cabi.check(self.lib.tdmpc2_pack_target_q(self.h, lins, stream.cuda_stream))
+            for t in keep:            # `keep` tensors may be freed now: their memory is not reused before the pack ran
+                t.record_stream(stream)
 
     def _rows_out(self, *shape) -> torch.Tensor:
         return torch.empty(*shape, device=self.device, dtype=torch.float32)
@@ -671,6 +673,60 @@ class Planner:
             _cabi.check(self.lib.tdmpc2_pi_loss_backward(self.h, C.byref(W), _ptr(tape), _ptr(z), _ptr(task), _ptr(eps),
                                                          _ptr(qidx), _ptr(drop), T, B, _ptr(scale), float(entropy_coef),
                                                          float(rho), C.byref(G), _ptr(ws), self._stream()))
+
+    def wm_loss_forward(self, obs0, action, task, drop, H, B):
+        """agent._update's taped forward: obs0 [B, obs_dim], action [H B, A], task [H B] | None, drop [num_q, H B, M] | None
+        -> tape, zs [H + 1, B, L], Q logits [num_q, H B, num_bins], reward logits [H B, num_bins], termination logits
+        [H B, 1] (episodic models) or None."""
+        cfg, R = self.cfg, H * B
+        nb = C.c_size_t()
+        _cabi.check(self.lib.tdmpc2_wm_loss_tape_bytes(self.h, H, B, C.byref(nb)))
+        tape = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        zs = self._rows_out(H + 1, B, cfg.latent_dim)
+        ql, rl = self._rows_out(cfg.num_q, R, cfg.num_bins), self._rows_out(R, cfg.num_bins)
+        tl = self._rows_out(R, 1) if cfg.episodic else None
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_wm_loss_forward(self.h, _ptr(obs0), _ptr(action), _ptr(task), _ptr(drop), H, B, _ptr(zs),
+                                                        _ptr(ql), _ptr(rl), _ptr(tl), _ptr(tape), self._stream()))
+        return tape, zs, ql, rl, tl
+
+    def wm_loss_backward(self, tensor, tape, obs0, action, task, drop, H, B, zs, ql, rl, tl, next_z, reward, td_target,
+                         terminated, grads):
+        """Adds dL/dparameter of _update's world-model loss to `grads` (.grad tensors by state-dict key: `_encoder.state.*`,
+        `_dynamics.*`, `_reward.*`, `_termination.*`, `_Qs.params.*`, `_task_emb.weight`).  `tensor(key)` returns the
+        model's fp32 tensor of a state-dict key."""
+        cfg = self.cfg
+
+        def lin(k, ln):
+            return _cabi.Linear(_ptr(tensor(k + ".weight")), _ptr(tensor(k + ".bias")),
+                                _ptr(tensor(k + ".ln.weight")) if ln else None, _ptr(tensor(k + ".ln.bias")) if ln else None)
+
+        def glin(k, ln):
+            return _cabi.LinearGrad(_ptr(grads[k + ".weight"]), _ptr(grads[k + ".bias"]),
+                                    _ptr(grads[k + ".ln.weight"]) if ln else None, _ptr(grads[k + ".ln.bias"]) if ln else None)
+        W, G = _cabi.Weights(), _cabi.WmGrads()
+        n = 0
+        while f"_encoder.state.{n}.weight" in grads:
+            W.enc[n], G.enc[n] = lin(f"_encoder.state.{n}", True), glin(f"_encoder.state.{n}", True)
+            n += 1
+        W.num_enc = G.num_enc = n
+        for i in range(3):
+            W.dynamics[i], G.dynamics[i] = lin(f"_dynamics.{i}", True), glin(f"_dynamics.{i}", True)
+            W.reward[i], G.reward[i] = lin(f"_reward.{i}", i < 2), glin(f"_reward.{i}", i < 2)
+            W.qs[i], G.qs[i] = lin(f"_Qs.params.{i}", i < 2), glin(f"_Qs.params.{i}", i < 2)
+            if cfg.episodic:
+                W.termination[i], G.termination[i] = lin(f"_termination.{i}", i < 2), glin(f"_termination.{i}", i < 2)
+        G.task_emb = _ptr(grads.get("_task_emb.weight"))
+        cf = _cabi.WmLossCoefs(cfg.consistency_coef, cfg.reward_coef, cfg.value_coef, cfg.termination_coef, cfg.rho,
+                               cfg.vmin, cfg.vmax, cfg.bin_size)
+        nb = C.c_size_t()
+        _cabi.check(self.lib.tdmpc2_wm_loss_workspace_bytes(self.h, H, B, C.byref(nb)))
+        ws = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_wm_loss_backward(
+                self.h, C.byref(W), _ptr(tape), _ptr(obs0), _ptr(action), _ptr(task), _ptr(drop), H, B, _ptr(zs), _ptr(ql),
+                _ptr(rl), _ptr(tl), _ptr(next_z), _ptr(reward), _ptr(td_target), _ptr(terminated), C.byref(cf), C.byref(G),
+                _ptr(ws), self._stream()))
 
     def estimate_value(self, z, actions, task, noise_pi, qidx):
         """z [E,N,L], actions [E,H,N,A], noise_pi [E,N,A], qidx [E,2] int32 -> [E,N]."""

@@ -6,8 +6,9 @@ Drop-in for the inference half of the reference class `TDMPC2`
 `._estimate_value()`, `._td_target()` keep their names, argument meaning and return shapes, so
 `evaluate.py:57-80` of the reference runs unchanged on it (INTEGRATION.md), and so does the
 no-grad block of `_update` (`model.encode` + `_td_target`, tdmpc2.py:259-264), and the policy update
-`update_pi` (tdmpc2.py:208-239) with its `scale` (RunningScale) and `pi_optim`.  The world model's losses and
-optimiser are out of scope; call `sync_weights()` after changing the model's parameters (incl. the target Q update).
+`update_pi` (tdmpc2.py:208-239) with its `scale` (RunningScale) and `pi_optim`, and the whole training step
+`update(buffer)` / `_update` (tdmpc2.py:259-346) with its `optim`, for state observations.  Call `sync_weights()` after
+changing the model's parameters outside these methods.
 
 New: an environments axis.  `obs [E, obs_dim]`, `t0 [E]`, `task [E]` plan E
 independent environments in one call; E == 1 (1-D obs) is the reference API.
@@ -19,6 +20,7 @@ import weakref
 from typing import Optional, Sequence, Union
 
 import torch
+import torch.nn.functional as F
 
 from .config import Config, get_discount
 from .planner import Noise, Planner, draw_noise
@@ -55,6 +57,16 @@ class TDMPC2(torch.nn.Module):
         self._pi_keys = [k for k in self.model.keys() if k.startswith("_pi.")]
         self.pi_optim = torch.optim.Adam([self.model.tensor(k) for k in self._pi_keys], lr=cfg.lr, eps=1e-5,
                                          capturable=self.device.type == "cuda")
+        # the world model's optimiser (tdmpc2.py:22-30): the reference's groups, in its order
+        keys = self.model.keys()
+        grp = lambda pfx: [k for k in keys if k.startswith(pfx)]
+        self._wm_groups = [grp("_encoder."), grp("_dynamics."), grp("_reward."), grp("_termination.") if cfg.episodic else [],
+                           grp("_Qs.params."), ["_task_emb.weight"] if cfg.multitask else []]
+        self._wm_keys = [k for g in self._wm_groups for k in g]
+        self.optim = torch.optim.Adam(
+            [{"params": [self.model.tensor(k) for k in self._wm_groups[0]], "lr": cfg.lr * cfg.enc_lr_scale}]
+            + [{"params": [self.model.tensor(k) for k in g]} for g in self._wm_groups[1:]],
+            lr=cfg.lr, capturable=self.device.type == "cuda")
 
     # ------------------------------------------------------------------ planner plumbing
     @property
@@ -264,6 +276,119 @@ class TDMPC2(torch.nn.Module):
                 "pi_scaled_entropy": scaled_entropy, "pi_scale": self.scale.value}
 
     @torch.no_grad()
+    def _renorm_task_emb(self, taskv) -> None:
+        """nn.Embedding(max_norm=1)'s lookup (world_model.py:21): the looked-up rows of `_task_emb.weight` with norm > 1
+        are scaled by 1 / (norm + 1e-7) in place.  Device-side masks: no host synchronisation."""
+        W = self.model.tensor("_task_emb.weight")
+        n = torch.linalg.vector_norm(W, dim=-1, keepdim=True)
+        hit = torch.zeros(W.shape[0], 1, dtype=torch.bool, device=W.device).index_fill_(0, taskv.long(), True)
+        W.mul_(torch.where(hit & (n > 1), 1.0 / (n + 1e-7), torch.ones_like(n)))
+        self.sync_weights()
+
+    def update(self, buffer):
+        """tdmpc2.py:335-346: one training step on `buffer.sample()` = (obs, action, reward, terminated, task)."""
+        obs, action, reward, terminated, task = buffer.sample()
+        kwargs = {}
+        if task is not None:
+            kwargs["task"] = task
+        return self._update(obs, action, reward, terminated, **kwargs)
+
+    def _update(self, obs, action, reward, terminated, task=None, *, td_eps=None, td_qidx=None, dropout_mask=None,
+                pi_eps=None, pi_qidx=None, pi_dropout_mask=None):
+        """tdmpc2.py:259-333 on the kernels, state observations.  obs [H+1, B, obs_dim], action [H, B, A], reward /
+        terminated [H, B, 1], task [B] | None.  The latent rollout and the heads run as taped row launches
+        (tdmpc2_wm_loss_forward), the backward chain of grad_kernels.cuh ADDS the gradients of the world-model loss to
+        `.grad` as autograd would; then torch's clip_grad_norm_ and optim.step(), update_pi on the detached latents, and
+        the Polyak update of the target Q ensemble.
+        Draws from self.generator in the reference's order: the TD target's pi noise and Q pair (`td_eps` [H, B, A],
+        `td_qidx` [2]), the dropout scale of Q layer 0 for the value loss (`dropout_mask` [num_q, H, B, mlp_dim] of
+        mask / (1 - p) values; the reference's vmap dropout stream is not replayed bit for bit), then update_pi's own
+        (`pi_eps`, `pi_qidx`, `pi_dropout_mask`, see update_pi).  Returns the reference's info dict."""
+        cfg, dev = self.cfg, self.device
+        if cfg.get("obs", "state") == "rgb":
+            raise NotImplementedError("_update covers state observations: the conv encoder's backward is not built")
+        if dev.type != "cuda":
+            raise RuntimeError("_update runs on the sm_90a kernels: the agent needs a CUDA device (there is no CPU fallback)")
+        obs_dim, A, L, M = cfg.obs_shape["state"][0], cfg.action_dim, cfg.latent_dim, cfg.mlp_dim
+        if obs.ndim != 3 or obs.shape[0] < 2 or obs.shape[1] < 1 or obs.shape[2] != obs_dim:
+            raise ValueError(f"obs must be [H + 1, B, {obs_dim}]; got {tuple(obs.shape)}")
+        H, B = int(obs.shape[0]) - 1, int(obs.shape[1])
+        for name, x, shape in (("action", action, (H, B, A)), ("reward", reward, (H, B, 1)), ("terminated", terminated, (H, B, 1))):
+            if tuple(x.shape) != shape:
+                raise ValueError(f"{name} must be {list(shape)}; got {tuple(x.shape)}")
+            if not x.is_floating_point():
+                raise ValueError(f"{name} must be a floating-point tensor; got {x.dtype}")
+        if not obs.is_floating_point():
+            raise ValueError(f"obs must be a floating-point tensor; got {obs.dtype}")
+        if cfg.multitask and task is None:
+            raise ValueError("multi-task model needs `task`")
+        drop = None
+        if dropout_mask is not None:
+            drop = torch.as_tensor(dropout_mask, device=dev)
+            if tuple(drop.shape) != (cfg.num_q, H, B, M):
+                raise ValueError(f"dropout_mask must be [{cfg.num_q}, {H}, {B}, {M}]; got {tuple(drop.shape)}")
+        f32 = lambda x: x.detach().to(dev, torch.float32).contiguous()
+        obs, action, reward, terminated = f32(obs), f32(action), f32(reward), f32(terminated)
+        pl, g = self.planner, self.generator
+        taskv = self.model._task_rows(pl, task, (H, B))
+        if cfg.multitask:
+            self._renorm_task_emb(taskv)                       # the first embedding lookup of the step
+
+        # targets (tdmpc2.py:261-264)
+        with torch.no_grad():
+            next_z = self.model.encode(obs[1:], task)
+            td_targets = self.model.td_target(next_z, reward, terminated, task, eps=td_eps, qidx=td_qidx)
+        self.model.train()
+        if drop is None and cfg.dropout > 0:                 # nn.Dropout(cfg.dropout) of Q layer 0 (layers.py:104-108)
+            keep = 1.0 - cfg.dropout
+            drop = torch.empty(cfg.num_q, H * B, M, device=dev).bernoulli_(keep, generator=g).div_(keep)
+        elif drop is not None:
+            drop = drop.to(torch.float32).reshape(cfg.num_q, H * B, M).contiguous()
+
+        # latent rollout and heads (tdmpc2.py:269-285), on the kernels with a tape
+        pl = self.planner
+        act_rows = action.reshape(H * B, A)
+        tape, zs, ql, rl, tl = pl.wm_loss_forward(obs[0], act_rows, taskv, drop, H, B)
+        rho = torch.pow(cfg.rho, torch.arange(H, device=dev, dtype=torch.float32))
+        consistency_loss = (F.mse_loss(zs[1:], next_z, reduction="none").mean(dim=(1, 2)) * rho).sum() / H
+        reward_loss = (_soft_ce(rl.view(H, B, -1), reward, cfg).mean(dim=(1, 2)) * rho).sum() / H
+        value_loss = (_soft_ce(ql.view(cfg.num_q, H, B, -1), td_targets.unsqueeze(0).expand(cfg.num_q, H, B, 1), cfg)
+                      .mean(dim=(2, 3)) * rho).sum() / (H * cfg.num_q)
+        if cfg.episodic:
+            termination_pred = tl.view(H, B, 1)
+            termination_loss = F.binary_cross_entropy_with_logits(termination_pred, terminated)
+        else:
+            termination_loss = 0.
+        total_loss = (cfg.consistency_coef * consistency_loss + cfg.reward_coef * reward_loss
+                      + cfg.termination_coef * termination_loss + cfg.value_coef * value_loss)
+
+        # backward, clip, step (tdmpc2.py:305-309); the embedding's .grad left by the previous update_pi is added to
+        params = [self.model.tensor(k) for k in self._wm_keys]
+        for p in params:
+            if p.grad is None:
+                p.grad = torch.zeros_like(p)
+        pl.wm_loss_backward(self.model.tensor, tape, obs[0], act_rows, taskv, drop, H, B, zs, ql, rl, tl, next_z, reward,
+                            td_targets, terminated, {k: p.grad for k, p in zip(self._wm_keys, params)})
+        grad_norm = torch.nn.utils.clip_grad_norm_([p for p in self.model.parameters() if p.grad is not None],
+                                                   cfg.grad_clip_norm)
+        self.optim.step()
+        self.optim.zero_grad(set_to_none=True)
+        self.sync_weights()                                     # update_pi reads the stepped Q weights
+
+        # policy update, target Q (tdmpc2.py:312-315)
+        if cfg.multitask:
+            self._renorm_task_emb(taskv)                       # update_pi's embedding lookup after the step
+        pi_info = self.update_pi(zs.detach(), task, eps=pi_eps, qidx=pi_qidx, dropout_mask=pi_dropout_mask)
+        self.model.soft_update_target_Q()
+        self.model.eval()
+        info = {"consistency_loss": consistency_loss, "reward_loss": reward_loss, "value_loss": value_loss,
+                "termination_loss": termination_loss, "total_loss": total_loss, "grad_norm": grad_norm}
+        if cfg.episodic:
+            info.update(_termination_statistics(torch.sigmoid(termination_pred[-1]), terminated[-1]))
+        info.update(pi_info)
+        return {k: v.detach().mean() if isinstance(v, torch.Tensor) else torch.tensor(v) for k, v in info.items()}
+
+    @torch.no_grad()
     def _td_target(self, next_z, reward, terminated, task, *, eps=None, qidx=None):
         """tdmpc2.py:242-257 as one fused launch: next_z [..., L], reward / terminated [..., 1] ->
         reward + discount * (1 - terminated) * Q(next_z, pi(next_z), 'min', target=True)  [..., 1].
@@ -289,3 +414,31 @@ class TDMPC2(torch.nn.Module):
         v = self.planner.estimate_value(zb, ab, taskv, eps_pi.reshape(E, cfg.num_samples, cfg.action_dim).contiguous(),
                                         qidx.reshape(E, 2).to(torch.int32).contiguous())
         return v[0].unsqueeze(-1) if single else v.unsqueeze(-1)
+
+
+def _two_hot(x, cfg):
+    """math.py:58-71 on x [..., 1] -> [..., num_bins]."""
+    x = torch.clamp(torch.sign(x) * torch.log(1 + torch.abs(x)), cfg.vmin, cfg.vmax).squeeze(-1)
+    idx = torch.floor((x - cfg.vmin) / cfg.bin_size)
+    off = ((x - cfg.vmin) / cfg.bin_size - idx).unsqueeze(-1)
+    out = torch.zeros(*x.shape, cfg.num_bins, device=x.device, dtype=x.dtype)
+    idx = idx.long().unsqueeze(-1)
+    out = out.scatter(-1, idx, 1 - off)
+    return out.scatter(-1, (idx + 1) % cfg.num_bins, off)
+
+
+def _soft_ce(pred, target, cfg):
+    """math.py:5-9: -(two_hot(target) . log_softmax(pred)) [..., 1]."""
+    return -(_two_hot(target, cfg) * F.log_softmax(pred, dim=-1)).sum(-1, keepdim=True)
+
+
+def _termination_statistics(pred, target, eps=1e-9):
+    """math.py:97-109."""
+    pred, target = pred.squeeze(-1), target.squeeze(-1)
+    rate = target.sum() / len(target)
+    tp = ((pred > 0.5) & (target == 1)).sum()
+    fn = ((pred <= 0.5) & (target == 1)).sum()
+    fp = ((pred > 0.5) & (target == 0)).sum()
+    recall = tp / (tp + fn + eps)
+    precision = tp / (tp + fp + eps)
+    return {"termination_rate": rate, "termination_f1": 2 * (precision * recall) / (precision + recall + eps)}

@@ -135,6 +135,15 @@ class WorldModel(nn.Module):
         the kernels' packed copies are re-packed before the next call that reads them."""
         self._version += 1
 
+    @torch.no_grad()
+    def soft_update_target_Q(self) -> None:
+        """world_model.py:82-86: Polyak-average `_target_Qs_params.*` towards the online `_Qs.params.*` by cfg.tau, in
+        place, then mark the packed copies stale."""
+        for k in self._keys:
+            if k.startswith("_target_Qs_params."):
+                self.tensor(k).lerp_(self.tensor("_Qs.params." + k[len("_target_Qs_params."):]), self.cfg.tau)
+        self.sync_weights()
+
     def _kernels(self) -> Planner:
         """The Planner whose packed weights these methods run on: the owning agent's, or a one-environment planner of
         this model's own (created on first use; CUDA only -- there is no CPU fallback)."""
