@@ -42,7 +42,9 @@ extern "C" {
                                        7: world-model methods on a flat batch (tdmpc2_wm_*, tdmpc2_td_target), target Q blob;
                                           later, additive: tdmpc2_pixel_encode_rows (old callers and bindings unaffected);
                                           later, additive: agent.update_pi (tdmpc2_pi_loss_*, tdmpc2_pi_grads),
-                                          agent._update (tdmpc2_wm_loss_*, tdmpc2_wm_grads) */
+                                          agent._update (tdmpc2_wm_loss_*, tdmpc2_wm_grads);
+                                          later, additive: agent._update of pixel models (tdmpc2_pixel_encode_taped,
+                                          tdmpc2_pixel_encode_backward, tdmpc2_conv_grads, tdmpc2_wm_loss_*_latent) */
 #define TDMPC2_MAX_ENC_LAYERS 8
 
 typedef enum tdmpc2_status {
@@ -212,6 +214,23 @@ int tdmpc2_pixel_encode(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_c
  * frame and shift.  rows < 1 or a null pointer: TDMPC2_ERR_INVALID. */
 int tdmpc2_pixel_encode_rows(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
                              const float* shift, const float* grid_base, int64_t rows, float* z_out, void* stream);
+/* Training (agent._update of pixel models, tdmpc2.py:266-309).  tdmpc2_pixel_encode_taped is tdmpc2_pixel_encode_rows that
+ * also writes each frame's post-ReLU maps to `tape` ([rows] slots of tape_bytes / rows; z is bit-identical to the untaped
+ * launch).  tdmpc2_pixel_encode_backward ADDS dL/dparameter of the four Conv2d layers to `grads`, like autograd
+ * accumulates .grad, given dz = dL/dz [rows, 16 * num_channels], the forward's z and tape and its frames and shifts
+ * (conv1's input is recomputed).  fp32 FFMA; reductions over frames in a fixed order (repeated calls give identical bits);
+ * no allocation, no host synchronisation.  workspace: tdmpc2_pixel_backward_workspace_bytes(rows). */
+typedef struct tdmpc2_conv_grads {   /* .grad of _encoder.rgb.{2,4,6,8}.{weight,bias} */
+  float* weight[4];
+  float* bias[4];
+} tdmpc2_conv_grads;
+int tdmpc2_pixel_encode_tape_bytes(const tdmpc2_pixel_encoder* e, int64_t rows, size_t* out);
+int tdmpc2_pixel_encode_taped(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
+                              const float* shift, const float* grid_base, int64_t rows, float* z_out, float* tape, void* stream);
+int tdmpc2_pixel_backward_workspace_bytes(const tdmpc2_pixel_encoder* e, int64_t rows, size_t* out);
+int tdmpc2_pixel_encode_backward(tdmpc2_pixel_encoder* e, const tdmpc2_conv_weights* w, const float* frames,
+                                 const float* shift, const float* grid_base, int64_t rows, const float* tape, const float* z,
+                                 const float* dz, const tdmpc2_conv_grads* grads, void* workspace, void* stream);
 
 /* Replaces ONE pass of the loop tdmpc2.py:173-197 (sample, _estimate_value
  * :122-136, topk, MPPI weights, refit) for all E environments.
@@ -363,6 +382,20 @@ int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const fl
                             const float* zs, const float* q_logits, const float* reward_logits, const float* term_logits,
                             const float* next_z, const float* reward, const float* td_target, const float* terminated,
                             const tdmpc2_wm_loss_coefs* coefs, const tdmpc2_wm_grads* grads, void* workspace, void* stream);
+/* Planners without a state encoder (pixel models, num_enc_layers = 0) get TDMPC2_ERR_UNSUPPORTED from the two calls above;
+ * they use these.  _latent forward: zs[0] ([B, L]) is the caller's, written by tdmpc2_pixel_encode_taped; the rest as
+ * tdmpc2_wm_loss_forward.  _latent backward: as tdmpc2_wm_loss_backward without the state encoder (grads->enc and
+ * w->enc are not read), and dL/dz_0 [B, L] is written to dz0, for tdmpc2_pixel_encode_backward.  tape_bytes and
+ * workspace_bytes answer for both variants. */
+int tdmpc2_wm_loss_forward_latent(tdmpc2_planner* p, const float* action, const int32_t* task, const float* dropout_mask,
+                                  int H, int B, float* zs, float* q_logits, float* reward_logits, float* term_logits,
+                                  float* tape, void* stream);
+int tdmpc2_wm_loss_backward_latent(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* action,
+                                   const int32_t* task, const float* dropout_mask, int H, int B, const float* zs,
+                                   const float* q_logits, const float* reward_logits, const float* term_logits,
+                                   const float* next_z, const float* reward, const float* td_target, const float* terminated,
+                                   const tdmpc2_wm_loss_coefs* coefs, const tdmpc2_wm_grads* grads, float* dz0,
+                                   void* workspace, void* stream);
 
 /* Diagnostics: y[rows, out] = act(LN(x W^T + b)) for ONE packed layer, through
  * the same fused kernels (rows <= 128).  layer index: 0.. = enc, then dynamics

@@ -26,7 +26,9 @@ SYMBOLS = [
     "tdmpc2_wm_encode", "tdmpc2_wm_next", "tdmpc2_wm_reward", "tdmpc2_wm_termination", "tdmpc2_wm_pi", "tdmpc2_wm_q",
     "tdmpc2_td_target", "tdmpc2_pi_loss_tape_bytes", "tdmpc2_pi_loss_workspace_bytes", "tdmpc2_pi_loss_forward",
     "tdmpc2_pi_loss_backward", "tdmpc2_wm_loss_tape_bytes", "tdmpc2_wm_loss_workspace_bytes", "tdmpc2_wm_loss_forward",
-    "tdmpc2_wm_loss_backward",
+    "tdmpc2_wm_loss_backward", "tdmpc2_pixel_encode_tape_bytes", "tdmpc2_pixel_encode_taped",
+    "tdmpc2_pixel_backward_workspace_bytes", "tdmpc2_pixel_encode_backward", "tdmpc2_wm_loss_forward_latent",
+    "tdmpc2_wm_loss_backward_latent",
 ]
 
 
@@ -54,6 +56,10 @@ class PixelDims(C.Structure):
 
 
 class ConvWeights(C.Structure):
+    _fields_ = [("weight", C.c_void_p * 4), ("bias", C.c_void_p * 4)]
+
+
+class ConvGrads(C.Structure):       # tdmpc2_conv_grads: .grad of _encoder.rgb.{2,4,6,8}.{weight,bias}
     _fields_ = [("weight", C.c_void_p * 4), ("bias", C.c_void_p * 4)]
 
 
@@ -152,6 +158,14 @@ def load():
     lib.tdmpc2_wm_loss_forward.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
     lib.tdmpc2_wm_loss_backward.argtypes = [vp, C.POINTER(Weights), vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp,
                                             vp, vp, C.POINTER(WmLossCoefs), C.POINTER(WmGrads), vp, vp]
+    lib.tdmpc2_pixel_encode_tape_bytes.argtypes = [vp, i64, C.POINTER(C.c_size_t)]
+    lib.tdmpc2_pixel_encode_taped.argtypes = [vp, vp, C.POINTER(ConvWeights), vp, vp, vp, i64, vp, vp, vp]
+    lib.tdmpc2_pixel_backward_workspace_bytes.argtypes = [vp, i64, C.POINTER(C.c_size_t)]
+    lib.tdmpc2_pixel_encode_backward.argtypes = [vp, C.POINTER(ConvWeights), vp, vp, vp, i64, vp, vp, vp, C.POINTER(ConvGrads),
+                                                 vp, vp]
+    lib.tdmpc2_wm_loss_forward_latent.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
+    lib.tdmpc2_wm_loss_backward_latent.argtypes = [vp, C.POINTER(Weights), vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp,
+                                                   vp, vp, vp, C.POINTER(WmLossCoefs), C.POINTER(WmGrads), vp, vp, vp]
     for s in SYMBOLS:
         f = getattr(lib, s)
         if f.restype is C.c_int and s not in ("tdmpc2_abi_version", "tdmpc2_planner_layer_count"):

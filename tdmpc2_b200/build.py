@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libtdmpc2_b200.so")
 STAMP = LIB + ".stamp"
-SOURCES = ["api.cu", "plan_kernels.cuh", "grad_kernels.cuh", "pixel_encoder.cuh", "ptx.cuh", "rng.cuh",
+SOURCES = ["api.cu", "plan_kernels.cuh", "grad_kernels.cuh", "pixel_encoder.cuh", "pixel_grad_kernels.cuh", "ptx.cuh", "rng.cuh",
            os.path.join("..", "..", "include", "tdmpc2_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]

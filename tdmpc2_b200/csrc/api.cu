@@ -18,6 +18,7 @@
 #include "plan_kernels.cuh"
 #include "grad_kernels.cuh"
 #include "pixel_encoder.cuh"
+#include "pixel_grad_kernels.cuh"
 
 using namespace tdmpc2;
 
@@ -45,6 +46,8 @@ static unsigned env_uint(const char* name, unsigned dflt) {
 }
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+// a workspace / tape segment of n floats at `off`, the next one starting on a 64-float boundary
+static size_t take64(size_t& off, size_t n) { const size_t o = off; off += (n + 63) / 64 * 64; return o; }
 static inline int pad_to(int x, int a) { return (x + a - 1) / a * a; }
 
 // ------------------------------------------------------------------------------------ pack kernels
@@ -727,13 +730,14 @@ extern "C" int tdmpc2_pixel_encoder_workspace_bytes(const tdmpc2_pixel_encoder* 
 }
 
 // One launch over `rows` frames: min(rows, SMs) CTAs, each looping over its frames with its own conv1 scratch slot.
+// tape != nullptr: the frames' post-ReLU maps are written to it as well (conv1 straight into the frame's slot).
 static int pixel_launch(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
-                        const float* shift, const float* grid_base, int64_t rows, float* z_out, void* stream_) {
+                        const float* shift, const float* grid_base, int64_t rows, float* z_out, float* tape, void* stream_) {
   if (!workspace || !w || !frames || !shift || !grid_base || !z_out) return fail(TDMPC2_ERR_INVALID, "null argument");
   if (rows < 1) return fail(TDMPC2_ERR_INVALID, "rows must be >= 1");
   for (int i = 0; i < 4; ++i) if (!w->weight[i] || !w->bias[i]) return fail(TDMPC2_ERR_INVALID, "pixel encoder: null conv weight");
   PixelParams P{};
-  P.frames = frames; P.shift = shift; P.grid = grid_base; P.scratch = static_cast<float*>(workspace); P.z = z_out;
+  P.frames = frames; P.shift = shift; P.grid = grid_base; P.scratch = static_cast<float*>(workspace); P.z = z_out; P.tape = tape;
   for (int i = 0; i < 4; ++i) { P.w[i] = w->weight[i]; P.b[i] = w->bias[i]; }
   P.rows = rows; P.C = e->d.in_channels; P.nc = e->d.num_channels; P.simnorm = e->d.simnorm_dim;
   P.smem_floats = static_cast<int>(e->smem / 4);
@@ -750,7 +754,7 @@ static int pixel_launch(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_c
 extern "C" int tdmpc2_pixel_encode(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
                                    const float* shift, const float* grid_base, float* z_out, void* stream_) {
   if (!e) return fail(TDMPC2_ERR_INVALID, "null argument");
-  return pixel_launch(e, workspace, w, frames, shift, grid_base, e->d.num_envs, z_out, stream_);
+  return pixel_launch(e, workspace, w, frames, shift, grid_base, e->d.num_envs, z_out, nullptr, stream_);
 }
 
 extern "C" int tdmpc2_pixel_encode_rows(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w,
@@ -761,7 +765,99 @@ extern "C" int tdmpc2_pixel_encode_rows(tdmpc2_pixel_encoder* e, void* workspace
     const int rc = check_device(&n);
     return rc ? rc : fail(TDMPC2_ERR_INVALID, "null pixel encoder");
   }
-  return pixel_launch(e, workspace, w, frames, shift, grid_base, rows, z_out, stream_);
+  return pixel_launch(e, workspace, w, frames, shift, grid_base, rows, z_out, nullptr, stream_);
+}
+
+// ---- the conv encoder's backward (pixel_grad_kernels.cuh): taped forward, then the chain from dL/dz to the conv grads
+extern "C" int tdmpc2_pixel_encode_tape_bytes(const tdmpc2_pixel_encoder* e, int64_t rows, size_t* out) {
+  if (!e || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (rows < 1) return fail(TDMPC2_ERR_INVALID, "rows must be >= 1");
+  *out = static_cast<size_t>(rows) * pix_tape_floats(e->d.num_channels) * 4;
+  return 0;
+}
+
+extern "C" int tdmpc2_pixel_encode_taped(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w,
+                                         const float* frames, const float* shift, const float* grid_base, int64_t rows,
+                                         float* z_out, float* tape, void* stream_) {
+  if (!e || !tape) return fail(TDMPC2_ERR_INVALID, "null argument");
+  return pixel_launch(e, workspace, w, frames, shift, grid_base, rows, z_out, tape, stream_);
+}
+
+// Workspace of the backward (floats): the data gradients dp4 [rows][16 nc], dp3 [rows][nc 36], dp2 [rows][nc 169],
+// dp1 [rows][nc 841], conv1's recomputed input [rows][C 4096], and the weight-gradient partials of the largest layer.
+struct PixGradWs {
+  size_t dp4, dp3, dp2, dp1, img, part, floats;
+};
+static PixGradWs pix_grad_ws(const tdmpc2_pixel_dims& d, int64_t rows) {
+  const size_t R = static_cast<size_t>(rows), nc = d.num_channels, C = d.in_channels;
+  PixGradWs w;
+  size_t off = 0;
+  w.dp4 = take64(off, R * nc * kPixO4 * kPixO4);
+  w.dp3 = take64(off, R * nc * kPixO3 * kPixO3);
+  w.dp2 = take64(off, R * nc * kPixO2 * kPixO2);
+  w.dp1 = take64(off, R * nc * kPixO1 * kPixO1);
+  w.img = take64(off, R * pix_stage_floats(d.in_channels));
+  const int IC[4] = {static_cast<int>(C), static_cast<int>(nc), static_cast<int>(nc), static_cast<int>(nc)};
+  const int KK[4] = {49, 25, 9, 9};
+  size_t part = 0;
+  for (int l = 0; l < 4; ++l)
+    part = std::max(part, static_cast<size_t>(pixg_nsplit(IC[l], d.num_channels, KK[l], rows)) * nc * pixg_cols(IC[l], KK[l]));
+  w.part = take64(off, part);
+  w.floats = off;
+  return w;
+}
+
+extern "C" int tdmpc2_pixel_backward_workspace_bytes(const tdmpc2_pixel_encoder* e, int64_t rows, size_t* out) {
+  if (!e || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (rows < 1) return fail(TDMPC2_ERR_INVALID, "rows must be >= 1");
+  *out = pix_grad_ws(e->d, rows).floats * 4;
+  return 0;
+}
+
+extern "C" int tdmpc2_pixel_encode_backward(tdmpc2_pixel_encoder* e, const tdmpc2_conv_weights* w, const float* frames,
+                                            const float* shift, const float* grid_base, int64_t rows, const float* tape,
+                                            const float* z, const float* dz, const tdmpc2_conv_grads* grads, void* workspace,
+                                            void* stream_) {
+  if (!e || !w || !frames || !shift || !grid_base || !tape || !z || !dz || !grads || !workspace)
+    return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (rows < 1) return fail(TDMPC2_ERR_INVALID, "rows must be >= 1");
+  for (int i = 0; i < 4; ++i)
+    if (!w->weight[i] || !w->bias[i] || !grads->weight[i] || !grads->bias[i])
+      return fail(TDMPC2_ERR_INVALID, "pixel encoder: null conv weight or gradient");
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  const int C = e->d.in_channels, nc = e->d.num_channels, L = nc * kPixO4 * kPixO4;
+  const int64_t tp = pix_tape_floats(nc);
+  const PixGradWs W = pix_grad_ws(e->d, rows);
+  float* ws = static_cast<float*>(workspace);
+  float *dp4 = ws + W.dp4, *dp3 = ws + W.dp3, *dp2 = ws + W.dp2, *dp1 = ws + W.dp1, *img = ws + W.img, *part = ws + W.part;
+  auto blocks = [](int64_t n) { return static_cast<int>(std::min<int64_t>((n + kPgThreads - 1) / kPgThreads, 1 << 20)); };
+  // the weight and bias gradients of layer l from its output gradient dy and its input x (frame pitch xp)
+  auto dw = [&](int l, auto kern, int KK, const float* dy, int OH, const float* x, int64_t xp, int IC, int IH) -> int {
+    const int ns = pixg_nsplit(IC, nc, KK, rows), cols = pixg_cols(IC, KK);
+    kern<<<dim3(pixg_ctas_x(IC, nc, KK), ns), kPgThreads, 0, st>>>(dy, nc, OH, OH, x, xp, IC, IH, IH, rows, ns, part);
+    CUDA_TRY(cudaGetLastError());
+    pixg_reduce<<<blocks(static_cast<int64_t>(nc) * cols), kPgThreads, 0, st>>>(part, ns, nc, cols, grads->weight[l], grads->bias[l]);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+  };
+  int rc;
+  pixg_simnorm_back<<<blocks(rows * (L / e->d.simnorm_dim)), kPgThreads, 0, st>>>(z, dz, rows, L, e->d.simnorm_dim, dp4);
+  CUDA_TRY(cudaGetLastError());
+  if ((rc = dw(3, pixg_dw<3, 1>, 9, dp4, kPixO4, tape + pix_tape_a3(nc), tp, nc, kPixO3))) return rc;
+  pixg_dx<3, 1><<<blocks(rows * nc * kPixO3 * kPixO3), kPgThreads, 0, st>>>(dp4, nc, kPixO4, kPixO4, w->weight[3], tape + pix_tape_a3(nc),
+                                                                            tp, nc, kPixO3, kPixO3, rows, dp3);
+  CUDA_TRY(cudaGetLastError());
+  if ((rc = dw(2, pixg_dw<3, 2>, 9, dp3, kPixO3, tape + pix_tape_a2(nc), tp, nc, kPixO2))) return rc;
+  pixg_dx<3, 2><<<blocks(rows * nc * kPixO2 * kPixO2), kPgThreads, 0, st>>>(dp3, nc, kPixO3, kPixO3, w->weight[2], tape + pix_tape_a2(nc),
+                                                                            tp, nc, kPixO2, kPixO2, rows, dp2);
+  CUDA_TRY(cudaGetLastError());
+  if ((rc = dw(1, pixg_dw<5, 2>, 25, dp2, kPixO2, tape, tp, nc, kPixO1))) return rc;
+  pixg_dx<5, 2><<<blocks(rows * nc * kPixO1 * kPixO1), kPgThreads, 0, st>>>(dp2, nc, kPixO2, kPixO2, w->weight[1], tape, tp, nc, kPixO1,
+                                                                            kPixO1, rows, dp1);
+  CUDA_TRY(cudaGetLastError());
+  pixg_stage<<<blocks(rows * pix_stage_floats(C)), kPgThreads, 0, st>>>(frames, shift, grid_base, rows, C, img);
+  CUDA_TRY(cudaGetLastError());
+  return dw(0, pixg_dw<7, 2>, 49, dp1, kPixO1, img, pix_stage_floats(C), C, kPixHW);
 }
 
 extern "C" int tdmpc2_plan_iter(tdmpc2_planner* p, const float* noise_r, const float* noise_pi, const int32_t* qidx,
@@ -1193,19 +1289,18 @@ extern "C" int tdmpc2_pi_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* 
 
 // ------------------------------------------------------------------------------------ agent._update (row-op tapes + grad_kernels.cuh)
 // The forward's tape (floats): one segment per row op, each [rows, pitch] of the pre-LayerNorm rows of its LayerNorm
-// layers in layer order -- encoder [B, (n_enc - 1) enc_dim + L]; dynamics [H B, 2 M + L] (step t's rows at t B);
+// layers in layer order -- encoder [B, (n_enc - 1) enc_dim + L] (empty without a state encoder); dynamics [H B, 2 M + L] (step t's rows at t B);
 // reward [H B, 2 M]; Q 'all' [H B, 2 M num_q] (head h's layers 0, 1 at (2 h + l) M, layer 0 after dropout);
 // termination [H B, 2 M] (episodic).
 struct WmTape {
   int p_enc, p_dyn, p_rew, p_q, p_term;
   size_t enc, dyn, rew, q, term, floats;
 };
-static size_t take64(size_t& off, size_t n) { const size_t o = off; off += (n + 63) / 64 * 64; return o; }
 static WmTape wm_tape(const tdmpc2_planner* p, int H, int B) {
   const tdmpc2_dims& d = p->d;
   const size_t R = static_cast<size_t>(H) * B;
   WmTape t;
-  t.p_enc = (p->num_enc - 1) * d.enc_dim + d.latent_dim;
+  t.p_enc = p->num_enc > 0 ? (p->num_enc - 1) * d.enc_dim + d.latent_dim : 0;
   t.p_dyn = 2 * d.mlp_dim + d.latent_dim; t.p_rew = 2 * d.mlp_dim; t.p_q = 2 * d.mlp_dim * d.num_q; t.p_term = 2 * d.mlp_dim;
   size_t off = 0;
   t.enc = take64(off, static_cast<size_t>(B) * t.p_enc);
@@ -1226,7 +1321,10 @@ struct WmWs {
 static WmWs wm_ws(const tdmpc2_planner* p, int H, int B) {
   const tdmpc2_dims& d = p->d;
   const size_t R = static_cast<size_t>(H) * B, M = d.mlp_dim, L = d.latent_dim, T = d.task_dim, nb = d.num_bins, nq = d.num_q;
-  const size_t LT = L + T, D = L + T + d.action_dim, E = d.enc_dim, EL = std::max(E, L), OT = d.obs_dim + T;
+  const size_t LT = L + T, D = L + T + d.action_dim;
+  // the encoder's segments are empty without a state encoder (pixel models: the conv encoder has its own workspace)
+  const bool enc = p->num_enc > 0;
+  const size_t E = enc ? d.enc_dim : 0, EL = enc ? std::max(E, L) : 0, OT = enc ? d.obs_dim + T : 0, BE = enc ? B : 0;
   WmWs w;
   w.nsplit = std::max(1, std::min(8, static_cast<int>(R / 256)));
   size_t off = 0;
@@ -1239,7 +1337,7 @@ static WmWs wm_ws(const tdmpc2_planner* p, int H, int B) {
   w.dp1 = take64(off, R * M); w.dyn1 = take64(off, R * M); w.dy1 = take64(off, R * M); w.h1 = take64(off, R * M);
   w.dp0 = take64(off, R * M); w.dyn0 = take64(off, R * M); w.dy0 = take64(off, R * M); w.h0 = take64(off, R * M);
   w.ea = take64(off, B * EL); w.eb = take64(off, B * EL); w.edyn = take64(off, B * EL); w.edy = take64(off, B * EL);
-  w.eh = take64(off, B * EL); w.ex = take64(off, B * OT); w.exe = take64(off, B * LT);
+  w.eh = take64(off, B * EL); w.ex = take64(off, B * OT); w.exe = take64(off, BE * LT);
   w.zero = take64(off, R * LT);
   w.part = take64(off, static_cast<size_t>(w.nsplit) * std::max({M, L, E, nb}) * std::max({M, D, E, OT}));
   w.iota = take64(off, nq);
@@ -1250,7 +1348,12 @@ static WmWs wm_ws(const tdmpc2_planner* p, int H, int B) {
 static int wm_dims_ok(const tdmpc2_planner* p, int H, int B) {
   if (H < 1 || B < 1) return fail(TDMPC2_ERR_INVALID, "H and B must be >= 1");
   if (static_cast<long long>(H + 1) * B > 0x7fffffff) return fail(TDMPC2_ERR_INVALID, "H * B too large");
-  if (p->num_enc == 0) return fail(TDMPC2_ERR_UNSUPPORTED, "the world-model loss needs a state encoder (the conv encoder's backward is not built)");
+  return 0;
+}
+static int wm_needs_encoder(const tdmpc2_planner* p) {
+  if (p->num_enc == 0)
+    return fail(TDMPC2_ERR_UNSUPPORTED, "this planner has no state encoder (pixel model): use tdmpc2_wm_loss_forward_latent / "
+                                        "tdmpc2_wm_loss_backward_latent with tdmpc2_pixel_encode_taped / tdmpc2_pixel_encode_backward");
   return 0;
 }
 
@@ -1270,20 +1373,24 @@ extern "C" int tdmpc2_wm_loss_workspace_bytes(const tdmpc2_planner* p, int H, in
   return 0;
 }
 
-extern "C" int tdmpc2_wm_loss_forward(tdmpc2_planner* p, const float* obs0, const float* action, const int32_t* task,
-                                      const float* dropout_mask, int H, int B, float* zs, float* q_logits, float* reward_logits,
-                                      float* term_logits, float* tape, void* stream_) {
+// latent: zs[0] is the caller's (the pixel encoder wrote it), and the ENCODE launch is skipped
+static int wm_forward_impl(tdmpc2_planner* p, bool latent, const float* obs0, const float* action, const int32_t* task,
+                           const float* dropout_mask, int H, int B, float* zs, float* q_logits, float* reward_logits,
+                           float* term_logits, float* tape, void* stream_) {
   int rc = rows_ready(p, B);
-  if (rc || (rc = wm_dims_ok(p, H, B)) || (rc = need_task(p, task))) return rc;
-  if (!obs0 || !action || !zs || !q_logits || !reward_logits || !tape) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (rc || (rc = wm_dims_ok(p, H, B)) || (!latent && (rc = wm_needs_encoder(p))) || (rc = need_task(p, task))) return rc;
+  if ((!latent && !obs0) || !action || !zs || !q_logits || !reward_logits || !tape) return fail(TDMPC2_ERR_INVALID, "null argument");
   if (p->d.episodic && !term_logits) return fail(TDMPC2_ERR_INVALID, "episodic model needs term_logits");
   const tdmpc2_dims& d = p->d;
   const int R = H * B;
   const size_t L = d.latent_dim, A = d.action_dim;
   const WmTape tp = wm_tape(p, H, B);
-  PlanParams prm = rows_params(p, ROP_ENCODE, B, task);
-  prm.rows_in = obs0; prm.rows_out = zs; prm.rows_tape = tape + tp.enc; prm.tape_pitch = tp.p_enc;
-  if ((rc = launch(p, prm, stream_))) return rc;
+  PlanParams prm;
+  if (!latent) {
+    prm = rows_params(p, ROP_ENCODE, B, task);
+    prm.rows_in = obs0; prm.rows_out = zs; prm.rows_tape = tape + tp.enc; prm.tape_pitch = tp.p_enc;
+    if ((rc = launch(p, prm, stream_))) return rc;
+  }
   for (int t = 0; t < H; ++t) {
     const size_t r0 = static_cast<size_t>(t) * B;
     prm = rows_params(p, ROP_NEXT, B, task ? task + r0 : nullptr);
@@ -1307,23 +1414,38 @@ extern "C" int tdmpc2_wm_loss_forward(tdmpc2_planner* p, const float* obs0, cons
   return 0;
 }
 
+extern "C" int tdmpc2_wm_loss_forward(tdmpc2_planner* p, const float* obs0, const float* action, const int32_t* task,
+                                      const float* dropout_mask, int H, int B, float* zs, float* q_logits, float* reward_logits,
+                                      float* term_logits, float* tape, void* stream_) {
+  return wm_forward_impl(p, false, obs0, action, task, dropout_mask, H, B, zs, q_logits, reward_logits, term_logits, tape, stream_);
+}
+
+extern "C" int tdmpc2_wm_loss_forward_latent(tdmpc2_planner* p, const float* action, const int32_t* task,
+                                             const float* dropout_mask, int H, int B, float* zs, float* q_logits,
+                                             float* reward_logits, float* term_logits, float* tape, void* stream_) {
+  return wm_forward_impl(p, true, nullptr, action, task, dropout_mask, H, B, zs, q_logits, reward_logits, term_logits, tape, stream_);
+}
+
 static bool lin_ok(const tdmpc2_linear& l, bool ln) { return l.weight && l.bias && (!ln || (l.ln_weight && l.ln_bias)); }
 static bool grad_ok(const tdmpc2_linear_grad& g, bool ln) { return g.weight && g.bias && (!ln || (g.ln_weight && g.ln_bias)); }
 
-extern "C" int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* obs0,
-                                       const float* action, const int32_t* task, const float* dropout_mask, int H, int B,
-                                       const float* zs, const float* q_logits, const float* reward_logits, const float* term_logits,
-                                       const float* next_z, const float* reward, const float* td_target, const float* terminated,
-                                       const tdmpc2_wm_loss_coefs* cf, const tdmpc2_wm_grads* gr, void* workspace, void* stream_) {
+// dz0 != nullptr (latent): step 4 (the state encoder) is skipped and dL/dz_0 [B, L] is copied to dz0 instead
+static int wm_backward_impl(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* obs0,
+                            const float* action, const int32_t* task, const float* dropout_mask, int H, int B,
+                            const float* zs, const float* q_logits, const float* reward_logits, const float* term_logits,
+                            const float* next_z, const float* reward, const float* td_target, const float* terminated,
+                            const tdmpc2_wm_loss_coefs* cf, const tdmpc2_wm_grads* gr, float* dz0, void* workspace, void* stream_) {
+  const bool latent = dz0 != nullptr;
   int rc = rows_ready(p, B);
-  if (rc || (rc = wm_dims_ok(p, H, B)) || (rc = need_task(p, task))) return rc;
+  if (rc || (rc = wm_dims_ok(p, H, B)) || (!latent && (rc = wm_needs_encoder(p))) || (rc = need_task(p, task))) return rc;
   const tdmpc2_dims& d = p->d;
-  if (!w || !tape || !obs0 || !action || !zs || !q_logits || !reward_logits || !next_z || !reward || !td_target || !cf || !gr ||
+  if (!w || !tape || (!latent && !obs0) || !action || !zs || !q_logits || !reward_logits || !next_z || !reward || !td_target || !cf || !gr ||
       !workspace)
     return fail(TDMPC2_ERR_INVALID, "null argument");
   if (d.episodic && (!term_logits || !terminated)) return fail(TDMPC2_ERR_INVALID, "episodic model needs term_logits and terminated");
-  if (w->num_enc != p->num_enc || gr->num_enc != p->num_enc) return fail(TDMPC2_ERR_INVALID, "num_enc differs from the planner's");
-  for (int i = 0; i < p->num_enc; ++i)
+  if (!latent && (w->num_enc != p->num_enc || gr->num_enc != p->num_enc))
+    return fail(TDMPC2_ERR_INVALID, "num_enc differs from the planner's");
+  for (int i = 0; !latent && i < p->num_enc; ++i)
     if (!lin_ok(w->enc[i], true) || !grad_ok(gr->enc[i], true)) return fail(TDMPC2_ERR_INVALID, "null encoder tensor or gradient");
   for (int i = 0; i < 3; ++i) {
     if (!lin_ok(w->dynamics[i], true) || !lin_ok(w->reward[i], i < 2) || !lin_ok(w->qs[i], i < 2) || !grad_ok(gr->dynamics[i], true) ||
@@ -1474,8 +1596,9 @@ extern "C" int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* 
       (rc = colsum(ws + W.dyn0, R, M, M, gd[0].ln_weight)) || (rc = colsum(ws + W.dy0, R, M, M, gd[0].ln_bias)))
     return rc;
 
+  if (latent) CUDA_TRY(cudaMemcpyAsync(dz0, ws + W.dz, static_cast<size_t>(B) * Lz * 4, cudaMemcpyDeviceToDevice, st));
   // ---- 4. dz_0 through the encoder: the SimNorm layer, then the Mish layers down to layer 0 (input [obs | emb])
-  {
+  if (!latent) {
     const int ne = p->num_enc;
     float *cur = ws + W.ea, *nxt = ws + W.eb;
     LnBackArgs lb{};
@@ -1511,13 +1634,17 @@ extern "C" int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* 
       xe = ws + W.ex;
     }
     if ((rc = dweight(cur, n_cur, xe, OT, OT, B, gr->enc[0].weight))) return rc;
+    if (Tq > 0 && (rc = dinput(cur, n_cur, w->enc[0].weight + d.obs_dim, OT, 0, nullptr, 1, Tq, ws + W.exe + Lz, LT, 0, B)))
+      return rc;
+  }
+  {
     if (Tq > 0) {
-      // ---- 5. the task embedding: encoder layer 0, dynamics layer 0, reward layer 0, each Q head's layer 0, in order
-      if ((rc = dinput(cur, n_cur, w->enc[0].weight + d.obs_dim, OT, 0, nullptr, 1, Tq, ws + W.exe + Lz, LT, 0, B))) return rc;
+      // ---- 5. the task embedding: encoder layer 0 (without the latent variant), dynamics layer 0, reward layer 0, each Q
+      // head's layer 0, in order
       CUDA_TRY(cudaMemsetAsync(ws + W.zero, 0, static_cast<size_t>(R) * LT * 4, st));
       const float* z0 = ws + W.zero;
       const dim3 eg(static_cast<int>((d.num_tasks * Tq + 127) / 128));
-      pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.exe + Lz, z0, z0, LT, task, B, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
+      if (!latent) pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.exe + Lz, z0, z0, LT, task, B, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
       pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.dxd + Lz, z0, z0, LT, task, R, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
       pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.dxr + Lz, z0, z0, LT, task, R, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
       for (int h = 0; h < nq; ++h)
@@ -1527,4 +1654,24 @@ extern "C" int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* 
     }
   }
   return 0;
+}
+
+extern "C" int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* obs0,
+                                       const float* action, const int32_t* task, const float* dropout_mask, int H, int B,
+                                       const float* zs, const float* q_logits, const float* reward_logits, const float* term_logits,
+                                       const float* next_z, const float* reward, const float* td_target, const float* terminated,
+                                       const tdmpc2_wm_loss_coefs* cf, const tdmpc2_wm_grads* gr, void* workspace, void* stream_) {
+  return wm_backward_impl(p, w, tape, obs0, action, task, dropout_mask, H, B, zs, q_logits, reward_logits, term_logits, next_z,
+                          reward, td_target, terminated, cf, gr, nullptr, workspace, stream_);
+}
+
+extern "C" int tdmpc2_wm_loss_backward_latent(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* action,
+                                              const int32_t* task, const float* dropout_mask, int H, int B, const float* zs,
+                                              const float* q_logits, const float* reward_logits, const float* term_logits,
+                                              const float* next_z, const float* reward, const float* td_target,
+                                              const float* terminated, const tdmpc2_wm_loss_coefs* cf, const tdmpc2_wm_grads* gr,
+                                              float* dz0, void* workspace, void* stream_) {
+  if (!dz0) return fail(TDMPC2_ERR_INVALID, "null argument");
+  return wm_backward_impl(p, w, tape, nullptr, action, task, dropout_mask, H, B, zs, q_logits, reward_logits, term_logits, next_z,
+                          reward, td_target, terminated, cf, gr, dz0, workspace, stream_);
 }

@@ -43,6 +43,7 @@ struct PixelParams {
   const float* b[4];
   float* scratch;        // [gridDim.x][nc * 29 * 29]: one conv1 slot per CTA
   float* z;              // [rows, 16 * nc]
+  float* tape;           // optional [rows][pix_tape_floats(nc)]: the post-ReLU maps a1 | a2 | a3 of every frame (backward)
   int64_t rows;
   int C, nc, simnorm;
   int smem_floats;       // dynamic shared memory of the launch, in floats
@@ -52,6 +53,12 @@ struct PixelParams {
 // layer's weight chunk follows its activations.
 __host__ __device__ __forceinline__ int pix_stage_floats(int C) { return C * kPixHW * kPixHW; }
 __host__ __device__ __forceinline__ int pix_maps_floats(int nc) { return nc * (kPixO2 * kPixO2 + kPixO3 * kPixO3 + kPixO4 * kPixO4); }
+// The taped forward's per-frame slot, in floats: a1 [nc][29][29] | a2 [nc][13][13] | a3 [nc][6][6], each segment starting
+// on a 64-float boundary.  conv4's output is not taped: SimNorm's backward reads z alone.
+__host__ __device__ __forceinline__ int pix_al64(int n) { return (n + 63) / 64 * 64; }
+__host__ __device__ __forceinline__ int pix_tape_a2(int nc) { return pix_al64(nc * kPixO1 * kPixO1); }
+__host__ __device__ __forceinline__ int pix_tape_a3(int nc) { return pix_tape_a2(nc) + pix_al64(nc * kPixO2 * kPixO2); }
+__host__ __device__ __forceinline__ int pix_tape_floats(int nc) { return pix_tape_a3(nc) + pix_al64(nc * kPixO3 * kPixO3); }
 // Weight chunk of one layer in `cap` floats: occ output channels x icc input channels ([icc][K][K][occ] + occ biases).
 // All output channels with all input channels when they fit, else the widest multiple of 8 output channels, else 8
 // output channels and as many input channels as fit (icc < 1: the layer does not fit at all).
@@ -70,6 +77,27 @@ __device__ __forceinline__ float pix_padded(const float* img, int py, int px) { 
   if (py < 0 || py >= kPixPadded || px < 0 || px >= kPixPadded) return 0.f;
   const int y = min(max(py - kPixPad, 0), kPixHW - 1), x = min(max(px - kPixPad, 0), kPixHW - 1);
   return img[y * kPixHW + x];
+}
+
+// Element i = (c * 64 + y) * 64 + x of ShiftAug + PixelPreprocess applied to one frame `img` [C][64][64] (values 0..255),
+// shift (sx, sy) already scaled by 2/70.  The forward's staging loop and the backward's recomputation of conv1's input both
+// call this, so the two cannot drift apart.
+__device__ __forceinline__ float pix_stage_value(const float* __restrict__ img, const float* __restrict__ grid, float sx, float sy,
+                                                 int i) {
+  const int c = i / (kPixHW * kPixHW), y = (i / kPixHW) % kPixHW, x = i % kPixHW;
+  const float fx = pix_unnormalize(__fadd_rn(grid[x], sx)), fy = pix_unnormalize(__fadd_rn(grid[y], sy));
+  const float wx = floorf(fx), ny = floorf(fy);
+  const float ex = wx + 1.f, sy1 = ny + 1.f;
+  const int ix = static_cast<int>(wx), iy = static_cast<int>(ny);
+  const float* ch = img + static_cast<size_t>(c) * kPixHW * kPixHW;
+  float v = pix_padded(ch, iy, ix) * ((ex - fx) * (sy1 - fy));
+  v += pix_padded(ch, iy, ix + 1) * ((fx - wx) * (sy1 - fy));
+  v += pix_padded(ch, iy + 1, ix) * ((ex - fx) * (fy - ny));
+  v += pix_padded(ch, iy + 1, ix + 1) * ((fx - wx) * (fy - ny));
+  return __fsub_rn(__fdiv_rn(v, 255.f), 0.5f);
+}
+__device__ __forceinline__ float pix_shift_scaled(const float* shift, int64_t e, int k) {
+  return __fmul_rn(shift[e * 2 + k], 2.0f / kPixPadded);
 }
 
 // out[oc][oy][ox] = act(b[oc] + sum_{ic,ky,kx} in[ic][oy*S+ky][ox*S+kx] * w[oc][ic][ky][kx]), one fmaf chain per output in
@@ -146,29 +174,19 @@ __device__ __forceinline__ void pix_conv(const float* in, int IC, int IH, int IW
 __global__ void __launch_bounds__(kPixThreads, 1) pixel_encode_kernel(const PixelParams P) {
   extern __shared__ __align__(16) float pix_smem[];
   const int stage = pix_stage_floats(P.C), maps = pix_maps_floats(P.nc);
-  float* s1 = P.scratch + static_cast<size_t>(blockIdx.x) * P.nc * kPixO1 * kPixO1;   // this CTA's conv1 slot
   float* s2 = pix_smem;                          // conv2-4 maps: the staged input is dead by then
   float* s3 = s2 + P.nc * kPixO2 * kPixO2;
   float* s4 = s3 + P.nc * kPixO3 * kPixO3;
   const int L = P.nc * kPixO4 * kPixO4;
   for (int64_t e = blockIdx.x; e < P.rows; e += gridDim.x) {
     const float* img = P.frames + e * P.C * kPixHW * kPixHW;
+    // conv1's output: this CTA's scratch slot, or the frame's tape slot (a1) when taping
+    float* tslot = P.tape ? P.tape + e * pix_tape_floats(P.nc) : nullptr;
+    float* s1 = tslot ? tslot : P.scratch + static_cast<size_t>(blockIdx.x) * P.nc * kPixO1 * kPixO1;
     __syncthreads();                             // the previous frame's SimNorm has read s4, which the stage overwrites
     // ---- ShiftAug + PixelPreprocess -> smem [C][64][64]
-    const float sx = __fmul_rn(P.shift[e * 2 + 0], 2.0f / kPixPadded), sy = __fmul_rn(P.shift[e * 2 + 1], 2.0f / kPixPadded);
-    for (int i = threadIdx.x; i < P.C * kPixHW * kPixHW; i += kPixThreads) {
-      const int c = i / (kPixHW * kPixHW), y = (i / kPixHW) % kPixHW, x = i % kPixHW;
-      const float fx = pix_unnormalize(__fadd_rn(P.grid[x], sx)), fy = pix_unnormalize(__fadd_rn(P.grid[y], sy));
-      const float wx = floorf(fx), ny = floorf(fy);
-      const float ex = wx + 1.f, sy1 = ny + 1.f;
-      const int ix = static_cast<int>(wx), iy = static_cast<int>(ny);
-      const float* ch = img + static_cast<size_t>(c) * kPixHW * kPixHW;
-      float v = pix_padded(ch, iy, ix) * ((ex - fx) * (sy1 - fy));
-      v += pix_padded(ch, iy, ix + 1) * ((fx - wx) * (sy1 - fy));
-      v += pix_padded(ch, iy + 1, ix) * ((ex - fx) * (fy - ny));
-      v += pix_padded(ch, iy + 1, ix + 1) * ((fx - wx) * (fy - ny));
-      pix_smem[i] = __fsub_rn(__fdiv_rn(v, 255.f), 0.5f);
-    }
+    const float sx = pix_shift_scaled(P.shift, e, 0), sy = pix_shift_scaled(P.shift, e, 1);
+    for (int i = threadIdx.x; i < P.C * kPixHW * kPixHW; i += kPixThreads) pix_smem[i] = pix_stage_value(img, P.grid, sx, sy, i);
     // each pix_conv starts with a barrier: its input is complete (conv1's global slot included -- written and read by
     // this CTA only) and the previous layer no longer reads the smem it stages its weights into
     pix_conv<7, 2, 4, true>(pix_smem, P.C, kPixHW, kPixHW, P.w[0], P.b[0], P.nc, s1, kPixO1, kPixO1, pix_smem + stage,
@@ -180,6 +198,10 @@ __global__ void __launch_bounds__(kPixThreads, 1) pixel_encode_kernel(const Pixe
     pix_conv<3, 1, 1, false>(s3, P.nc, kPixO3, kPixO3, P.w[3], P.b[3], P.nc, s4, kPixO4, kPixO4, pix_smem + maps,
                              P.smem_floats - maps);
     __syncthreads();
+    if (tslot) {                                 // a2, a3: still intact in smem (conv4 staged its weights after s4)
+      for (int i = threadIdx.x; i < P.nc * kPixO2 * kPixO2; i += kPixThreads) tslot[pix_tape_a2(P.nc) + i] = s2[i];
+      for (int i = threadIdx.x; i < P.nc * kPixO3 * kPixO3; i += kPixThreads) tslot[pix_tape_a3(P.nc) + i] = s3[i];
+    }
     // ---- Flatten ([nc][4][4] is already the flattened order) + SimNorm: softmax over groups of `simnorm` consecutive values
     float* zrow = P.z + e * L;
     for (int g0 = threadIdx.x * P.simnorm; g0 < L; g0 += kPixThreads * P.simnorm) {

@@ -363,17 +363,59 @@ class Planner:
         shift [R, 2] (x, y) -> a fresh z [R, L].  Bit-identical to encode_pixels for the same frame and shift."""
         if self.pix is None or self._conv is None:
             raise _cabi.CabiError("encode_pixel_rows needs a cfg.obs == 'rgb' planner with packed weights")
+        frames, shift, R = self._pixel_rows(frames, shift)
+        z = self._rows_out(R, self.cfg.latent_dim)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_pixel_encode_rows(self.pix, self.pix_ws.data_ptr(), C.byref(self._conv), _ptr(frames),
+                                                          _ptr(shift), _ptr(self.pix_grid), R, _ptr(z), self._stream()))
+        return z
+
+    def _pixel_rows(self, frames, shift):
         frames = frames.to(self.device, torch.float32).contiguous()      # ShiftAug's x.float() (layers.py:44)
         shift = shift.to(self.device, torch.float32).contiguous()
         R = frames.shape[0]
         if frames.ndim != 4 or tuple(frames.shape[1:]) != (self.cfg.obs_shape["rgb"][0], 64, 64) or tuple(shift.shape) != (R, 2):
             raise ValueError(f"frames must be [R, {self.cfg.obs_shape['rgb'][0]}, 64, 64] and shift [R, 2]; got "
                              f"{tuple(frames.shape)} and {tuple(shift.shape)}")
-        z = self._rows_out(R, self.cfg.latent_dim)
+        return frames, shift, R
+
+    def encode_pixel_rows_taped(self, frames, shift, out=None):
+        """encode_pixel_rows that also keeps the activations the conv backward needs: -> (z [R, L], tape).  `out`: an
+        optional contiguous [R, L] fp32 tensor to write z into (e.g. zs[0] of the world-model loss).  z is bit-identical to
+        encode_pixel_rows's."""
+        if self.pix is None or self._conv is None:
+            raise _cabi.CabiError("encode_pixel_rows_taped needs a cfg.obs == 'rgb' planner with packed weights")
+        frames, shift, R = self._pixel_rows(frames, shift)
+        z = self._rows_out(R, self.cfg.latent_dim) if out is None else out
+        nb = C.c_size_t()
+        _cabi.check(self.lib.tdmpc2_pixel_encode_tape_bytes(self.pix, R, C.byref(nb)))
+        tape = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.device):
-            _cabi.check(self.lib.tdmpc2_pixel_encode_rows(self.pix, self.pix_ws.data_ptr(), C.byref(self._conv), _ptr(frames),
-                                                          _ptr(shift), _ptr(self.pix_grid), R, _ptr(z), self._stream()))
-        return z
+            _cabi.check(self.lib.tdmpc2_pixel_encode_taped(self.pix, self.pix_ws.data_ptr(), C.byref(self._conv), _ptr(frames),
+                                                           _ptr(shift), _ptr(self.pix_grid), R, _ptr(z), _ptr(tape),
+                                                           self._stream()))
+        return z, tape
+
+    def pixel_encode_backward(self, tensor, tape, frames, shift, z, dz, grads) -> None:
+        """Adds dL/dparameter of the conv encoder to `grads` (the `.grad` tensors of `_encoder.rgb.{2,4,6,8}.{weight,bias}`
+        by state-dict key), given dz = dL/dz [R, L] and the taped forward's tape and z on the same frames and shifts.
+        `tensor(key)` returns the model's fp32 tensor of a state-dict key."""
+        if self.pix is None:
+            raise _cabi.CabiError("pixel_encode_backward needs a cfg.obs == 'rgb' planner")
+        frames, shift, R = self._pixel_rows(frames, shift)
+        W, G = _cabi.ConvWeights(), _cabi.ConvGrads()
+        for i, idx in enumerate((2, 4, 6, 8)):
+            k = f"_encoder.rgb.{idx}"
+            W.weight[i], W.bias[i] = _ptr(tensor(k + ".weight")), _ptr(tensor(k + ".bias"))
+            G.weight[i], G.bias[i] = _ptr(grads[k + ".weight"]), _ptr(grads[k + ".bias"])
+        z, dz = z.reshape(R, -1).contiguous(), dz.reshape(R, -1).contiguous()
+        nb = C.c_size_t()
+        _cabi.check(self.lib.tdmpc2_pixel_backward_workspace_bytes(self.pix, R, C.byref(nb)))
+        ws = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_pixel_encode_backward(self.pix, C.byref(W), _ptr(frames), _ptr(shift), _ptr(self.pix_grid),
+                                                              R, _ptr(tape), _ptr(z), _ptr(dz), C.byref(G), _ptr(ws),
+                                                              self._stream()))
 
     def prologue_latent(self, z, task, t0, prev_mean, noise_prior) -> None:
         self._keep = [z, task, t0, prev_mean, noise_prior]
@@ -690,11 +732,22 @@ class Planner:
                                                         _ptr(ql), _ptr(rl), _ptr(tl), _ptr(tape), self._stream()))
         return tape, zs, ql, rl, tl
 
-    def wm_loss_backward(self, tensor, tape, obs0, action, task, drop, H, B, zs, ql, rl, tl, next_z, reward, td_target,
-                         terminated, grads):
-        """Adds dL/dparameter of _update's world-model loss to `grads` (.grad tensors by state-dict key: `_encoder.state.*`,
-        `_dynamics.*`, `_reward.*`, `_termination.*`, `_Qs.params.*`, `_task_emb.weight`).  `tensor(key)` returns the
-        model's fp32 tensor of a state-dict key."""
+    def wm_loss_forward_latent(self, zs, action, task, drop, H, B):
+        """wm_loss_forward for a latent z_0 the caller wrote into zs[0] (pixel models: encode_pixel_rows_taped(..., out=zs[0])):
+        zs [H + 1, B, L] fp32 contiguous, filled in place -> tape, zs, Q logits, reward logits, termination logits | None."""
+        cfg, R = self.cfg, H * B
+        nb = C.c_size_t()
+        _cabi.check(self.lib.tdmpc2_wm_loss_tape_bytes(self.h, H, B, C.byref(nb)))
+        tape = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        ql, rl = self._rows_out(cfg.num_q, R, cfg.num_bins), self._rows_out(R, cfg.num_bins)
+        tl = self._rows_out(R, 1) if cfg.episodic else None
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_wm_loss_forward_latent(self.h, _ptr(action), _ptr(task), _ptr(drop), H, B, _ptr(zs),
+                                                               _ptr(ql), _ptr(rl), _ptr(tl), _ptr(tape), self._stream()))
+        return tape, zs, ql, rl, tl
+
+    def _wm_loss_structs(self, tensor, grads):
+        """(weights, grads, coefficients) structs of the world-model loss's backward."""
         cfg = self.cfg
 
         def lin(k, ln):
@@ -719,14 +772,39 @@ class Planner:
         G.task_emb = _ptr(grads.get("_task_emb.weight"))
         cf = _cabi.WmLossCoefs(cfg.consistency_coef, cfg.reward_coef, cfg.value_coef, cfg.termination_coef, cfg.rho,
                                cfg.vmin, cfg.vmax, cfg.bin_size)
+        return W, G, cf
+
+    def _wm_loss_workspace(self, H, B):
         nb = C.c_size_t()
         _cabi.check(self.lib.tdmpc2_wm_loss_workspace_bytes(self.h, H, B, C.byref(nb)))
-        ws = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        return torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+
+    def wm_loss_backward(self, tensor, tape, obs0, action, task, drop, H, B, zs, ql, rl, tl, next_z, reward, td_target,
+                         terminated, grads):
+        """Adds dL/dparameter of _update's world-model loss to `grads` (.grad tensors by state-dict key: `_encoder.state.*`,
+        `_dynamics.*`, `_reward.*`, `_termination.*`, `_Qs.params.*`, `_task_emb.weight`).  `tensor(key)` returns the
+        model's fp32 tensor of a state-dict key."""
+        W, G, cf = self._wm_loss_structs(tensor, grads)
+        ws = self._wm_loss_workspace(H, B)
         with torch.cuda.device(self.device):
             _cabi.check(self.lib.tdmpc2_wm_loss_backward(
                 self.h, C.byref(W), _ptr(tape), _ptr(obs0), _ptr(action), _ptr(task), _ptr(drop), H, B, _ptr(zs), _ptr(ql),
                 _ptr(rl), _ptr(tl), _ptr(next_z), _ptr(reward), _ptr(td_target), _ptr(terminated), C.byref(cf), C.byref(G),
                 _ptr(ws), self._stream()))
+
+    def wm_loss_backward_latent(self, tensor, tape, action, task, drop, H, B, zs, ql, rl, tl, next_z, reward, td_target,
+                                terminated, grads) -> torch.Tensor:
+        """wm_loss_backward without the state encoder (`_encoder.*` of `grads` is not touched) -> dL/dz_0 [B, L], for
+        pixel_encode_backward."""
+        W, G, cf = self._wm_loss_structs(tensor, grads)
+        ws = self._wm_loss_workspace(H, B)
+        dz0 = self._rows_out(B, self.cfg.latent_dim)
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.tdmpc2_wm_loss_backward_latent(
+                self.h, C.byref(W), _ptr(tape), _ptr(action), _ptr(task), _ptr(drop), H, B, _ptr(zs), _ptr(ql), _ptr(rl),
+                _ptr(tl), _ptr(next_z), _ptr(reward), _ptr(td_target), _ptr(terminated), C.byref(cf), C.byref(G), _ptr(dz0),
+                _ptr(ws), self._stream()))
+        return dz0
 
     def estimate_value(self, z, actions, task, noise_pi, qidx):
         """z [E,N,L], actions [E,H,N,A], noise_pi [E,N,A], qidx [E,2] int32 -> [E,N]."""

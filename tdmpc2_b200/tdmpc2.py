@@ -7,7 +7,7 @@ Drop-in for the inference half of the reference class `TDMPC2`
 `evaluate.py:57-80` of the reference runs unchanged on it (INTEGRATION.md), and so does the
 no-grad block of `_update` (`model.encode` + `_td_target`, tdmpc2.py:259-264), and the policy update
 `update_pi` (tdmpc2.py:208-239) with its `scale` (RunningScale) and `pi_optim`, and the whole training step
-`update(buffer)` / `_update` (tdmpc2.py:259-346) with its `optim`, for state observations.  Call `sync_weights()` after
+`update(buffer)` / `_update` (tdmpc2.py:259-346) with its `optim`, for state and pixel observations.  Call `sync_weights()` after
 changing the model's parameters outside these methods.
 
 New: an environments axis.  `obs [E, obs_dim]`, `t0 [E]`, `task [E]` plan E
@@ -23,7 +23,7 @@ import torch
 import torch.nn.functional as F
 
 from .config import Config, get_discount
-from .planner import Noise, Planner, draw_noise
+from .planner import Noise, Planner, draw_noise, draw_shifts
 from .scale import RunningScale
 from .world_model import WorldModel, convert_legacy_checkpoint
 
@@ -294,32 +294,50 @@ class TDMPC2(torch.nn.Module):
         return self._update(obs, action, reward, terminated, **kwargs)
 
     def _update(self, obs, action, reward, terminated, task=None, *, td_eps=None, td_qidx=None, dropout_mask=None,
-                pi_eps=None, pi_qidx=None, pi_dropout_mask=None):
-        """tdmpc2.py:259-333 on the kernels, state observations.  obs [H+1, B, obs_dim], action [H, B, A], reward /
-        terminated [H, B, 1], task [B] | None.  The latent rollout and the heads run as taped row launches
-        (tdmpc2_wm_loss_forward), the backward chain of grad_kernels.cuh ADDS the gradients of the world-model loss to
-        `.grad` as autograd would; then torch's clip_grad_norm_ and optim.step(), update_pi on the detached latents, and
-        the Polyak update of the target Q ensemble.
-        Draws from self.generator in the reference's order: the TD target's pi noise and Q pair (`td_eps` [H, B, A],
-        `td_qidx` [2]), the dropout scale of Q layer 0 for the value loss (`dropout_mask` [num_q, H, B, mlp_dim] of
-        mask / (1 - p) values; the reference's vmap dropout stream is not replayed bit for bit), then update_pi's own
-        (`pi_eps`, `pi_qidx`, `pi_dropout_mask`, see update_pi).  Returns the reference's info dict."""
+                pi_eps=None, pi_qidx=None, pi_dropout_mask=None, shift=None):
+        """tdmpc2.py:259-333 on the kernels.  obs [H+1, B, obs_dim] (state) or [H+1, B, C, 64, 64] (pixels, any dtype,
+        values 0..255), action [H, B, A], reward / terminated [H, B, 1], task [B] | None.  The latent rollout and the heads
+        run as taped row launches (tdmpc2_wm_loss_forward), the backward chain of grad_kernels.cuh ADDS the gradients of
+        the world-model loss to `.grad` as autograd would; then torch's clip_grad_norm_ and optim.step(), update_pi on the
+        detached latents, and the Polyak update of the target Q ensemble.  Pixel models encode obs[0] with a taped conv
+        forward into zs[0] (tdmpc2_pixel_encode_taped, tdmpc2_wm_loss_forward_latent), and dL/dz_0 runs through the conv
+        backward of pixel_grad_kernels.cuh into `.grad` of `_encoder.rgb.*`.
+        Draws from self.generator in the reference's order: pixel models' ShiftAug shifts of obs[1:] (H draws of (B, 2)),
+        the TD target's pi noise and Q pair (`td_eps` [H, B, A], `td_qidx` [2]), pixel models' shift of obs[0], the
+        dropout scale of Q layer 0 for the value loss (`dropout_mask` [num_q, H, B, mlp_dim] of mask / (1 - p) values;
+        the reference's vmap dropout stream is not replayed bit for bit), then update_pi's own (`pi_eps`, `pi_qidx`,
+        `pi_dropout_mask`, see update_pi).  `shift` [H+1, B, 2] passes the shifts explicitly, shift[t] belonging to
+        obs[t].  Returns the reference's info dict."""
         cfg, dev = self.cfg, self.device
-        if cfg.get("obs", "state") == "rgb":
-            raise NotImplementedError("_update covers state observations: the conv encoder's backward is not built")
+        rgb = cfg.get("obs", "state") == "rgb"
+        if rgb and dev.type != "cuda":
+            raise NotImplementedError("pixel `_update` runs on the sm_90a conv encoder kernels: no CPU fallback")
         if dev.type != "cuda":
             raise RuntimeError("_update runs on the sm_90a kernels: the agent needs a CUDA device (there is no CPU fallback)")
-        obs_dim, A, L, M = cfg.obs_shape["state"][0], cfg.action_dim, cfg.latent_dim, cfg.mlp_dim
-        if obs.ndim != 3 or obs.shape[0] < 2 or obs.shape[1] < 1 or obs.shape[2] != obs_dim:
-            raise ValueError(f"obs must be [H + 1, B, {obs_dim}]; got {tuple(obs.shape)}")
+        A, L, M = cfg.action_dim, cfg.latent_dim, cfg.mlp_dim
+        if rgb:
+            C_in = cfg.obs_shape["rgb"][0]
+            if obs.ndim != 5 or obs.shape[0] < 2 or obs.shape[1] < 1 or tuple(obs.shape[2:]) != (C_in, 64, 64):
+                raise ValueError(f"obs must be [H + 1, B, {C_in}, 64, 64]; got {tuple(obs.shape)}")
+        else:
+            obs_dim = cfg.obs_shape["state"][0]
+            if obs.ndim != 3 or obs.shape[0] < 2 or obs.shape[1] < 1 or obs.shape[2] != obs_dim:
+                raise ValueError(f"obs must be [H + 1, B, {obs_dim}]; got {tuple(obs.shape)}")
         H, B = int(obs.shape[0]) - 1, int(obs.shape[1])
         for name, x, shape in (("action", action, (H, B, A)), ("reward", reward, (H, B, 1)), ("terminated", terminated, (H, B, 1))):
             if tuple(x.shape) != shape:
                 raise ValueError(f"{name} must be {list(shape)}; got {tuple(x.shape)}")
             if not x.is_floating_point():
                 raise ValueError(f"{name} must be a floating-point tensor; got {x.dtype}")
-        if not obs.is_floating_point():
+        if not rgb and not obs.is_floating_point():
             raise ValueError(f"obs must be a floating-point tensor; got {obs.dtype}")
+        if shift is not None:
+            if not rgb:
+                raise ValueError("shift applies to pixel models (cfg.obs == 'rgb')")
+            shift = torch.as_tensor(shift, device=dev)
+            if tuple(shift.shape) != (H + 1, B, 2):
+                raise ValueError(f"shift must be [{H + 1}, {B}, 2]; got {tuple(shift.shape)}")
+            shift = shift.to(torch.float32)
         if cfg.multitask and task is None:
             raise ValueError("multi-task model needs `task`")
         drop = None
@@ -336,9 +354,14 @@ class TDMPC2(torch.nn.Module):
 
         # targets (tdmpc2.py:261-264)
         with torch.no_grad():
-            next_z = self.model.encode(obs[1:], task)
+            if rgb:
+                next_z = self.model.encode(obs[1:], task, shift=None if shift is None else shift[1:])
+            else:
+                next_z = self.model.encode(obs[1:], task)
             td_targets = self.model.td_target(next_z, reward, terminated, task, eps=td_eps, qidx=td_qidx)
         self.model.train()
+        if rgb:                                              # ShiftAug's draw inside encode(obs[0]) (layers.py:55)
+            shift0 = draw_shifts((B,), dev, g) if shift is None else shift[0]
         if drop is None and cfg.dropout > 0:                 # nn.Dropout(cfg.dropout) of Q layer 0 (layers.py:104-108)
             keep = 1.0 - cfg.dropout
             drop = torch.empty(cfg.num_q, H * B, M, device=dev).bernoulli_(keep, generator=g).div_(keep)
@@ -348,7 +371,12 @@ class TDMPC2(torch.nn.Module):
         # latent rollout and heads (tdmpc2.py:269-285), on the kernels with a tape
         pl = self.planner
         act_rows = action.reshape(H * B, A)
-        tape, zs, ql, rl, tl = pl.wm_loss_forward(obs[0], act_rows, taskv, drop, H, B)
+        if rgb:
+            zs = torch.empty(H + 1, B, L, device=dev, dtype=torch.float32)
+            _, pix_tape = pl.encode_pixel_rows_taped(obs[0], shift0, out=zs[0])
+            tape, zs, ql, rl, tl = pl.wm_loss_forward_latent(zs, act_rows, taskv, drop, H, B)
+        else:
+            tape, zs, ql, rl, tl = pl.wm_loss_forward(obs[0], act_rows, taskv, drop, H, B)
         rho = torch.pow(cfg.rho, torch.arange(H, device=dev, dtype=torch.float32))
         consistency_loss = (F.mse_loss(zs[1:], next_z, reduction="none").mean(dim=(1, 2)) * rho).sum() / H
         reward_loss = (_soft_ce(rl.view(H, B, -1), reward, cfg).mean(dim=(1, 2)) * rho).sum() / H
@@ -367,8 +395,14 @@ class TDMPC2(torch.nn.Module):
         for p in params:
             if p.grad is None:
                 p.grad = torch.zeros_like(p)
-        pl.wm_loss_backward(self.model.tensor, tape, obs[0], act_rows, taskv, drop, H, B, zs, ql, rl, tl, next_z, reward,
-                            td_targets, terminated, {k: p.grad for k, p in zip(self._wm_keys, params)})
+        grads = {k: p.grad for k, p in zip(self._wm_keys, params)}
+        if rgb:
+            dz0 = pl.wm_loss_backward_latent(self.model.tensor, tape, act_rows, taskv, drop, H, B, zs, ql, rl, tl, next_z,
+                                             reward, td_targets, terminated, grads)
+            pl.pixel_encode_backward(self.model.tensor, pix_tape, obs[0], shift0, zs[0], dz0, grads)
+        else:
+            pl.wm_loss_backward(self.model.tensor, tape, obs[0], act_rows, taskv, drop, H, B, zs, ql, rl, tl, next_z, reward,
+                                td_targets, terminated, grads)
         grad_norm = torch.nn.utils.clip_grad_norm_([p for p in self.model.parameters() if p.grad is not None],
                                                    cfg.grad_clip_norm)
         self.optim.step()
