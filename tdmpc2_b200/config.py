@@ -51,6 +51,9 @@ _DEFAULTS: Dict[str, Any] = dict(
     lr=3e-4, enc_lr_scale=0.3, tau=0.01, rho=0.5, grad_clip_norm=20, batch_size=256, seed=1, compile=False,
     # replay buffer (config.yaml:15,29), read by buffer.Buffer: capacity = min(buffer_size, steps)
     steps=10_000_000, buffer_size=1_000_000,
+    # training loops (config.yaml:11-12), read by trainer.OnlineTrainer / OfflineTrainer; seed_steps None means
+    # max(1000, 5 * episode_length) (envs/__init__.py:82), resolved by trainer.seed_steps
+    eval_episodes=10, eval_freq=50_000, seed_steps=None,
     # filled in by make_cfg
     multitask=False, tasks=None, obs_shape=None, action_dim=None, action_dims=None,
     episode_length=None, episode_lengths=None, bin_size=None,
