@@ -35,18 +35,13 @@
 extern "C" {
 #endif
 
-#define TDMPC2_B200_ABI_VERSION 7   /* 2: tdmpc2_weights.termination, dims.episodic = 1 accepted; 3: tdmpc2_planner_set_l2_persist;
-                                       4: tdmpc2_planner_set_passes (declared non-parity fast mode), set_kseg, iter_engine;
+#define TDMPC2_B200_ABI_VERSION 8   /* 2: tdmpc2_weights.termination, dims.episodic = 1 accepted; 3: a persisting-L2 knob;
+                                       4: tdmpc2_planner_set_passes (declared non-parity fast mode), reduction-segment knobs, engine query;
                                        5: pixel encoder (tdmpc2_pixel_*), tdmpc2_plan_prologue_latent, dims.num_enc_layers = 0;
                                        6: tdmpc2_plan_iter_rng (declared non-parity in-kernel noise), tdmpc2_debug_rng;
-                                       7: world-model methods on a flat batch (tdmpc2_wm_*, tdmpc2_td_target), target Q blob;
-                                          later, additive: tdmpc2_pixel_encode_rows (old callers and bindings unaffected);
-                                          later, additive: agent.update_pi (tdmpc2_pi_loss_*, tdmpc2_pi_grads),
-                                          agent._update (tdmpc2_wm_loss_*, tdmpc2_wm_grads);
-                                          later, additive: agent._update of pixel models (tdmpc2_pixel_encode_taped,
-                                          tdmpc2_pixel_encode_backward, tdmpc2_conv_grads, tdmpc2_wm_loss_*_latent);
-                                          later, additive: the replay buffer's sampler (tdmpc2_buffer_sample,
-                                          tdmpc2_buffer_field) */
+                                       7: world-model methods on a flat batch (tdmpc2_wm_*, tdmpc2_td_target), target Q blob, then
+                                          agent.update_pi, agent._update of state and pixel models, the replay buffer's sampler;
+                                       8: removed engines 2-4, the engine query, the L2 and reduction-segment knobs; one tdmpc2_pixel_encode */
 #define TDMPC2_MAX_ENC_LAYERS 8
 
 typedef enum tdmpc2_status {
@@ -58,15 +53,10 @@ typedef enum tdmpc2_status {
   TDMPC2_ERR_UNSUPPORTED = -5  /* config outside what the reference's planner itself accepts (multi-task episodic) */
 } tdmpc2_status;
 
-/* GEMM engine used by the fused MLP kernels. */
+/* GEMM engine used by the fused MLP kernels (tdmpc2_planner_set_engine; any other code is TDMPC2_ERR_INVALID). */
 typedef enum tdmpc2_engine {
-  TDMPC2_ENGINE_TCGEN05 = 0,   /* TMA + wgmma (3x fp16-split, fp32 register accumulate): the product path */
-  TDMPC2_ENGINE_SIMT = 1,      /* CUDA-core fp32 FFMA over the same packed operands: bring-up / diagnostics  */
-  /* Engines 2 - 4 (CTA pairs, ping-pong halves, weight prefetch) were designed around cta_group::2 MMAs, which sm_90a
-     does not have.  They are accepted and run as engine 0 (tdmpc2_planner_iter_engine reports 0). */
-  TDMPC2_ENGINE_TCGEN05_2SM = 2,
-  TDMPC2_ENGINE_TCGEN05_PP = 3,
-  TDMPC2_ENGINE_TCGEN05_2SM_PF = 4
+  TDMPC2_ENGINE_TCGEN05 = 0,   /* TMA + wgmma (3x fp16-split, fp32 register accumulate): the product path; the name is historical */
+  TDMPC2_ENGINE_SIMT = 1       /* CUDA-core fp32 FFMA over the same packed operands: the reference engine 0 is tested against */
 } tdmpc2_engine;
 
 /* Planner + model dimensions.  Mirrors the keys the reference reads from cfg:
@@ -139,18 +129,6 @@ int tdmpc2_planner_workspace_bytes(const tdmpc2_planner* p, size_t* out);
  * workspace and encode the TMA descriptors.  Synchronous. */
 int tdmpc2_planner_bind(tdmpc2_planner* p, void* packed, void* workspace);
 int tdmpc2_planner_set_engine(tdmpc2_planner* p, int engine);
-/* The engine the CEM-iteration launches actually run: the requested one falls back (3 -> 2 -> 0) when the model or the
- * batch shape does not fit it.  -1 on a null planner. */
-int tdmpc2_planner_iter_engine(const tdmpc2_planner* p);
-/* enable != 0: every planning launch carries an access-policy window that keeps the per-CTA activation scratch in the
- * persisting part of L2 (sets the DEVICE-wide cudaLimitPersistingL2CacheSize, hence opt-in); 0 switches it off.
- * No reference counterpart (the reference's activations are ordinary torch tensors). */
-int tdmpc2_planner_set_l2_persist(tdmpc2_planner* p, int enable);
-/* Reduction-segment knobs (k_elems >= 0) of the wide layers and of the head layers.  The wgmma engine already adds the
- * partial sum of every 64-element K-chunk with round-to-nearest, so on this build they validate their argument and
- * change nothing.  No reference counterpart. */
-int tdmpc2_planner_set_kseg(tdmpc2_planner* p, int k_elems);
-int tdmpc2_planner_set_head_kseg(tdmpc2_planner* p, int k_elems);
 /* Arithmetic of the tensor-core engine 0.  passes = 3 (default): every product is three fp16 MMAs over the hi / lo
  * operand planes -- the mode whose results match the reference's fp32 plan() (tdmpc2.py:138-206) within 1e-4.
  * passes = 1: DECLARED NON-PARITY fast mode -- hi planes only (one fp16 MMA per product, fp32 accumulate; ~1e-3
@@ -191,7 +169,6 @@ int tdmpc2_debug_rng(const uint64_t* rng_state, uint32_t stream, uint64_t group0
  * (layers.py:36-59; part of the nn.Sequential, hence applied at inference too), PixelPreprocess (:62-71), four
  * Conv2d (7/2, 5/2, 3/2, 3/1) with ReLU between them, Flatten, SimNorm.  64 x 64 frames; latent_dim = 16 * num_channels. */
 typedef struct tdmpc2_pixel_dims {
-  int32_t num_envs;        /* E                                                          */
   int32_t in_channels;     /* cfg.obs_shape['rgb'][0] (3 x frame stack)                  */
   int32_t num_channels;    /* cfg.num_channels (config.yaml:58), a multiple of 8         */
   int32_t simnorm_dim;     /* cfg.simnorm_dim                                            */
@@ -204,31 +181,27 @@ typedef struct tdmpc2_pixel_encoder tdmpc2_pixel_encoder;
 int tdmpc2_pixel_encoder_create(const tdmpc2_pixel_dims* dims, tdmpc2_pixel_encoder** out);
 void tdmpc2_pixel_encoder_destroy(tdmpc2_pixel_encoder* e);
 int tdmpc2_pixel_encoder_workspace_bytes(const tdmpc2_pixel_encoder* e, size_t* out);
-/*   frames [E, C, 64, 64] fp32 in 0..255; shift [E, 2] = the (x, y) values torch.randint(0, 7) draws in ShiftAug
+/* One launch over `rows` frames (e.g. the planning prologue's E observations, or WorldModel.encode(obs[1:]) of _update
+ * (tdmpc2.py:262) on a [T, B, C, 64, 64] batch flattened by the caller):
+ *   frames [rows, C, 64, 64] fp32 in 0..255; shift [rows, 2] = the (x, y) values torch.randint(0, 7) draws in ShiftAug
  *   (layers.py:55), as floats; grid_base [64] = torch.linspace(-1 + 1/70, 1 - 1/70, 70)[:64] (layers.py:51);
- *   z_out [E, 16 * num_channels]; workspace: caller-owned, tdmpc2_pixel_encoder_workspace_bytes. */
+ *   z_out [rows, 16 * num_channels]; workspace: caller-owned, tdmpc2_pixel_encoder_workspace_bytes (it does not depend
+ *   on rows); tape: NULL, or [rows] slots of tdmpc2_pixel_encode_tape_bytes / rows that receive each frame's post-ReLU
+ *   maps for the backward below (z is bit-identical either way).
+ * No allocation and no host synchronisation (capturable in a CUDA graph).  rows < 1 or a null pointer other than tape:
+ * TDMPC2_ERR_INVALID. */
 int tdmpc2_pixel_encode(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
-                        const float* shift, const float* grid_base, float* z_out, void* stream);
-/* The same encoder over any number of frames, e.g. WorldModel.encode(obs[1:]) of _update (tdmpc2.py:262) on a
- * [T, B, C, 64, 64] batch flattened by the caller: frames [rows, C, 64, 64], shift [rows, 2], z_out [rows, 16 * num_channels].
- * One launch, the same workspace as tdmpc2_pixel_encode (its size does not depend on rows), no allocation and no host
- * synchronisation (capturable in a CUDA graph).  z of a frame is bit-identical to tdmpc2_pixel_encode's for the same
- * frame and shift.  rows < 1 or a null pointer: TDMPC2_ERR_INVALID. */
-int tdmpc2_pixel_encode_rows(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
-                             const float* shift, const float* grid_base, int64_t rows, float* z_out, void* stream);
-/* Training (agent._update of pixel models, tdmpc2.py:266-309).  tdmpc2_pixel_encode_taped is tdmpc2_pixel_encode_rows that
- * also writes each frame's post-ReLU maps to `tape` ([rows] slots of tape_bytes / rows; z is bit-identical to the untaped
- * launch).  tdmpc2_pixel_encode_backward ADDS dL/dparameter of the four Conv2d layers to `grads`, like autograd
- * accumulates .grad, given dz = dL/dz [rows, 16 * num_channels], the forward's z and tape and its frames and shifts
- * (conv1's input is recomputed).  fp32 FFMA; reductions over frames in a fixed order (repeated calls give identical bits);
- * no allocation, no host synchronisation.  workspace: tdmpc2_pixel_backward_workspace_bytes(rows). */
+                        const float* shift, const float* grid_base, int64_t rows, float* z_out, float* tape, void* stream);
+/* Training (agent._update of pixel models, tdmpc2.py:266-309).  tdmpc2_pixel_encode_backward ADDS dL/dparameter of the
+ * four Conv2d layers to `grads`, like autograd accumulates .grad, given dz = dL/dz [rows, 16 * num_channels], the taped
+ * forward's z and tape and its frames and shifts (conv1's input is recomputed).  fp32 FFMA; reductions over frames in a
+ * fixed order (repeated calls give identical bits); no allocation, no host synchronisation.  workspace:
+ * tdmpc2_pixel_backward_workspace_bytes(rows). */
 typedef struct tdmpc2_conv_grads {   /* .grad of _encoder.rgb.{2,4,6,8}.{weight,bias} */
   float* weight[4];
   float* bias[4];
 } tdmpc2_conv_grads;
 int tdmpc2_pixel_encode_tape_bytes(const tdmpc2_pixel_encoder* e, int64_t rows, size_t* out);
-int tdmpc2_pixel_encode_taped(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
-                              const float* shift, const float* grid_base, int64_t rows, float* z_out, float* tape, void* stream);
 int tdmpc2_pixel_backward_workspace_bytes(const tdmpc2_pixel_encoder* e, int64_t rows, size_t* out);
 int tdmpc2_pixel_encode_backward(tdmpc2_pixel_encoder* e, const tdmpc2_conv_weights* w, const float* frames,
                                  const float* shift, const float* grid_base, int64_t rows, const float* tape, const float* z,
@@ -385,7 +358,7 @@ int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const fl
                             const float* next_z, const float* reward, const float* td_target, const float* terminated,
                             const tdmpc2_wm_loss_coefs* coefs, const tdmpc2_wm_grads* grads, void* workspace, void* stream);
 /* Planners without a state encoder (pixel models, num_enc_layers = 0) get TDMPC2_ERR_UNSUPPORTED from the two calls above;
- * they use these.  _latent forward: zs[0] ([B, L]) is the caller's, written by tdmpc2_pixel_encode_taped; the rest as
+ * they use these.  _latent forward: zs[0] ([B, L]) is the caller's, written by a taped tdmpc2_pixel_encode; the rest as
  * tdmpc2_wm_loss_forward.  _latent backward: as tdmpc2_wm_loss_backward without the state encoder (grads->enc and
  * w->enc are not read), and dL/dz_0 [B, L] is written to dz0, for tdmpc2_pixel_encode_backward.  tape_bytes and
  * workspace_bytes answer for both variants. */

@@ -4,7 +4,7 @@ Model: c1 with obs="rgb", obs_channels=9 (num_channels 32, latent 512).  Arms:
   a  Planner.encode_pixel_rows (the kernel alone) at each frame count
   b  WorldModel.encode end to end: uint8 frames [T, 256, C, 64, 64], ShiftAug draws, fp32 conversion, one launch
   c  batched eager fp32 PyTorch: grid_sample + 4 x conv2d (cuDNN, TF32 off) + SimNorm
-  d  Planner(cfg, E).encode_pixels, the planning prologue's call, at E in --envs
+  d  Planner(cfg, E).encode_pixel_rows into the static latent buffer, the planning prologue's call, at E in --envs
 CUDA-event medians after warm-up; prints the GPU name and power limit, and FP32 TFLOP/s computed from the shapes.
 
     python scripts/bench_pixel_encode.py [--frames 768 8192] [--envs 1 256 768] [--arms abcd] [--dump DIR]
@@ -96,7 +96,7 @@ def dump(out_dir, envs):
             pl = Planner(cfg, E, "cuda:0")
             pl.pack(sd)
             frames, shift = frames_and_shift(cfg, E, 1000 + E)
-            rec[f"{tag}_E{E}"] = pl.encode_pixels(frames, shift).cpu().numpy()
+            rec[f"{tag}_E{E}"] = pl.encode_pixel_rows(frames, shift, out=pl.pix_z).cpu().numpy()
     os.makedirs(out_dir, exist_ok=True)
     np.savez(os.path.join(out_dir, "pixel_z.npz"), **rec)
     print(json.dumps({"dump": os.path.join(out_dir, "pixel_z.npz"), "keys": sorted(rec)}))
@@ -158,7 +158,7 @@ def main():
             plE = Planner(cfgE, E, "cuda:0")
             plE.pack(sd)
             frames, shift = frames_and_shift(cfgE, E, 8)
-            ms = median_ms(lambda: plE.encode_pixels(frames, shift), args.reps, args.warmup)
+            ms = median_ms(lambda: plE.encode_pixel_rows(frames, shift, out=plE.pix_z), args.reps, args.warmup)
             res[f"d_prologue_E{E}_ms"], res[f"d_prologue_E{E}_tflops"] = round(ms, 4), rate(E, ms)
             del plE
     res["datasheet_fp32_bound_ms"] = {R: round(R * flop / 67e12 * 1e3, 3) for R in args.frames}

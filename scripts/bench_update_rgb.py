@@ -6,7 +6,7 @@ PyTorch autograd (cuDNN convolutions, TF32 off) with a capturable Adam on the sa
 The workload is c1 with pixel observations (C = 9 stacked channels, num_channels = 32, latent 512).  The kernel arm is
 the whole _update: encode(obs[1:]) + TD target, the taped conv forward of obs[0], the latent world-model loss forward and
 backward, the conv backward chain, clip_grad_norm_, Adam, update_pi and the target soft update.  It is broken down into
-the taped conv forward (tdmpc2_pixel_encode_taped) and the conv backward chain (tdmpc2_pixel_encode_backward) timed
+the taped conv forward (tdmpc2_pixel_encode with a tape) and the conv backward chain (tdmpc2_pixel_encode_backward) timed
 alone; the rest is the difference.  The eager arm runs the world-model loss (ShiftAug + conv encoder of obs[0], H
 dynamics steps, num_q Q heads with dropout, reward head), backward, clip and Adam, given the TD targets (it does not run
 update_pi).  Prints the GPU's name and power limit, then one JSON line.

@@ -10,7 +10,7 @@ wl = sys.argv[1] if len(sys.argv) > 1 else "c2"
 E = int(sys.argv[2]) if len(sys.argv) > 2 else 37
 iters = int(sys.argv[3]) if len(sys.argv) > 3 else 3
 cfg = workload(wl, num_envs=E)
-pl = Planner(cfg, E, "cuda:0", engine=os.environ.get("TDMPC2_ENGINE"))     # None: the default engine (ping-pong, falling back to CTA pairs)
+pl = Planner(cfg, E, "cuda:0", engine=os.environ.get("TDMPC2_ENGINE"))     # None: the default engine (tcgen05)
 pl.pack(synth_state_dict(cfg, seed=1))
 dev = torch.device("cuda:0")
 n = draw_noise(cfg, E, dev, reference_order=False)

@@ -10,23 +10,23 @@ import os
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("TDMPC2_B200_LIB") or os.path.join(HERE, "libtdmpc2_b200.so")
 MAX_ENC_LAYERS = 8
-ENGINE_TCGEN05, ENGINE_SIMT, ENGINE_TCGEN05_2SM, ENGINE_TCGEN05_PP, ENGINE_TCGEN05_2SM_PF = 0, 1, 2, 3, 4
+ENGINE_TCGEN05, ENGINE_SIMT = 0, 1     # tdmpc2_engine
 Q_ALL, Q_MIN, Q_AVG = 0, 1, 2   # tdmpc2_q_return
-ABI_VERSION = 7            # TDMPC2_B200_ABI_VERSION of include/tdmpc2_b200.h this binding was written against
+ABI_VERSION = 8            # TDMPC2_B200_ABI_VERSION of include/tdmpc2_b200.h this binding was written against
 
 # every symbol include/tdmpc2_b200.h declares
 SYMBOLS = [
     "tdmpc2_abi_version", "tdmpc2_last_error", "tdmpc2_planner_create", "tdmpc2_planner_destroy",
     "tdmpc2_planner_packed_bytes", "tdmpc2_planner_workspace_bytes", "tdmpc2_planner_bind",
-    "tdmpc2_planner_set_engine", "tdmpc2_planner_iter_engine", "tdmpc2_planner_set_l2_persist", "tdmpc2_planner_set_kseg", "tdmpc2_planner_set_head_kseg", "tdmpc2_planner_set_passes", "tdmpc2_pack_weights", "tdmpc2_plan_prologue", "tdmpc2_plan_prologue_latent",
-    "tdmpc2_pixel_encoder_create", "tdmpc2_pixel_encoder_destroy", "tdmpc2_pixel_encoder_workspace_bytes", "tdmpc2_pixel_encode", "tdmpc2_pixel_encode_rows", "tdmpc2_plan_iter", "tdmpc2_plan_iter_rng", "tdmpc2_debug_rng",
+    "tdmpc2_planner_set_engine", "tdmpc2_planner_set_passes", "tdmpc2_pack_weights", "tdmpc2_plan_prologue", "tdmpc2_plan_prologue_latent",
+    "tdmpc2_pixel_encoder_create", "tdmpc2_pixel_encoder_destroy", "tdmpc2_pixel_encoder_workspace_bytes", "tdmpc2_pixel_encode", "tdmpc2_plan_iter", "tdmpc2_plan_iter_rng", "tdmpc2_debug_rng",
     "tdmpc2_plan_epilogue", "tdmpc2_plan_get_state", "tdmpc2_estimate_value", "tdmpc2_debug_layer",
     "tdmpc2_planner_layer_count", "tdmpc2_planner_launch_count", "tdmpc2_planner_set_profile",
     "tdmpc2_planner_target_q_bytes", "tdmpc2_planner_bind_target_q", "tdmpc2_pack_target_q",
     "tdmpc2_wm_encode", "tdmpc2_wm_next", "tdmpc2_wm_reward", "tdmpc2_wm_termination", "tdmpc2_wm_pi", "tdmpc2_wm_q",
     "tdmpc2_td_target", "tdmpc2_pi_loss_tape_bytes", "tdmpc2_pi_loss_workspace_bytes", "tdmpc2_pi_loss_forward",
     "tdmpc2_pi_loss_backward", "tdmpc2_wm_loss_tape_bytes", "tdmpc2_wm_loss_workspace_bytes", "tdmpc2_wm_loss_forward",
-    "tdmpc2_wm_loss_backward", "tdmpc2_pixel_encode_tape_bytes", "tdmpc2_pixel_encode_taped",
+    "tdmpc2_wm_loss_backward", "tdmpc2_pixel_encode_tape_bytes",
     "tdmpc2_pixel_backward_workspace_bytes", "tdmpc2_pixel_encode_backward", "tdmpc2_wm_loss_forward_latent",
     "tdmpc2_wm_loss_backward_latent", "tdmpc2_buffer_sample",
 ]
@@ -52,7 +52,7 @@ class Weights(C.Structure):
 
 
 class PixelDims(C.Structure):
-    _fields_ = [(n, C.c_int32) for n in ("num_envs", "in_channels", "num_channels", "simnorm_dim")]
+    _fields_ = [(n, C.c_int32) for n in ("in_channels", "num_channels", "simnorm_dim")]
 
 
 class ConvWeights(C.Structure):
@@ -118,10 +118,6 @@ def load():
     lib.tdmpc2_planner_workspace_bytes.argtypes = [vp, C.POINTER(C.c_size_t)]
     lib.tdmpc2_planner_bind.argtypes = [vp, vp, vp]
     lib.tdmpc2_planner_set_engine.argtypes = [vp, C.c_int]
-    lib.tdmpc2_planner_iter_engine.argtypes = [vp]
-    lib.tdmpc2_planner_set_l2_persist.argtypes = [vp, C.c_int]
-    lib.tdmpc2_planner_set_kseg.argtypes = [vp, C.c_int]
-    lib.tdmpc2_planner_set_head_kseg.argtypes = [vp, C.c_int]
     lib.tdmpc2_planner_set_passes.argtypes = [vp, C.c_int]
     lib.tdmpc2_pack_weights.argtypes = [vp, C.POINTER(Weights), vp]
     lib.tdmpc2_plan_prologue.argtypes = [vp, vp, vp, vp, vp, vp, vp]
@@ -130,8 +126,7 @@ def load():
     lib.tdmpc2_pixel_encoder_destroy.argtypes = [vp]
     lib.tdmpc2_pixel_encoder_destroy.restype = None
     lib.tdmpc2_pixel_encoder_workspace_bytes.argtypes = [vp, C.POINTER(C.c_size_t)]
-    lib.tdmpc2_pixel_encode.argtypes = [vp, vp, C.POINTER(ConvWeights), vp, vp, vp, vp, vp]
-    lib.tdmpc2_pixel_encode_rows.argtypes = [vp, vp, C.POINTER(ConvWeights), vp, vp, vp, i64, vp, vp]
+    lib.tdmpc2_pixel_encode.argtypes = [vp, vp, C.POINTER(ConvWeights), vp, vp, vp, i64, vp, vp, vp]
     lib.tdmpc2_plan_iter.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.tdmpc2_plan_iter_rng.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp]
     lib.tdmpc2_debug_rng.argtypes = [vp, C.c_uint32, C.c_uint64, C.c_int, vp, vp]
@@ -164,7 +159,6 @@ def load():
     lib.tdmpc2_wm_loss_backward.argtypes = [vp, C.POINTER(Weights), vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp,
                                             vp, vp, C.POINTER(WmLossCoefs), C.POINTER(WmGrads), vp, vp]
     lib.tdmpc2_pixel_encode_tape_bytes.argtypes = [vp, i64, C.POINTER(C.c_size_t)]
-    lib.tdmpc2_pixel_encode_taped.argtypes = [vp, vp, C.POINTER(ConvWeights), vp, vp, vp, i64, vp, vp, vp]
     lib.tdmpc2_pixel_backward_workspace_bytes.argtypes = [vp, i64, C.POINTER(C.c_size_t)]
     lib.tdmpc2_pixel_encode_backward.argtypes = [vp, C.POINTER(ConvWeights), vp, vp, vp, i64, vp, vp, vp, C.POINTER(ConvGrads),
                                                  vp, vp]
@@ -172,10 +166,6 @@ def load():
     lib.tdmpc2_wm_loss_backward_latent.argtypes = [vp, C.POINTER(Weights), vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp,
                                                    vp, vp, vp, C.POINTER(WmLossCoefs), C.POINTER(WmGrads), vp, vp, vp]
     lib.tdmpc2_buffer_sample.argtypes = [C.POINTER(BufferField), C.c_int, i64, vp, vp, i64, vp, vp, C.c_int, C.c_int, vp]
-    for s in SYMBOLS:
-        f = getattr(lib, s)
-        if f.restype is C.c_int and s not in ("tdmpc2_abi_version", "tdmpc2_planner_layer_count"):
-            pass
     _lib = lib
     return lib
 

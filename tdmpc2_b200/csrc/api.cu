@@ -198,8 +198,6 @@ struct tdmpc2_planner {
   bool attr_done[6] = {};           // dynamic-smem opt-in done, per plan_kernel instantiation
   TargetQ tq;
   int64_t launches = 0;
-  size_t l2_window_bytes = 0;       // > 0: launches carry a persisting-L2 access-policy window over the activation scratch
-  float l2_hit_ratio = 1.f;
   int passes = 3;                   // 3 = fp32-parity arithmetic, 1 = declared non-parity fast mode (PlanParams::passes)
   int zb_kc0 = 0, zb_pitch = 0;     // shared-latent fold (PlanParams::zbias): K-chunks of [z | emb] folded into a per-env bias
   const int32_t* cur_task = nullptr;
@@ -356,21 +354,9 @@ extern "C" int tdmpc2_planner_set_profile(tdmpc2_planner* p, long long* device_b
   return 0;
 }
 extern "C" int tdmpc2_planner_set_engine(tdmpc2_planner* p, int engine) {
-  if (!p || (engine != TDMPC2_ENGINE_TCGEN05 && engine != TDMPC2_ENGINE_SIMT && engine != TDMPC2_ENGINE_TCGEN05_2SM &&
-             engine != TDMPC2_ENGINE_TCGEN05_PP && engine != TDMPC2_ENGINE_TCGEN05_2SM_PF))
-    return fail(TDMPC2_ERR_INVALID, "bad engine");
+  if (!p || (engine != TDMPC2_ENGINE_TCGEN05 && engine != TDMPC2_ENGINE_SIMT))
+    return fail(TDMPC2_ERR_INVALID, "bad engine: 0 (tensor cores) or 1 (SIMT)");
   p->engine = engine;
-  return 0;
-}
-
-// The tensor-core engine adds every 64-element K-chunk's partial sum with round-to-nearest, which is finer than any
-// segment length these calls can ask for: they validate their argument and change nothing on this build.
-extern "C" int tdmpc2_planner_set_kseg(tdmpc2_planner* p, int k_elems) {
-  if (!p || k_elems < 0) return fail(TDMPC2_ERR_INVALID, "bad kseg");
-  return 0;
-}
-extern "C" int tdmpc2_planner_set_head_kseg(tdmpc2_planner* p, int k_elems) {
-  if (!p || k_elems < 0) return fail(TDMPC2_ERR_INVALID, "bad head kseg");
   return 0;
 }
 
@@ -547,22 +533,6 @@ extern "C" int tdmpc2_pack_weights(tdmpc2_planner* p, const tdmpc2_weights* w, v
 }
 
 // ------------------------------------------------------------------------------------ launches
-// The engine the CEM-iteration launches of this planner actually run.  The CTA-pair and ping-pong engines (2, 3, 4) are
-// built on Blackwell's cta_group::2 MMAs; on sm_90a they run as the single-CTA tensor-core engine 0.
-extern "C" int tdmpc2_planner_iter_engine(const tdmpc2_planner* p) {
-  if (!p) return -1;
-  return p->engine == TDMPC2_ENGINE_SIMT ? TDMPC2_ENGINE_SIMT : TDMPC2_ENGINE_TCGEN05;
-}
-
-// Launch attributes shared by every plan_kernel launch: when enabled (tdmpc2_planner_set_l2_persist), an access-policy
-// window that keeps the per-CTA activation scratch (X + H planes, contiguous in the workspace) resident in the
-// persisting part of L2, so that its dirty lines are not written back to HBM while noise and weights stream through.
-struct LaunchCfg {
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[1];
-  LaunchCfg(tdmpc2_planner* p, int grid, size_t smem, cudaStream_t st);
-};
-
 // Every plan_kernel launch.  The instantiation follows the engine and the kind of launch: planning, the rollout modes of
 // an episodic model (MODE_ITER / MODE_VALUE with the termination head), or row mode.  Row launches are not profiled.
 static int launch(tdmpc2_planner* p, const PlanParams& prm, void* stream_) {
@@ -583,44 +553,12 @@ static int launch(tdmpc2_planner* p, const PlanParams& prm, void* stream_) {
   prm2.prof = rows ? nullptr : p->prof;
   prm2.prof_slots = p->nslots;
   prm2.passes = p->passes;
-  LaunchCfg lc(p, std::min(prm.ntiles, p->nslots), kSmemBytes, static_cast<cudaStream_t>(stream_));
-  CUDA_TRY(cudaLaunchKernelEx(&lc.cfg, kernel, prm2));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(std::min(prm.ntiles, p->nslots)); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = kSmemBytes;
+  cfg.stream = static_cast<cudaStream_t>(stream_);
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, kernel, prm2));
   CUDA_TRY(cudaGetLastError());
   p->launches += 1;
-  return 0;
-}
-
-LaunchCfg::LaunchCfg(tdmpc2_planner* p, int grid, size_t smem, cudaStream_t st) {
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  int n = 0;
-  if (p->l2_window_bytes > 0) {
-    attr[n].id = cudaLaunchAttributeAccessPolicyWindow;
-    attr[n].val.accessPolicyWindow.base_ptr = p->ws + p->off_X;
-    attr[n].val.accessPolicyWindow.num_bytes = p->l2_window_bytes;
-    attr[n].val.accessPolicyWindow.hitRatio = p->l2_hit_ratio;
-    attr[n].val.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    attr[n].val.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    ++n;
-  }
-  cfg.attrs = attr; cfg.numAttrs = n;
-}
-
-// Keep the activation scratch in the persisting part of L2 (0 = off).  Sets the device's persisting-L2 carve-out to
-// what the scratch needs (capped by the device maximum) -- a device-wide setting, hence opt-in.
-extern "C" int tdmpc2_planner_set_l2_persist(tdmpc2_planner* p, int enable) {
-  if (!p) return fail(TDMPC2_ERR_INVALID, "null planner");
-  if (!p->bound) return fail(TDMPC2_ERR_STATE, "tdmpc2_planner_bind must be called first");
-  if (!enable) { p->l2_window_bytes = 0; return 0; }
-  int dev = 0, max_persist = 0, max_window = 0;
-  CUDA_TRY(cudaGetDevice(&dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, dev));
-  const size_t scratch = p->off_raw - p->off_X;              // X planes + H planes of all slots
-  if (max_persist <= 0 || max_window <= 0) return fail(TDMPC2_ERR_UNSUPPORTED, "device has no persisting L2");
-  const size_t carve = std::min<size_t>(scratch, static_cast<size_t>(max_persist));
-  CUDA_TRY(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve));
-  p->l2_window_bytes = std::min<size_t>(scratch, static_cast<size_t>(max_window));
-  p->l2_hit_ratio = std::min(1.0f, static_cast<float>(carve) / static_cast<float>(p->l2_window_bytes));
   return 0;
 }
 
@@ -698,7 +636,7 @@ struct tdmpc2_pixel_encoder {
 extern "C" int tdmpc2_pixel_encoder_create(const tdmpc2_pixel_dims* dims, tdmpc2_pixel_encoder** out) {
   if (!dims || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
   const tdmpc2_pixel_dims& d = *dims;
-  if (d.num_envs < 1 || d.in_channels < 1 || d.num_channels < 8 || d.num_channels % 8 != 0 || d.simnorm_dim < 1 ||
+  if (d.in_channels < 1 || d.num_channels < 8 || d.num_channels % 8 != 0 || d.simnorm_dim < 1 ||
       (16 * d.num_channels) % d.simnorm_dim != 0)
     return fail(TDMPC2_ERR_INVALID, "pixel encoder: num_channels must be a positive multiple of 8 and simnorm_dim must divide 16 * num_channels");
   int num_sms = 0;
@@ -732,8 +670,14 @@ extern "C" int tdmpc2_pixel_encoder_workspace_bytes(const tdmpc2_pixel_encoder* 
 
 // One launch over `rows` frames: min(rows, SMs) CTAs, each looping over its frames with its own conv1 scratch slot.
 // tape != nullptr: the frames' post-ReLU maps are written to it as well (conv1 straight into the frame's slot).
-static int pixel_launch(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
-                        const float* shift, const float* grid_base, int64_t rows, float* z_out, float* tape, void* stream_) {
+extern "C" int tdmpc2_pixel_encode(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
+                                   const float* shift, const float* grid_base, int64_t rows, float* z_out, float* tape,
+                                   void* stream_) {
+  if (!e) {                        // an encoder exists only where a device does: report the missing device first
+    int n = 0;
+    const int rc = check_device(&n);
+    return rc ? rc : fail(TDMPC2_ERR_INVALID, "null pixel encoder");
+  }
   if (!workspace || !w || !frames || !shift || !grid_base || !z_out) return fail(TDMPC2_ERR_INVALID, "null argument");
   if (rows < 1) return fail(TDMPC2_ERR_INVALID, "rows must be >= 1");
   for (int i = 0; i < 4; ++i) if (!w->weight[i] || !w->bias[i]) return fail(TDMPC2_ERR_INVALID, "pixel encoder: null conv weight");
@@ -752,36 +696,12 @@ static int pixel_launch(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_c
   return 0;
 }
 
-extern "C" int tdmpc2_pixel_encode(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w, const float* frames,
-                                   const float* shift, const float* grid_base, float* z_out, void* stream_) {
-  if (!e) return fail(TDMPC2_ERR_INVALID, "null argument");
-  return pixel_launch(e, workspace, w, frames, shift, grid_base, e->d.num_envs, z_out, nullptr, stream_);
-}
-
-extern "C" int tdmpc2_pixel_encode_rows(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w,
-                                        const float* frames, const float* shift, const float* grid_base, int64_t rows,
-                                        float* z_out, void* stream_) {
-  if (!e) {                        // an encoder exists only where a device does: report the missing device first
-    int n = 0;
-    const int rc = check_device(&n);
-    return rc ? rc : fail(TDMPC2_ERR_INVALID, "null pixel encoder");
-  }
-  return pixel_launch(e, workspace, w, frames, shift, grid_base, rows, z_out, nullptr, stream_);
-}
-
 // ---- the conv encoder's backward (pixel_grad_kernels.cuh): taped forward, then the chain from dL/dz to the conv grads
 extern "C" int tdmpc2_pixel_encode_tape_bytes(const tdmpc2_pixel_encoder* e, int64_t rows, size_t* out) {
   if (!e || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
   if (rows < 1) return fail(TDMPC2_ERR_INVALID, "rows must be >= 1");
   *out = static_cast<size_t>(rows) * pix_tape_floats(e->d.num_channels) * 4;
   return 0;
-}
-
-extern "C" int tdmpc2_pixel_encode_taped(tdmpc2_pixel_encoder* e, void* workspace, const tdmpc2_conv_weights* w,
-                                         const float* frames, const float* shift, const float* grid_base, int64_t rows,
-                                         float* z_out, float* tape, void* stream_) {
-  if (!e || !tape) return fail(TDMPC2_ERR_INVALID, "null argument");
-  return pixel_launch(e, workspace, w, frames, shift, grid_base, rows, z_out, tape, stream_);
 }
 
 // Workspace of the backward (floats): the data gradients dp4 [rows][16 nc], dp3 [rows][nc 36], dp2 [rows][nc 169],
@@ -1354,7 +1274,7 @@ static int wm_dims_ok(const tdmpc2_planner* p, int H, int B) {
 static int wm_needs_encoder(const tdmpc2_planner* p) {
   if (p->num_enc == 0)
     return fail(TDMPC2_ERR_UNSUPPORTED, "this planner has no state encoder (pixel model): use tdmpc2_wm_loss_forward_latent / "
-                                        "tdmpc2_wm_loss_backward_latent with tdmpc2_pixel_encode_taped / tdmpc2_pixel_encode_backward");
+                                        "tdmpc2_wm_loss_backward_latent with a taped tdmpc2_pixel_encode / tdmpc2_pixel_encode_backward");
   return 0;
 }
 

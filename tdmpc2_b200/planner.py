@@ -21,12 +21,10 @@ from . import _cabi
 from .config import Config, get_discount
 
 
-# GEMM engine of the CEM-iteration kernel (include/tdmpc2_b200.h, tdmpc2_engine); TDMPC2_B200_ENGINE overrides.  On sm_90a
-# "tcgen05pp", "tcgen05x2" and "tcgen05x2pf" run as "tcgen05" (the TMA + wgmma engine); "auto" picks among those names.
-DEFAULT_ENGINE = os.environ.get("TDMPC2_B200_ENGINE", "auto")
-# Reduction-segment knob of the C ABI (tdmpc2_planner_set_kseg); the wgmma engine adds every 64-element K-chunk with
-# round-to-nearest, so the value has no effect on this build.
-DEFAULT_KSEG = 2048
+# GEMM engine of the fused kernels (include/tdmpc2_b200.h, tdmpc2_engine); TDMPC2_B200_ENGINE overrides.  "tcgen05" is the
+# TMA + wgmma engine, "simt" the CUDA-core fp32 engine the tests compare it against.
+ENGINES = {"tcgen05": _cabi.ENGINE_TCGEN05, "simt": _cabi.ENGINE_SIMT}
+DEFAULT_ENGINE = os.environ.get("TDMPC2_B200_ENGINE", "tcgen05")
 
 
 @dataclass
@@ -169,6 +167,30 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
+def _linear(struct, get, prefix: str, ln: bool):
+    """A tdmpc2_linear / tdmpc2_linear_grad (`struct`) of the state-dict entries `prefix`.weight / .bias and, when the
+    layer has a LayerNorm (`ln`), .ln.weight / .ln.bias; `get(key)` returns the tensor of a key."""
+    keys = (".weight", ".bias") + ((".ln.weight", ".ln.bias") if ln else ())
+    return struct(*[_ptr(get(prefix + k)) for k in keys])
+
+
+def _conv(struct, get):
+    """A tdmpc2_conv_weights / tdmpc2_conv_grads (`struct`) of the Conv2d modules of layers.conv, Sequential indices 2, 4,
+    6, 8 (layers.py:136-150); `get(key)` returns the tensor of a state-dict key."""
+    c = struct()
+    for i, idx in enumerate((2, 4, 6, 8)):
+        c.weight[i], c.bias[i] = _ptr(get(f"_encoder.rgb.{idx}.weight")), _ptr(get(f"_encoder.rgb.{idx}.bias"))
+    return c
+
+
+def _fp32_copies(sd: Dict[str, torch.Tensor], device, keep: list):
+    """key -> a contiguous fp32 copy of sd[key] on `device`, appended to `keep` (the C call that reads it is asynchronous)."""
+    def get(k):
+        keep.append(sd[k].detach().to(device, torch.float32).contiguous())
+        return keep[-1]
+    return get
+
+
 class Planner:
     """Owns one tdmpc2_planner handle plus its packed weights and workspace."""
 
@@ -202,7 +224,7 @@ class Planner:
         self.pix = None
         if self.rgb:           # pixel observations: the conv encoder is its own small object (include/tdmpc2_b200.h)
             C_in = cfg.obs_shape["rgb"][0]
-            pd = _cabi.PixelDims(num_envs=self.E, in_channels=C_in, num_channels=cfg.num_channels, simnorm_dim=cfg.simnorm_dim)
+            pd = _cabi.PixelDims(in_channels=C_in, num_channels=cfg.num_channels, simnorm_dim=cfg.simnorm_dim)
             ph = C.c_void_p()
             with torch.cuda.device(self.device):
                 _cabi.check(self.lib.tdmpc2_pixel_encoder_create(C.byref(pd), C.byref(ph)))
@@ -216,17 +238,6 @@ class Planner:
             self.pix_grid = torch.linspace(-1.0 + eps, 1.0 - eps, 64 + 2 * 3, device=self.device, dtype=torch.float32)[:64].contiguous()
             self._conv = None
         self.set_engine(engine)
-        # TDMPC2_B200_L2_PERSIST=1: keep the activation scratch in the persisting part of L2 (device-wide carve-out)
-        self.l2_persist = os.environ.get("TDMPC2_B200_L2_PERSIST", "0") not in ("", "0")
-        if self.l2_persist:
-            with torch.cuda.device(self.device):
-                _cabi.check(self.lib.tdmpc2_planner_set_l2_persist(self.h, 1))
-        # reduction-segment knob (see include/tdmpc2_b200.h, tdmpc2_planner_set_kseg)
-        self.kseg = int(os.environ.get("TDMPC2_B200_KSEG", cfg.get("kseg", DEFAULT_KSEG)))
-        _cabi.check(self.lib.tdmpc2_planner_set_kseg(self.h, self.kseg))
-        if "TDMPC2_B200_HEAD_KSEG" in os.environ or cfg.get("head_kseg", None) is not None:
-            _cabi.check(self.lib.tdmpc2_planner_set_head_kseg(
-                self.h, int(os.environ.get("TDMPC2_B200_HEAD_KSEG", cfg.get("head_kseg", 512) or 0))))
         # arithmetic: 3 = fp32-parity (default); 1 = the declared NON-PARITY fast mode (see include/tdmpc2_b200.h)
         self.passes = int(os.environ.get("TDMPC2_B200_PASSES", cfg.get("passes", 3) or 3))
         _cabi.check(self.lib.tdmpc2_planner_set_passes(self.h, self.passes))
@@ -258,25 +269,17 @@ class Planner:
         except Exception:
             pass
 
-    def set_engine(self, engine: str) -> None:
+    def set_engine(self, engine: Optional[str]) -> None:
         engine = engine or DEFAULT_ENGINE
-        if engine == "auto":
-            tiles = self.E * ((self.cfg.num_samples + 127) // 128)
-            sms = torch.cuda.get_device_properties(self.device).multi_processor_count
-            engine = "tcgen05pp" if tiles <= sms else "tcgen05x2"
-        self.engine_name = engine
-        code = {"tcgen05": _cabi.ENGINE_TCGEN05, "simt": _cabi.ENGINE_SIMT, "tcgen05x2": _cabi.ENGINE_TCGEN05_2SM,
-                "tcgen05pp": _cabi.ENGINE_TCGEN05_PP, "tcgen05x2pf": _cabi.ENGINE_TCGEN05_2SM_PF}[engine]
-        _cabi.check(self.lib.tdmpc2_planner_set_engine(self.h, code))
+        if engine not in ENGINES:
+            raise ValueError(f"unknown engine {engine!r}: the engines are 'tcgen05' and 'simt'")
+        _cabi.check(self.lib.tdmpc2_planner_set_engine(self.h, ENGINES[engine]))
         self.engine = engine
 
     @property
     def iter_engine(self) -> str:
-        """The engine the CEM-iteration launches actually run (the requested one falls back when the model / batch
-        shape does not fit it)."""
-        code = int(self.lib.tdmpc2_planner_iter_engine(self.h))
-        return {_cabi.ENGINE_TCGEN05: "tcgen05", _cabi.ENGINE_SIMT: "simt", _cabi.ENGINE_TCGEN05_2SM: "tcgen05x2",
-                _cabi.ENGINE_TCGEN05_PP: "tcgen05pp", _cabi.ENGINE_TCGEN05_2SM_PF: "tcgen05x2pf"}.get(code, "?")
+        """The engine the planning launches run: "tcgen05" or "simt"."""
+        return self.engine
 
     @property
     def launches(self) -> int:
@@ -290,28 +293,14 @@ class Planner:
     def pack(self, sd: Dict[str, torch.Tensor]) -> None:
         """Pack a reference-layout state dict (tensors on any device) for the kernels."""
         cfg = self.cfg
-        f = lambda k: sd[k].detach().to(self.device, torch.float32).contiguous()
         keep = []
-
-        def lin(prefix):
-            w, b = f(prefix + ".weight"), f(prefix + ".bias")
-            keep.extend([w, b])
-            g = beta = None
-            if prefix + ".ln.weight" in sd:
-                g, beta = f(prefix + ".ln.weight"), f(prefix + ".ln.bias")
-                keep.extend([g, beta])
-            return _cabi.Linear(_ptr(w), _ptr(b), _ptr(g), _ptr(beta))
-
+        f = _fp32_copies(sd, self.device, keep)
+        lin = lambda prefix: _linear(_cabi.Linear, f, prefix, prefix + ".ln.weight" in sd)
         W = _cabi.Weights()
         n = 0
-        if self.rgb:       # layers.conv: Conv2d modules at Sequential indices 2, 4, 6, 8 (layers.py:136-150); used as they are
-            cw = _cabi.ConvWeights()
-            conv_keep = []
-            for i, idx in enumerate((2, 4, 6, 8)):
-                w_, b_ = f(f"_encoder.rgb.{idx}.weight"), f(f"_encoder.rgb.{idx}.bias")
-                conv_keep.extend([w_, b_])
-                cw.weight[i], cw.bias[i] = w_.data_ptr(), b_.data_ptr()
-            self._conv, self._conv_keep = cw, conv_keep
+        if self.rgb:       # the conv encoder reads these copies at every encode: they stay alive until the next pack
+            self._conv_keep = []
+            self._conv = _conv(_cabi.ConvWeights, _fp32_copies(sd, self.device, self._conv_keep))
         else:
             while f"_encoder.state.{n}.weight" in sd:
                 W.enc[n] = lin(f"_encoder.state.{n}")
@@ -325,9 +314,7 @@ class Planner:
             if cfg.episodic:
                 W.termination[i] = lin(f"_termination.{i}")      # world_model.py:28
         if cfg.multitask:
-            emb, masks = f("_task_emb.weight"), f("_action_masks")
-            keep.extend([emb, masks])
-            W.task_emb, W.action_masks = _ptr(emb), _ptr(masks)
+            W.task_emb, W.action_masks = _ptr(f("_task_emb.weight")), _ptr(f("_action_masks"))
         if self._tables is None:      # built once: torch.tensor() of host values is a synchronising copy
             self._tables = (discount_table(cfg, self.device),
                             torch.linspace(cfg.vmin, cfg.vmax, cfg.num_bins, device=self.device, dtype=torch.float32))  # math.py:80
@@ -346,29 +333,26 @@ class Planner:
             _cabi.check(self.lib.tdmpc2_plan_prologue(self.h, _ptr(obs), _ptr(task), _ptr(t0), _ptr(prev_mean),
                                                       _ptr(noise_prior), self._stream()))
 
-    def encode_pixels(self, frames, shift) -> torch.Tensor:
-        """z = encode(obs) for pixel observations: frames [E, C, 64, 64] (any dtype, values 0..255), shift [E, 2] -> the
-        planner's static latent buffer [E, L]."""
+    def encode_pixel_rows(self, frames, shift, out=None) -> torch.Tensor:
+        """z = encode(obs) for any number of pixel frames in one launch: frames [R, C, 64, 64] (any dtype, values 0..255),
+        shift [R, 2] (x, y) -> z [R, L], written to `out` (a contiguous [R, L] fp32 tensor) or to a fresh tensor."""
+        return self._pixel_encode(frames, shift, out, taped=False)[0]
+
+    def encode_pixel_rows_taped(self, frames, shift, out=None):
+        """encode_pixel_rows that also keeps the activations the conv backward needs: -> (z [R, L], tape).  z is
+        bit-identical to encode_pixel_rows's."""
+        return self._pixel_encode(frames, shift, out, taped=True)
+
+    def _pixel_encode(self, frames, shift, out, taped: bool):
         if self.pix is None or self._conv is None:
-            raise _cabi.CabiError("encode_pixels needs a cfg.obs == 'rgb' planner with packed weights")
-        frames = frames.to(self.device, torch.float32).contiguous()
-        self._keep_pix = [frames, shift]
+            raise _cabi.CabiError("pixel encoding needs a cfg.obs == 'rgb' planner with packed weights")
+        frames, shift, R = self._pixel_rows(frames, shift)
+        z = self._rows_out(R, self.cfg.latent_dim) if out is None else out
+        tape = self._scratch(self.lib.tdmpc2_pixel_encode_tape_bytes, self.pix, R) if taped else None
         with torch.cuda.device(self.device):
             _cabi.check(self.lib.tdmpc2_pixel_encode(self.pix, self.pix_ws.data_ptr(), C.byref(self._conv), _ptr(frames),
-                                                     _ptr(shift), _ptr(self.pix_grid), _ptr(self.pix_z), self._stream()))
-        return self.pix_z
-
-    def encode_pixel_rows(self, frames, shift) -> torch.Tensor:
-        """z = encode(obs) for any number of pixel frames in one launch: frames [R, C, 64, 64] (any dtype, values 0..255),
-        shift [R, 2] (x, y) -> a fresh z [R, L].  Bit-identical to encode_pixels for the same frame and shift."""
-        if self.pix is None or self._conv is None:
-            raise _cabi.CabiError("encode_pixel_rows needs a cfg.obs == 'rgb' planner with packed weights")
-        frames, shift, R = self._pixel_rows(frames, shift)
-        z = self._rows_out(R, self.cfg.latent_dim)
-        with torch.cuda.device(self.device):
-            _cabi.check(self.lib.tdmpc2_pixel_encode_rows(self.pix, self.pix_ws.data_ptr(), C.byref(self._conv), _ptr(frames),
-                                                          _ptr(shift), _ptr(self.pix_grid), R, _ptr(z), self._stream()))
-        return z
+                                                     _ptr(shift), _ptr(self.pix_grid), R, _ptr(z), _ptr(tape), self._stream()))
+        return z, tape
 
     def _pixel_rows(self, frames, shift):
         frames = frames.to(self.device, torch.float32).contiguous()      # ShiftAug's x.float() (layers.py:44)
@@ -379,23 +363,6 @@ class Planner:
                              f"{tuple(frames.shape)} and {tuple(shift.shape)}")
         return frames, shift, R
 
-    def encode_pixel_rows_taped(self, frames, shift, out=None):
-        """encode_pixel_rows that also keeps the activations the conv backward needs: -> (z [R, L], tape).  `out`: an
-        optional contiguous [R, L] fp32 tensor to write z into (e.g. zs[0] of the world-model loss).  z is bit-identical to
-        encode_pixel_rows's."""
-        if self.pix is None or self._conv is None:
-            raise _cabi.CabiError("encode_pixel_rows_taped needs a cfg.obs == 'rgb' planner with packed weights")
-        frames, shift, R = self._pixel_rows(frames, shift)
-        z = self._rows_out(R, self.cfg.latent_dim) if out is None else out
-        nb = C.c_size_t()
-        _cabi.check(self.lib.tdmpc2_pixel_encode_tape_bytes(self.pix, R, C.byref(nb)))
-        tape = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
-        with torch.cuda.device(self.device):
-            _cabi.check(self.lib.tdmpc2_pixel_encode_taped(self.pix, self.pix_ws.data_ptr(), C.byref(self._conv), _ptr(frames),
-                                                           _ptr(shift), _ptr(self.pix_grid), R, _ptr(z), _ptr(tape),
-                                                           self._stream()))
-        return z, tape
-
     def pixel_encode_backward(self, tensor, tape, frames, shift, z, dz, grads) -> None:
         """Adds dL/dparameter of the conv encoder to `grads` (the `.grad` tensors of `_encoder.rgb.{2,4,6,8}.{weight,bias}`
         by state-dict key), given dz = dL/dz [R, L] and the taped forward's tape and z on the same frames and shifts.
@@ -403,15 +370,9 @@ class Planner:
         if self.pix is None:
             raise _cabi.CabiError("pixel_encode_backward needs a cfg.obs == 'rgb' planner")
         frames, shift, R = self._pixel_rows(frames, shift)
-        W, G = _cabi.ConvWeights(), _cabi.ConvGrads()
-        for i, idx in enumerate((2, 4, 6, 8)):
-            k = f"_encoder.rgb.{idx}"
-            W.weight[i], W.bias[i] = _ptr(tensor(k + ".weight")), _ptr(tensor(k + ".bias"))
-            G.weight[i], G.bias[i] = _ptr(grads[k + ".weight"]), _ptr(grads[k + ".bias"])
+        W, G = _conv(_cabi.ConvWeights, tensor), _conv(_cabi.ConvGrads, grads.__getitem__)
         z, dz = z.reshape(R, -1).contiguous(), dz.reshape(R, -1).contiguous()
-        nb = C.c_size_t()
-        _cabi.check(self.lib.tdmpc2_pixel_backward_workspace_bytes(self.pix, R, C.byref(nb)))
-        ws = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        ws = self._scratch(self.lib.tdmpc2_pixel_backward_workspace_bytes, self.pix, R)
         with torch.cuda.device(self.device):
             _cabi.check(self.lib.tdmpc2_pixel_encode_backward(self.pix, C.byref(W), _ptr(frames), _ptr(shift), _ptr(self.pix_grid),
                                                               R, _ptr(tape), _ptr(z), _ptr(dz), C.byref(G), _ptr(ws),
@@ -455,7 +416,7 @@ class Planner:
         """prologue -> I x iter -> epilogue on the current stream (10 launches for I = 6)."""
         cfg, E, dev = self.cfg, self.E, self.device
         if self.rgb:
-            self.prologue_latent(self.encode_pixels(obs, noise.shift), task, t0, prev_mean, noise.prior)
+            self.prologue_latent(self.encode_pixel_rows(obs, noise.shift, out=self.pix_z), task, t0, prev_mean, noise.prior)
         else:
             self.prologue(obs, task, t0, prev_mean, noise.prior)
         if tr is not None:
@@ -559,7 +520,7 @@ class Planner:
                 nz.prior[0, t] = torch.randn(P, A, **kw)
             main.wait_event(side.record_event())
         if self.rgb:
-            self.prologue_latent(self.encode_pixels(obs, nz.shift), task, t0, prev_mean, nz.prior)
+            self.prologue_latent(self.encode_pixel_rows(obs, nz.shift, out=self.pix_z), task, t0, prev_mean, nz.prior)
         else:
             self.prologue(obs, task, t0, prev_mean, nz.prior)
         for it in range(I):
@@ -603,7 +564,6 @@ class Planner:
     # Inputs are [rows, .] fp32 and task [rows] int32 | None, contiguous on self.device; outputs are fresh tensors.
     def pack_target_q(self, sd: Dict[str, torch.Tensor]) -> None:
         """Pack `_target_Qs_params.*` of a reference-layout state dict into the target blob (allocated on first use)."""
-        f = lambda k: sd[k].detach().to(self.device, torch.float32).contiguous()
         with torch.cuda.device(self.device):
             if self.target_blob is None:
                 nb = C.c_size_t()
@@ -612,13 +572,10 @@ class Planner:
                 _cabi.check(self.lib.tdmpc2_planner_bind_target_q(self.h, blob.data_ptr()))
                 self.target_blob = blob
             keep, lins = [], (_cabi.Linear * 3)()
+            f = _fp32_copies(sd, self.device, keep)
             for i in range(3):
                 pfx = f"_target_Qs_params.{i}"
-                t = [f(pfx + ".weight"), f(pfx + ".bias")]
-                if pfx + ".ln.weight" in sd:
-                    t += [f(pfx + ".ln.weight"), f(pfx + ".ln.bias")]
-                keep.extend(t)
-                lins[i] = _cabi.Linear(*[x.data_ptr() for x in t])
+                lins[i] = _linear(_cabi.Linear, f, pfx, pfx + ".ln.weight" in sd)
             stream = torch.cuda.current_stream(self.device)
             _cabi.check(self.lib.tdmpc2_pack_target_q(self.h, lins, stream.cuda_stream))
             for t in keep:            # `keep` tensors may be freed now: their memory is not reused before the pack ran
@@ -626,6 +583,12 @@ class Planner:
 
     def _rows_out(self, *shape) -> torch.Tensor:
         return torch.empty(*shape, device=self.device, dtype=torch.float32)
+
+    def _scratch(self, query, *args) -> torch.Tensor:
+        """An fp32 tape or workspace of the size a `*_bytes` query of the C ABI reports for `args`."""
+        nb = C.c_size_t()
+        _cabi.check(query(*args, C.byref(nb)))
+        return torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
 
     def wm_encode(self, obs, task) -> torch.Tensor:
         z = self._rows_out(obs.shape[0], self.cfg.latent_dim)
@@ -683,9 +646,7 @@ class Planner:
         """update_pi's forward on z [rows, L]: -> tape, action [rows, A], q [rows, 1], [rows, 2] = (gaussian log-prob,
         sum of the squash terms).  drop: Q layer 0's dropout scale [num_q, rows, M] or None."""
         R = z.shape[0]
-        nb = C.c_size_t()
-        _cabi.check(self.lib.tdmpc2_pi_loss_tape_bytes(self.h, R, C.byref(nb)))
-        tape = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        tape = self._scratch(self.lib.tdmpc2_pi_loss_tape_bytes, self.h, R)
         act, q, lp = self._rows_out(R, self.cfg.action_dim), self._rows_out(R, 1), self._rows_out(R, 2)
         with torch.cuda.device(self.device):
             _cabi.check(self.lib.tdmpc2_pi_loss_forward(self.h, _ptr(z), _ptr(task), _ptr(eps), _ptr(qidx), _ptr(drop), R,
@@ -697,20 +658,15 @@ class Planner:
         multi-task models, to `emb_grad`.  `tensor(key)` returns the model's fp32 tensor of a state-dict key."""
         W = _cabi.Weights()
         for i in range(3):
-            for pfx, dst in (("_pi", W.pi), ("_Qs.params", W.qs)):
-                k = f"{pfx}.{i}"
-                ln = i < 2
-                dst[i] = _cabi.Linear(_ptr(tensor(k + ".weight")), _ptr(tensor(k + ".bias")),
-                                      _ptr(tensor(k + ".ln.weight")) if ln else None, _ptr(tensor(k + ".ln.bias")) if ln else None)
+            W.pi[i] = _linear(_cabi.Linear, tensor, f"_pi.{i}", i < 2)
+            W.qs[i] = _linear(_cabi.Linear, tensor, f"_Qs.params.{i}", i < 2)
         G = _cabi.PiGrads()
         for i in range(3):
             G.weight[i], G.bias[i] = _ptr(grads[f"_pi.{i}.weight"]), _ptr(grads[f"_pi.{i}.bias"])
             if i < 2:
                 G.ln_weight[i], G.ln_bias[i] = _ptr(grads[f"_pi.{i}.ln.weight"]), _ptr(grads[f"_pi.{i}.ln.bias"])
         G.task_emb = _ptr(emb_grad)
-        nb = C.c_size_t()
-        _cabi.check(self.lib.tdmpc2_pi_loss_workspace_bytes(self.h, max(1, T * B), C.byref(nb)))
-        ws = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        ws = self._scratch(self.lib.tdmpc2_pi_loss_workspace_bytes, self.h, max(1, T * B))
         with torch.cuda.device(self.device):
             _cabi.check(self.lib.tdmpc2_pi_loss_backward(self.h, C.byref(W), _ptr(tape), _ptr(z), _ptr(task), _ptr(eps),
                                                          _ptr(qidx), _ptr(drop), T, B, _ptr(scale), float(entropy_coef),
@@ -721,9 +677,7 @@ class Planner:
         -> tape, zs [H + 1, B, L], Q logits [num_q, H B, num_bins], reward logits [H B, num_bins], termination logits
         [H B, 1] (episodic models) or None."""
         cfg, R = self.cfg, H * B
-        nb = C.c_size_t()
-        _cabi.check(self.lib.tdmpc2_wm_loss_tape_bytes(self.h, H, B, C.byref(nb)))
-        tape = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        tape = self._scratch(self.lib.tdmpc2_wm_loss_tape_bytes, self.h, H, B)
         zs = self._rows_out(H + 1, B, cfg.latent_dim)
         ql, rl = self._rows_out(cfg.num_q, R, cfg.num_bins), self._rows_out(R, cfg.num_bins)
         tl = self._rows_out(R, 1) if cfg.episodic else None
@@ -736,9 +690,7 @@ class Planner:
         """wm_loss_forward for a latent z_0 the caller wrote into zs[0] (pixel models: encode_pixel_rows_taped(..., out=zs[0])):
         zs [H + 1, B, L] fp32 contiguous, filled in place -> tape, zs, Q logits, reward logits, termination logits | None."""
         cfg, R = self.cfg, H * B
-        nb = C.c_size_t()
-        _cabi.check(self.lib.tdmpc2_wm_loss_tape_bytes(self.h, H, B, C.byref(nb)))
-        tape = torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
+        tape = self._scratch(self.lib.tdmpc2_wm_loss_tape_bytes, self.h, H, B)
         ql, rl = self._rows_out(cfg.num_q, R, cfg.num_bins), self._rows_out(R, cfg.num_bins)
         tl = self._rows_out(R, 1) if cfg.episodic else None
         with torch.cuda.device(self.device):
@@ -749,35 +701,23 @@ class Planner:
     def _wm_loss_structs(self, tensor, grads):
         """(weights, grads, coefficients) structs of the world-model loss's backward."""
         cfg = self.cfg
-
-        def lin(k, ln):
-            return _cabi.Linear(_ptr(tensor(k + ".weight")), _ptr(tensor(k + ".bias")),
-                                _ptr(tensor(k + ".ln.weight")) if ln else None, _ptr(tensor(k + ".ln.bias")) if ln else None)
-
-        def glin(k, ln):
-            return _cabi.LinearGrad(_ptr(grads[k + ".weight"]), _ptr(grads[k + ".bias"]),
-                                    _ptr(grads[k + ".ln.weight"]) if ln else None, _ptr(grads[k + ".ln.bias"]) if ln else None)
+        both = lambda k, ln: (_linear(_cabi.Linear, tensor, k, ln), _linear(_cabi.LinearGrad, grads.__getitem__, k, ln))
         W, G = _cabi.Weights(), _cabi.WmGrads()
         n = 0
         while f"_encoder.state.{n}.weight" in grads:
-            W.enc[n], G.enc[n] = lin(f"_encoder.state.{n}", True), glin(f"_encoder.state.{n}", True)
+            W.enc[n], G.enc[n] = both(f"_encoder.state.{n}", True)
             n += 1
         W.num_enc = G.num_enc = n
         for i in range(3):
-            W.dynamics[i], G.dynamics[i] = lin(f"_dynamics.{i}", True), glin(f"_dynamics.{i}", True)
-            W.reward[i], G.reward[i] = lin(f"_reward.{i}", i < 2), glin(f"_reward.{i}", i < 2)
-            W.qs[i], G.qs[i] = lin(f"_Qs.params.{i}", i < 2), glin(f"_Qs.params.{i}", i < 2)
+            W.dynamics[i], G.dynamics[i] = both(f"_dynamics.{i}", True)
+            W.reward[i], G.reward[i] = both(f"_reward.{i}", i < 2)
+            W.qs[i], G.qs[i] = both(f"_Qs.params.{i}", i < 2)
             if cfg.episodic:
-                W.termination[i], G.termination[i] = lin(f"_termination.{i}", i < 2), glin(f"_termination.{i}", i < 2)
+                W.termination[i], G.termination[i] = both(f"_termination.{i}", i < 2)
         G.task_emb = _ptr(grads.get("_task_emb.weight"))
         cf = _cabi.WmLossCoefs(cfg.consistency_coef, cfg.reward_coef, cfg.value_coef, cfg.termination_coef, cfg.rho,
                                cfg.vmin, cfg.vmax, cfg.bin_size)
         return W, G, cf
-
-    def _wm_loss_workspace(self, H, B):
-        nb = C.c_size_t()
-        _cabi.check(self.lib.tdmpc2_wm_loss_workspace_bytes(self.h, H, B, C.byref(nb)))
-        return torch.empty(nb.value // 4, device=self.device, dtype=torch.float32)
 
     def wm_loss_backward(self, tensor, tape, obs0, action, task, drop, H, B, zs, ql, rl, tl, next_z, reward, td_target,
                          terminated, grads):
@@ -785,7 +725,7 @@ class Planner:
         `_dynamics.*`, `_reward.*`, `_termination.*`, `_Qs.params.*`, `_task_emb.weight`).  `tensor(key)` returns the
         model's fp32 tensor of a state-dict key."""
         W, G, cf = self._wm_loss_structs(tensor, grads)
-        ws = self._wm_loss_workspace(H, B)
+        ws = self._scratch(self.lib.tdmpc2_wm_loss_workspace_bytes, self.h, H, B)
         with torch.cuda.device(self.device):
             _cabi.check(self.lib.tdmpc2_wm_loss_backward(
                 self.h, C.byref(W), _ptr(tape), _ptr(obs0), _ptr(action), _ptr(task), _ptr(drop), H, B, _ptr(zs), _ptr(ql),
@@ -797,7 +737,7 @@ class Planner:
         """wm_loss_backward without the state encoder (`_encoder.*` of `grads` is not touched) -> dL/dz_0 [B, L], for
         pixel_encode_backward."""
         W, G, cf = self._wm_loss_structs(tensor, grads)
-        ws = self._wm_loss_workspace(H, B)
+        ws = self._scratch(self.lib.tdmpc2_wm_loss_workspace_bytes, self.h, H, B)
         dz0 = self._rows_out(B, self.cfg.latent_dim)
         with torch.cuda.device(self.device):
             _cabi.check(self.lib.tdmpc2_wm_loss_backward_latent(

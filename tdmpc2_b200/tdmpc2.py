@@ -141,7 +141,7 @@ class TDMPC2(torch.nn.Module):
         pl = self.planner
         if rgb:                                                                     # ShiftAug's draw comes first (layers.py:55)
             shift = torch.randint(0, 7, (E, 2), device=dev, dtype=torch.float32, generator=self.generator)
-            z = pl.encode_pixels(obs, shift)
+            z = pl.encode_pixel_rows(obs, shift)
         else:
             z = pl.wm_encode(obs, taskv)
         if eval_mode:
@@ -300,7 +300,7 @@ class TDMPC2(torch.nn.Module):
         run as taped row launches (tdmpc2_wm_loss_forward), the backward chain of grad_kernels.cuh ADDS the gradients of
         the world-model loss to `.grad` as autograd would; then torch's clip_grad_norm_ and optim.step(), update_pi on the
         detached latents, and the Polyak update of the target Q ensemble.  Pixel models encode obs[0] with a taped conv
-        forward into zs[0] (tdmpc2_pixel_encode_taped, tdmpc2_wm_loss_forward_latent), and dL/dz_0 runs through the conv
+        forward into zs[0] (a taped tdmpc2_pixel_encode, tdmpc2_wm_loss_forward_latent), and dL/dz_0 runs through the conv
         backward of pixel_grad_kernels.cuh into `.grad` of `_encoder.rgb.*`.
         Draws from self.generator in the reference's order: pixel models' ShiftAug shifts of obs[1:] (H draws of (B, 2)),
         the TD target's pi noise and Q pair (`td_eps` [H, B, A], `td_qidx` [2]), pixel models' shift of obs[0], the

@@ -33,6 +33,7 @@ def test_struct_layout_matches_header():
     from tdmpc2_b200 import _cabi
     assert C.sizeof(_cabi.Dims) == 18 * 4 + 5 * 4
     assert C.sizeof(_cabi.Linear) == 4 * 8
+    assert C.sizeof(_cabi.PixelDims) == 3 * 4
     assert C.sizeof(_cabi.Weights) == 8 + (_cabi.MAX_ENC_LAYERS + 12) * 32 + 4 * 8 + 3 * 32   # ... + termination[3]
 
 

@@ -144,7 +144,7 @@ def test_non_mpc_act_runs_the_policy_through_the_kernels():
         assert torch.all(got_eps[e, cfg.action_dims[task[e]]:] == 0)
 
 
-@pytest.mark.parametrize("wl,engine", [("c1", "tcgen05x2"), ("c1", "tcgen05"), ("tiny-mt", "tcgen05x2"), ("tiny-mt", "simt")])
+@pytest.mark.parametrize("wl,engine", [("c1", "tcgen05"), ("tiny-mt", "tcgen05"), ("tiny-mt", "simt")])
 def test_shared_latent_fold_only_reorders_the_sum(wl, engine, monkeypatch):
     """At rollout step 0 every sample row of an environment carries the same [z | emb] (z.repeat(N), tdmpc2.py:163): the
     prologue folds its product with reward.0 / dynamics.0 into a per-environment bias (zbias_kernel) and the t = 0
@@ -170,6 +170,21 @@ def test_shared_latent_fold_only_reorders_the_sum(wl, engine, monkeypatch):
         vals[fold] = tr["values"][:, 0].cpu()          # first iteration: identical inputs on both sides
     d = (vals["1"] - vals["0"]).abs().max().item()
     assert 0.0 < d < 2e-5, d                           # > 0: the fold really ran
+
+
+def test_only_the_two_engines_are_accepted():
+    """"tcgen05" and "simt" (codes 0 and 1) are the engines; the names and codes of the removed Blackwell-era engines are
+    errors, not aliases of "tcgen05"."""
+    from tdmpc2_b200.planner import Planner
+    cfg = workload("tiny", num_envs=1)
+    for name in ("auto", "tcgen05x2", "tcgen05pp", "tcgen05x2pf"):
+        with pytest.raises(ValueError, match="'tcgen05' and 'simt'"):
+            Planner(cfg, 1, "cuda:0", engine=name)
+    pl = Planner(cfg, 1, "cuda:0")
+    assert pl.iter_engine == "tcgen05"
+    for code in (2, 3, 4, 5):
+        assert pl.lib.tdmpc2_planner_set_engine(pl.h, code) == -1         # TDMPC2_ERR_INVALID
+    assert Planner(cfg, 1, "cuda:0", engine="simt").iter_engine == "simt"
 
 
 @pytest.mark.parametrize("wl", ["tiny", "tiny-mt", "tiny-rgb"])

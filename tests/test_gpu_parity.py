@@ -10,7 +10,7 @@ from helpers import stable_positions, boundary_separated
 
 pytestmark = pytest.mark.gpu
 
-ENGINES = ["simt", "tcgen05", "tcgen05x2"]
+ENGINES = ["simt", "tcgen05"]
 
 
 def _planner(cfg, E, engine, sd):
@@ -236,7 +236,7 @@ def test_tensor_core_engine_matches_oracle_and_simt_engine(perturb):
 TERM_MARGIN = 2e-5     # |termination logit| below this: the 0.5 decision is not well defined under ~1e-6 kernel error
 
 
-@pytest.mark.parametrize("engine", ["simt", "tcgen05", "tcgen05x2"])
+@pytest.mark.parametrize("engine", ["simt", "tcgen05"])
 @pytest.mark.parametrize("wl,E", [("tiny", 2), ("c1", 2)])
 def test_episodic_plan_matches_oracle(engine, wl, E):
     """Episodic models run the termination head on z_{t+1} inside the fused rollout and carry the sticky

@@ -17,7 +17,7 @@ def _frames(cfg, E, seed):
 
 
 @pytest.mark.parametrize("E", [1, 5])
-def test_pixel_encoder_matches_oracle(E):
+def test_encode_pixel_rows_matches_oracle(E):
     """z = encode(frames) for every shift pair the reference can draw on some environment: 1e-5 (the convolutions are exact
     fp32 products summed in a different order than ATen's; SimNorm outputs are <= 1)."""
     from oracle.plan_oracle import OracleModel
@@ -29,7 +29,7 @@ def test_pixel_encoder_matches_oracle(E):
     want = OracleModel(cfg, sd).encode_rgb(frames, shift)
     pl = Planner(cfg, E, "cuda:0")
     pl.pack(sd)
-    got = pl.encode_pixels(frames.cuda(), shift.cuda()).cpu()
+    got = pl.encode_pixel_rows(frames.cuda(), shift.cuda(), out=pl.pix_z).cpu()
     torch.cuda.synchronize()
     assert got.shape == (E, cfg.latent_dim)
     assert torch.allclose(got, want, atol=1e-5, rtol=0), (got - want).abs().max()

@@ -40,7 +40,7 @@ def test_generator_statistics_and_determinism():
     assert abs(float((x * _dump(lib, st, 5, 0, n // 4)).mean())) < 0.005                           # another stream
 
 
-@pytest.mark.parametrize("wl,engine", [("c1", "tcgen05pp"), ("c1", "tcgen05x2"), ("tiny-mt", "tcgen05x2"), ("tiny-wide", "tcgen05x2")])
+@pytest.mark.parametrize("wl,engine", [("c1", "tcgen05"), ("tiny-mt", "tcgen05"), ("tiny-wide", "tcgen05")])
 def test_in_kernel_noise_is_consistent_between_action_pass_and_refit(wl, engine):
     from tdmpc2_b200.planner import Planner, draw_noise
     E = 2

@@ -1,6 +1,6 @@
 """Pixel-model `encode` on batches of frames without a GPU: the oracle against fixtures minted from the reference's own
 `WorldModel.encode` on [T, B, C, 64, 64] frames followed by `_td_target` (oracle/wm_rgb_oracle.py), ShiftAug's
-draw order, and the row-batched C entry point's no-device failure."""
+draw order, and the C entry point's no-device failure."""
 import pytest
 import torch
 
@@ -40,20 +40,22 @@ def test_draw_helper_reproduces_shiftaug_draws(name):
         assert torch.equal(got, want), batch
 
 
-def test_pixel_encode_rows_exported():
+def test_single_pixel_encode_call_exported():
     from tdmpc2_b200 import build, _cabi
     build.build()
     lib = _cabi.load()
-    assert "tdmpc2_pixel_encode_rows" in _cabi.SYMBOLS and hasattr(lib, "tdmpc2_pixel_encode_rows")
-    assert lib.tdmpc2_abi_version() == _cabi.ABI_VERSION == 7
+    assert "tdmpc2_pixel_encode" in _cabi.SYMBOLS and hasattr(lib, "tdmpc2_pixel_encode")
+    for old in ("tdmpc2_pixel_encode_rows", "tdmpc2_pixel_encode_taped"):     # ABI 8 merged them into tdmpc2_pixel_encode
+        assert old not in _cabi.SYMBOLS and not hasattr(lib, old), old
+    assert lib.tdmpc2_abi_version() == _cabi.ABI_VERSION == 8
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
-def test_pixel_encode_rows_needs_a_device():
+def test_single_pixel_encode_call_needs_a_device():
     from tdmpc2_b200 import build, _cabi
     build.build()
     lib = _cabi.load()
-    assert lib.tdmpc2_pixel_encode_rows(None, None, None, None, None, None, 1, None, None) == -2   # TDMPC2_ERR_NO_DEVICE
+    assert lib.tdmpc2_pixel_encode(None, None, None, None, None, None, 1, None, None, None) == -2   # TDMPC2_ERR_NO_DEVICE
     assert b"no CUDA device" in lib.tdmpc2_last_error()
 
 

@@ -79,9 +79,9 @@ def lib():
     return _cabi.load()
 
 
-def test_world_model_entry_points_exported(lib):
+def test_world_model_entry_points_exported_by_abi_8(lib):
     from tdmpc2_b200 import _cabi
-    assert _cabi.ABI_VERSION == 7 and lib.tdmpc2_abi_version() == 7
+    assert _cabi.ABI_VERSION == 8 and lib.tdmpc2_abi_version() == 8
     for s in NEW_SYMBOLS:
         assert s in _cabi.SYMBOLS and hasattr(lib, s), s
 
