@@ -1,9 +1,10 @@
 """Online training throughput: OnlineTrainer on a toy environment with c1's shapes (state obs 223, A = 38, the 5M preset,
 B = 256, H = 3), at E = 1 and E = 16 environments in lock-step.
 
-    python scripts/bench_train.py [--envs 1 16] [--seed-steps 511] [--measure-steps 320] [--warm-acts 4]
+    python scripts/bench_train.py [--envs 1 16] [--seed-steps 511] [--measure-steps 320] [--warm-acts 4] [--compile]
 
-Each E runs twice from the same seeds.
+Each E runs twice from the same seeds.  With --compile, each E runs three times: untimed without and with cfg.compile
+(every update a CUDA-graph replay after its first two calls), then split with cfg.compile.
   untimed  trainer.train() as a user runs it; the window opens at the `--warm-acts`-th training act() (the act graph and
            every update shape are warm by then) and closes when train() returns, each end behind a device synchronise.
            Reports env steps per second in the window.
@@ -88,9 +89,9 @@ class Clock:
         return call
 
 
-def run(E, split, args):
+def run(E, split, args, compile_=False):
     cfg = workload("c1", num_envs=E, batch_size=256, horizon=3, episode_length=LENGTH, seed_steps=args.seed_steps,
-                   steps=args.seed_steps + args.measure_steps, eval_freq=10 ** 9, eval_episodes=1)
+                   steps=args.seed_steps + args.measure_steps, eval_freq=10 ** 9, eval_episodes=1, compile=compile_)
     set_seed(1)
     agent = TDMPC2(cfg, device="cuda")
     agent.generator = torch.Generator("cuda").manual_seed(2)
@@ -126,6 +127,7 @@ def main():
     ap.add_argument("--seed-steps", type=int, default=511)
     ap.add_argument("--measure-steps", type=int, default=320)
     ap.add_argument("--warm-acts", type=int, default=4)
+    ap.add_argument("--compile", action="store_true", help="also run with cfg.compile (the update as a CUDA graph)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_train.py times the H100 kernels: no CUDA device")
@@ -133,7 +135,11 @@ def main():
     print(info)
     out = {"gpu": info, "workload": "c1 shapes (obs 223, A 38, 5M), B 256, H 3", "seed_steps": args.seed_steps}
     for E in args.envs:
-        res = {"untimed": run(E, False, args), "split": run(E, True, args)}
+        if args.compile:
+            res = {"untimed": run(E, False, args), "untimed_compile": run(E, False, args, True),
+                   "split_compile": run(E, True, args, True)}
+        else:
+            res = {"untimed": run(E, False, args), "split": run(E, True, args)}
         print(f"E={E}: {res}", flush=True)
         out[f"E{E}"] = res
     print(json.dumps(out))

@@ -275,6 +275,8 @@ class Planner:
             raise ValueError(f"unknown engine {engine!r}: the engines are 'tcgen05' and 'simt'")
         _cabi.check(self.lib.tdmpc2_planner_set_engine(self.h, ENGINES[engine]))
         self.engine = engine
+        # captured training steps of the owning agent (TDMPC2._update_graphed, cfg.compile): their launches name the engine
+        self.update_graphs = {}
 
     @property
     def iter_engine(self) -> str:

@@ -52,6 +52,10 @@ class TDMPC2(torch.nn.Module):
         self._use_graph = bool(cfg.get("cuda_graph", True))   # replay the launch chain as one CUDA graph (cfg.compile's role)
         # one environment: interleave the reference-order noise draws with the launches instead (TDMPC2_B200_E1_GRAPH=1: A/B knob)
         self._e1_interleaved = bool(cfg.get("e1_interleaved", True)) and os.environ.get("TDMPC2_B200_E1_GRAPH", "0") in ("", "0")
+        # cfg.compile (tdmpc2.py:41-43): `_update` without explicit draws replays one CUDA graph of the whole step
+        self._compile = bool(cfg.get("compile", False))
+        self._update_warm = None     # (key, bindings) of the last graph-eligible eager call: the next call may capture
+        self.update_path = None      # how the last `_update` ran: "eager", "captured" (capture + first replay), "replayed"
         # the policy update (tdmpc2.py:26-30,41): Adam over the `_pi.*` parameters, and the running Q scale
         self.scale = RunningScale(cfg, self.device)
         self._pi_keys = [k for k in self.model.keys() if k.startswith("_pi.")]
@@ -307,14 +311,27 @@ class TDMPC2(torch.nn.Module):
         dropout scale of Q layer 0 for the value loss (`dropout_mask` [num_q, H, B, mlp_dim] of mask / (1 - p) values;
         the reference's vmap dropout stream is not replayed bit for bit), then update_pi's own (`pi_eps`, `pi_qidx`,
         `pi_dropout_mask`, see update_pi).  `shift` [H+1, B, 2] passes the shifts explicitly, shift[t] belonging to
-        obs[t].  Returns the reference's info dict."""
+        obs[t].  Returns the reference's info dict.
+
+        With cfg.compile, a call without explicit draws (all seven None, as in `update(buffer)`) replays a captured CUDA
+        graph of the whole step (`_update_graphed`); `update_path` tells which way a call ran."""
+        draws = (td_eps, td_qidx, dropout_mask, pi_eps, pi_qidx, pi_dropout_mask, shift)
+        if self._compile and self.device.type == "cuda" and all(x is None for x in draws):
+            return self._update_graphed(obs, action, reward, terminated, task)
+        self.update_path = "eager"
+        return self._update_step(obs, action, reward, terminated, task, td_eps=td_eps, td_qidx=td_qidx,
+                                 dropout_mask=dropout_mask, pi_eps=pi_eps, pi_qidx=pi_qidx, pi_dropout_mask=pi_dropout_mask,
+                                 shift=shift)
+
+    def _batch_dims(self, obs, action, reward, terminated, task):
+        """_update's checks of the batch (and of the device: there is no CPU fallback) -> (H, B)."""
         cfg, dev = self.cfg, self.device
         rgb = cfg.get("obs", "state") == "rgb"
         if rgb and dev.type != "cuda":
             raise NotImplementedError("pixel `_update` runs on the sm_90a conv encoder kernels: no CPU fallback")
         if dev.type != "cuda":
             raise RuntimeError("_update runs on the sm_90a kernels: the agent needs a CUDA device (there is no CPU fallback)")
-        A, L, M = cfg.action_dim, cfg.latent_dim, cfg.mlp_dim
+        A = cfg.action_dim
         if rgb:
             C_in = cfg.obs_shape["rgb"][0]
             if obs.ndim != 5 or obs.shape[0] < 2 or obs.shape[1] < 1 or tuple(obs.shape[2:]) != (C_in, 64, 64):
@@ -331,6 +348,15 @@ class TDMPC2(torch.nn.Module):
                 raise ValueError(f"{name} must be a floating-point tensor; got {x.dtype}")
         if not rgb and not obs.is_floating_point():
             raise ValueError(f"obs must be a floating-point tensor; got {obs.dtype}")
+        return H, B
+
+    def _update_step(self, obs, action, reward, terminated, task=None, *, td_eps=None, td_qidx=None, dropout_mask=None,
+                     pi_eps=None, pi_qidx=None, pi_dropout_mask=None, shift=None):
+        """The training step of `_update`, issued launch by launch (the eager path, and what a graph captures)."""
+        cfg, dev = self.cfg, self.device
+        rgb = cfg.get("obs", "state") == "rgb"
+        H, B = self._batch_dims(obs, action, reward, terminated, task)
+        A, L, M = cfg.action_dim, cfg.latent_dim, cfg.mlp_dim
         if shift is not None:
             if not rgb:
                 raise ValueError("shift applies to pixel models (cfg.obs == 'rgb')")
@@ -421,6 +447,99 @@ class TDMPC2(torch.nn.Module):
             info.update(_termination_statistics(torch.sigmoid(termination_pred[-1]), terminated[-1]))
         info.update(pi_info)
         return {k: v.detach().mean() if isinstance(v, torch.Tensor) else torch.tensor(v) for k, v in info.items()}
+
+    # ------------------------------------------------------------------ cfg.compile: the training step as one CUDA graph
+    def _graph_bindings(self):
+        """What a captured step reads or writes at addresses Python could rebind: the planner, the generator, both
+        optimisers' state (load_state_dict replaces it) and the carried `_task_emb.weight.grad` of multi-task models.
+        None when a `.grad` is set that an eager call would not have left (only the carried one is)."""
+        emb = self.model.tensor("_task_emb.weight") if self.cfg.multitask else None
+        for p in self.model.parameters():
+            if p.grad is not None and p is not emb:
+                return None
+        return (self._planner, self.generator, self.optim.state, self.pi_optim.state, None if emb is None else emb.grad)
+
+    def _update_graphed(self, obs, action, reward, terminated, task):
+        """`_update` with cfg.compile.  The first call for a key (batch shape, dtypes, task, engine, generator) runs
+        eagerly; it creates Adam's state, the target blob, the tables and the kernels' attributes.  The next call captures
+        the step with torch.cuda.graph over static copies of the inputs and replays it at once (the capture runs
+        nothing); later calls copy the inputs in and replay.  A new generator, `Planner.set_engine`, a rebound
+        `_task_emb.weight.grad` or an optimiser's load_state_dict drops the graph: the next call runs eagerly again.
+        The graph re-packs the weights from the parameters, so `load()` needs no recapture.  The returned dict holds
+        fresh tensors."""
+        H, B = self._batch_dims(obs, action, reward, terminated, task)
+        if (task is not None and not torch.is_tensor(task)) or (self.cfg.multitask and task is None):
+            self.update_path = "eager"          # a host task index (or none where one is needed): not graphed
+            return self._update_step(obs, action, reward, terminated, task)
+        pl = self._planner if self._planner is not None else self.planner      # a fresh agent's first call creates it
+        inputs = (obs, action, reward, terminated) + (() if task is None else (task,))
+        key = (H, B, tuple(x.dtype for x in inputs), None if task is None else tuple(task.shape), pl.engine,
+               id(self.generator))
+        bindings = self._graph_bindings()
+        same = lambda a, b: a is not None and b is not None and all(x is y for x, y in zip(a, b))
+        for k in [k for k, s in pl.update_graphs.items() if not same(s["bindings"], bindings)]:
+            del pl.update_graphs[k]             # it would touch memory that Python has rebound
+        st = pl.update_graphs.get(key)
+        if st is None and self._update_warm is not None and self._update_warm[0] == key and same(self._update_warm[1], bindings):
+            try:
+                st = self._capture_update(pl, key, inputs, bindings)
+            except RuntimeError as e:            # capture unsupported here: keep issuing the step launch by launch
+                import warnings
+                warnings.warn(f"CUDA-graph capture of the training step failed ({e}); updating eagerly")
+                self._compile = False
+                self.update_path = "eager"
+                return self._update_step(obs, action, reward, terminated, task)
+            return self._replay_update(pl, st, inputs, "captured")
+        if st is None:
+            self.update_path = "eager"
+            info = self._update_step(obs, action, reward, terminated, task)
+            self._update_warm = (key, self._graph_bindings())
+            return info
+        return self._replay_update(pl, st, inputs, "replayed")
+
+    def _capture_update(self, pl, key, inputs, bindings):
+        """Capture `_update_step` on static copies of `inputs` (caller's dtypes) from the state an eager call left."""
+        static = [torch.empty_like(x, device=self.device) for x in inputs]
+        emb = self.model.tensor("_task_emb.weight") if self.cfg.multitask else None
+        carried = None if emb is None else emb.grad      # the gradient update_pi leaves for the next step
+        self._weights_dirty, pl.target_version = True, None     # both re-packs go into the graph, whatever act() did
+        g = torch.cuda.CUDAGraph()
+        if self.generator is not None:                   # the default generator is registered by the capture itself
+            g.register_generator_state(self.generator)
+        n0 = pl.launches
+        try:
+            with torch.cuda.graph(g):
+                info = self._update_step(*static[:4], static[4] if len(static) > 4 else None)
+                if carried is not None:                  # zero_grad rebound it: write it back where the next replay reads
+                    carried.copy_(emb.grad)
+                dev_keys = [k for k, v in info.items() if v.is_cuda]
+                vec = torch.stack([info[k] for k in dev_keys])   # the info dict's device values, copied out in one go
+        except BaseException:
+            for p in self.model.parameters():            # leave the host state as the eager call before the capture did
+                p.grad = None
+            if emb is not None:
+                emb.grad = carried
+            self.model.eval()
+            self.sync_weights()
+            raise
+        if emb is not None:
+            emb.grad = carried
+        launches = pl.launches - n0
+        pl._graph_launches -= launches                   # the capture pass itself launched nothing
+        st = dict(graph=g, inputs=static, launches=launches, vec=vec, bindings=bindings,
+                  keys=[(k, dev_keys.index(k) if k in dev_keys else v) for k, v in info.items()])
+        pl.update_graphs[key] = st
+        return st
+
+    def _replay_update(self, pl, st, inputs, path):
+        for s, x in zip(st["inputs"], inputs):
+            s.copy_(x)
+        st["graph"].replay()
+        pl._graph_launches += st["launches"]
+        self.sync_weights()                              # as the step's Polyak update leaves it: both packs are stale
+        self.update_path = path
+        vec = st["vec"].clone()
+        return {k: vec[i] if isinstance(i, int) else i.clone() for k, i in st["keys"]}
 
     @torch.no_grad()
     def _td_target(self, next_z, reward, terminated, task, *, eps=None, qidx=None):
