@@ -42,7 +42,9 @@ def percentile_scale(x: torch.Tensor, value: torch.Tensor, tau: float) -> torch.
     return torch.lerp(value, torch.clamp(p[1] - p[0], min=1.0).to(value.dtype), tau)
 
 
-def _mlp(P, prefix, x, head=None, drop=None):
+def _mlp(P, prefix, x, head=None, drop=None, sub=None, split=False):
+    """`sub(i, x)` and `split` as in update_oracle._net."""
+    from oracle.update_oracle import split_act
     for i in range(3):
         w, b = P[f"{prefix}.{i}.weight"], P[f"{prefix}.{i}.bias"]
         g = P.get(f"{prefix}.{i}.ln.weight")
@@ -50,20 +52,28 @@ def _mlp(P, prefix, x, head=None, drop=None):
         if head is not None:
             w, b = w[head], b[head]
             g, beta = (None, None) if g is None else (g[head], beta[head])
-        x = F.linear(x, w, b)
+        x = F.linear(split_act(x) if split else x, w, b)
+        if g is not None and i == 0 and drop is not None:
+            x = x * drop                                           # nn.Dropout: x * (mask / (1 - p))
+        if sub is not None:
+            x = sub(i, x)
         if g is not None:
-            if i == 0 and drop is not None:
-                x = x * drop                                       # nn.Dropout: x * (mask / (1 - p))
             x = F.mish(F.layer_norm(x, (x.shape[-1],), g, beta, 1e-5))
     return x
 
 
 def update_pi_oracle(cfg, sd: Dict[str, torch.Tensor], zs, task, eps, qidx, drop=None, scale_value=1.0,
-                     dtype=torch.float32, steps_state=None):
+                     dtype=torch.float32, steps_state=None, tape=None, split=False):
     """One update_pi.  zs [T, B, L]; task [B] or None; eps [T, B, A]; qidx [2]; drop [num_q, T, B, M] or None;
     scale_value: RunningScale.value before the call.  Returns a dict: loss, grads (by key, before clipping; "_task_emb.weight"
     for multi-task models), grad_norm, scale (after), params (the `_pi.*` tensors after one Adam step), entropy,
-    scaled_entropy, q.  `steps_state`: an Adam state dict to continue from (successive steps)."""
+    scaled_entropy, q.  `steps_state`: an Adam state dict to continue from (successive steps).  `split`: every Linear
+    reads its input rounded as the kernels' forward stores it (update_oracle.split_act).
+
+    `tape`: the forward anchored on the kernels' (update_oracle.Tape), keys `_pi.<i>` (layer 2: the head's logits
+    [mean | log_std]), `act` (the action the Q heads read), `_Qs.<u>.<i>` for the head in slot u of qidx, and `scale`,
+    the running scale after its update, which replaces the percentile's.  The call returns after the backward: loss,
+    grads."""
     from oracle.plan_oracle import two_hot_inv
     P = {k: (v.detach().to(dtype).clone() if torch.is_tensor(v) and v.is_floating_point() else v) for k, v in sd.items()}
     for k in PI_KEYS:
@@ -78,7 +88,8 @@ def update_pi_oracle(cfg, sd: Dict[str, torch.Tensor], zs, task, eps, qidx, drop
             Wr = torch.where(n > 1, W * (1.0 / (n + 1e-7)), W)
         emb = (W + (Wr - W).detach())[task.long()].unsqueeze(0).expand(T, B, -1)
         x = torch.cat([zs, emb], dim=-1)
-    mean, log_std = _mlp(P, "_pi", x).chunk(2, dim=-1)
+    sub = (lambda key: None) if tape is None else tape.at
+    mean, log_std = _mlp(P, "_pi", x, sub=sub("_pi"), split=split).chunk(2, dim=-1)
     log_std = P["log_std_min"] + 0.5 * P["log_std_dif"] * (torch.tanh(log_std) + 1)
     if cfg.multitask:
         m = P["_action_masks"][task.long()].unsqueeze(0)
@@ -91,12 +102,17 @@ def update_pi_oracle(cfg, sd: Dict[str, torch.Tensor], zs, task, eps, qidx, drop
     action = torch.tanh(mean + eps * log_std.exp())
     log_pi = log_prob - torch.log(F.relu(1 - action.pow(2)) + 1e-6).sum(-1, keepdim=True)
     scaled_entropy = -log_pi * (scaled_log_prob / (log_pi + 1e-8))
-    xq = torch.cat([x, action], dim=-1)
+    # the Q heads read the taped action; the squash term is a function of the logits (the backward recomputes it)
+    xq = torch.cat([x, action if tape is None else tape("act", action)], dim=-1)
     heads = [int(h) for h in qidx]
-    Qs = [two_hot_inv(_mlp(P, "_Qs.params", xq, head=h, drop=None if drop is None else drop[h].to(dtype)), cfg) for h in heads]
+    Qs = [two_hot_inv(_mlp(P, "_Qs.params", xq, head=h, drop=None if drop is None else drop[h].to(dtype),
+                           sub=sub(f"_Qs.{u}"), split=split), cfg) for u, h in enumerate(heads)]
     q = (Qs[0] + Qs[1]) / 2
     value = torch.as_tensor(scale_value, dtype=torch.float32).reshape(1)
-    new_value = percentile_scale(q[0].detach().float(), value, cfg.tau)
+    if tape is not None:
+        new_value = tape.values["scale"].reshape(1)
+    else:
+        new_value = percentile_scale(q[0].detach().float(), value, cfg.tau)
     qs = q / new_value.to(dtype)
     rho = torch.pow(cfg.rho, torch.arange(T)).to(dtype)
     loss = (-(cfg.entropy_coef * scaled_entropy + qs).mean(dim=(1, 2)) * rho).mean()
@@ -105,6 +121,8 @@ def update_pi_oracle(cfg, sd: Dict[str, torch.Tensor], zs, task, eps, qidx, drop
     grads = {k: P[k].grad.detach().clone() for k in PI_KEYS}
     if cfg.multitask:
         grads["_task_emb.weight"] = P["_task_emb.weight"].grad.detach().clone()
+    if tape is not None:
+        return dict(loss=loss.detach(), grads=grads)
     norm = torch.nn.utils.clip_grad_norm_(params, cfg.grad_clip_norm)
     opt = torch.optim.Adam(params, lr=cfg.lr, eps=1e-5, capturable=False)
     if steps_state is not None:

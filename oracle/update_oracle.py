@@ -67,7 +67,30 @@ def split_act(x):
     return x + (hi + (x.detach() - hi).half().to(x.dtype) - x.detach())
 
 
-def _net(P, prefix, x, last, head=None, drop=None, V=8, split=False):
+class Tape:
+    """Forward values the kernels taped, substituted into an oracle's forward by key: a value the oracle computes is
+    replaced by the taped one while its derivative still comes from the graph (x + (taped - x).detach()), so that the
+    oracle's backward runs on the kernels' own forward and its error is the backward arithmetic's alone.  `got` keeps
+    what the oracle computed before each substitution (one layer on the kernels' input), by the same key."""
+
+    def __init__(self, values: Dict[str, torch.Tensor]):
+        self.values, self.got = values, {}
+
+    def __call__(self, key, x):
+        t = self.values.get(key)
+        if t is None:
+            return x
+        self.got[key] = x.detach()
+        return x + (t.to(x.dtype).reshape(x.shape) - x).detach()
+
+    def at(self, prefix):
+        """The `sub` of _net for the layers `prefix`.0, `prefix`.1, ..."""
+        return lambda i, x: self(f"{prefix}.{i}", x)
+
+
+def _net(P, prefix, x, last, head=None, drop=None, V=8, split=False, sub=None):
+    """`sub(i, x)`: the value of layer i's Linear (after the dropout scale of layer 0) -> the value the layer goes on
+    with (Tape.at)."""
     n = 0
     while f"{prefix}.{n}.weight" in P:
         n += 1
@@ -78,10 +101,12 @@ def _net(P, prefix, x, last, head=None, drop=None, V=8, split=False):
             w, b = w[head], b[head]
             g, beta = (None, None) if g is None else (g[head], beta[head])
         x = F.linear(split_act(x) if split else x, w, b)
+        if i == 0 and drop is not None and g is not None:
+            x = x * drop
+        if sub is not None:
+            x = sub(i, x)
         if g is None:
             continue
-        if i == 0 and drop is not None:
-            x = x * drop
         x = F.layer_norm(x, (x.shape[-1],), g, beta, 1e-5)
         if i < n - 1:
             x = F.mish(x)
@@ -94,13 +119,19 @@ def _net(P, prefix, x, last, head=None, drop=None, V=8, split=False):
 
 def update_oracle(cfg, sd: Dict[str, torch.Tensor], obs, action, reward, terminated, task, td_eps, td_qidx, drop,
                   pi_eps, pi_qidx, pi_drop, scale_value=1.0, dtype=torch.float32, emb_grad=None, adam_state=None,
-                  pi_adam_state=None, split=False):
+                  pi_adam_state=None, split=False, tape: Optional[Tape] = None):
     """One _update.  obs [H+1, B, obs_dim], action [H, B, A], reward / terminated [H, B, 1], task [B] or None;
     td_eps [H, B, A], td_qidx [2]; drop / pi_drop [num_q, H(+1), B, M] or None; pi_eps [H+1, B, A], pi_qidx [2].
     Returns a dict: the losses, grads (by key, before clipping), grad_norm, sd (the state dict after the step, the
     target soft update and update_pi), pi (update_pi_oracle's result), emb_grad (the embedding gradient update_pi
     leaves), adam / pi_adam states, zs.  `split`: every Linear of the world-model loss reads its input rounded as the
-    kernels' forward stores it (split_act), for a yardstick on the kernels' rounded operands."""
+    kernels' forward stores it (split_act), for a yardstick on the kernels' rounded operands.
+
+    `tape`: the world-model loss's forward anchored on the kernels' (Tape), a test of the backward alone.  Keys
+    `<prefix>.<i>` per Linear (`_encoder.state`, `_dynamics@<t>` for rollout step t, `_Qs.<h>` for head h, `_reward`,
+    `_termination`), `zs.<t>` per latent, and `next_z` / `td`, which replace the TD targets' computation.  A model
+    without a state encoder (pixels) starts from the leaf zs.0, whose gradient is returned as dz0.  The call returns
+    after the backward: the losses, grads, dz0."""
     P = {k: (v.detach().to(dtype).clone() if torch.is_tensor(v) and v.is_floating_point() else v) for k, v in sd.items()}
     for k in list(P):
         if k.startswith("_detach_Qs_params."):
@@ -111,26 +142,40 @@ def update_oracle(cfg, sd: Dict[str, torch.Tensor], obs, action, reward, termina
     if mt:
         renorm_rows(P["_task_emb.weight"], task)
     taskHB = task.long().unsqueeze(0).expand(H, B) if mt else None
-    with torch.no_grad():
-        wm = WMOracle(cfg, P, dtype)
-        next_z = wm.encode(obs[1:], taskHB)
-        td = wm.td_target(next_z, reward, terminated, taskHB, td_eps, td_qidx)
+    if tape is not None:
+        next_z, td = tape.values["next_z"].to(dtype), tape.values["td"].to(dtype)
+    else:
+        with torch.no_grad():
+            wm = WMOracle(cfg, P, dtype)
+            next_z = wm.encode(obs[1:], taskHB)
+            td = wm.td_target(next_z, reward, terminated, taskHB, td_eps, td_qidx)
+    sub = (lambda key: None) if tape is None else tape.at
+    at = (lambda key, x: x) if tape is None else tape
+    latent = "_encoder.state.0.weight" not in P
 
-    keys = [k for g in wm_groups(cfg, list(sd.keys())) for k in g]
+    keys = [k for g in wm_groups(cfg, list(sd.keys())) for k in g if not (latent and k.startswith("_encoder."))]
     for k in keys:
         P[k].requires_grad_(True)
     cat = (lambda x, t: torch.cat([x, P["_task_emb.weight"][t.long()]], dim=-1)) if mt else (lambda x, t: x)
-    z = _net(P, "_encoder.state", cat(obs[0], task), "simnorm", V=cfg.simnorm_dim, split=split)
+    if latent:
+        assert tape is not None, "a model without a state encoder needs its taped z_0"
+        z = tape.values["zs.0"].to(dtype).reshape(B, cfg.latent_dim).requires_grad_(True)
+    else:
+        z = at("zs.0", _net(P, "_encoder.state", cat(obs[0], task), "simnorm", V=cfg.simnorm_dim, split=split,
+                            sub=sub("_encoder.state")))
+    z0 = z
     zs, cons = [z], 0
     for t in range(H):
-        z = _net(P, "_dynamics", torch.cat([cat(z, task), action[t]], dim=-1), "simnorm", V=cfg.simnorm_dim, split=split)
+        z = _net(P, "_dynamics", torch.cat([cat(z, task), action[t]], dim=-1), "simnorm", V=cfg.simnorm_dim, split=split,
+                 sub=sub(f"_dynamics@{t}"))
+        z = at(f"zs.{t + 1}", z)
         cons = cons + F.mse_loss(z, next_z[t]) * cfg.rho ** t
         zs.append(z)
     Z = torch.stack(zs)
     x = torch.cat([cat(Z[:-1], taskHB), action], dim=-1)
-    qs = torch.stack([_net(P, QS[:-1], x, "none", head=h, drop=None if drop is None else drop[h].to(dtype), split=split)
-                      for h in range(cfg.num_q)])
-    rp = _net(P, "_reward", x, "none", split=split)
+    qs = torch.stack([_net(P, QS[:-1], x, "none", head=h, drop=None if drop is None else drop[h].to(dtype), split=split,
+                           sub=sub(f"_Qs.{h}")) for h in range(cfg.num_q)])
+    rp = _net(P, "_reward", x, "none", split=split, sub=sub("_reward"))
     rew_loss, val_loss = 0, 0
     for t in range(H):
         rew_loss = rew_loss + soft_ce(rp[t], reward[t], cfg).mean() * cfg.rho ** t
@@ -138,16 +183,21 @@ def update_oracle(cfg, sd: Dict[str, torch.Tensor], obs, action, reward, termina
             val_loss = val_loss + soft_ce(qs[h, t], td[t], cfg).mean() * cfg.rho ** t
     cons, rew_loss, val_loss = cons / H, rew_loss / H, val_loss / (H * cfg.num_q)
     if cfg.episodic:
-        term_pred = _net(P, "_termination", Z[1:], "none", split=split)
+        term_pred = _net(P, "_termination", Z[1:], "none", split=split, sub=sub("_termination"))
         term_loss = F.binary_cross_entropy_with_logits(term_pred, terminated)
     else:
         term_loss = torch.zeros((), dtype=dtype)
     total = (cfg.consistency_coef * cons + cfg.reward_coef * rew_loss + cfg.termination_coef * term_loss
              + cfg.value_coef * val_loss)
+    if tape is not None:
+        z0.retain_grad()
     total.backward()
     if mt and emb_grad is not None:
         P["_task_emb.weight"].grad += emb_grad.to(dtype)
     grads = {k: P[k].grad.detach().clone() for k in keys}
+    if tape is not None:
+        return dict(consistency_loss=cons.detach(), reward_loss=rew_loss.detach(), value_loss=val_loss.detach(),
+                    termination_loss=term_loss.detach(), total_loss=total.detach(), grads=grads, dz0=z0.grad.detach())
     params = [P[k] for k in keys]
     norm = torch.nn.utils.clip_grad_norm_(params, cfg.grad_clip_norm)
     groups = wm_groups(cfg, list(sd.keys()))

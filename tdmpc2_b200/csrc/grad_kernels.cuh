@@ -13,7 +13,9 @@
 //   gemm_f32 / pl_reduce / pl_colsum / pl_emb_grad   dW, db, dgamma, dbeta of pi layers 2 -> 0 and the embedding
 //
 // Arithmetic is fp32 FFMA; weights are the fp32 state-dict tensors.  Every reduction over rows runs in a fixed order
-// (split-K partials summed split by split, column sums row by row): two calls on the same inputs give the same bits.
+// (split-K partials summed split by split, GEMM K tiles and column sums in fixed blocks): two calls on the same inputs
+// give the same bits.  Long sums are blocked so that an output's rounding chain stays short: a plain running sum over
+// R rows carries ~R roundings, far more than the blocked sums of a float64-checked reference at R in the thousands.
 // Nothing allocates or synchronises with the host, so the chain can be captured in a CUDA graph.
 #pragma once
 #include <cuda_runtime.h>
@@ -24,7 +26,8 @@ namespace tdmpc2 {
 // ------------------------------------------------------------------------------------ generic fp32 GEMM
 // C[i, j] = sum_k A(i, k) B(k, j) over the batch blockIdx.z / nsplit and the K range of split blockIdx.z % nsplit;
 // A(i, k) = A[i * a_i + k * a_k], B(k, j) = B[k * b_k + j * b_j].  Batch z offsets A, C by z * a_z, z * c_z and B by
-// (bsel ? bsel[z] : z) * b_z; split s writes its partial sum at C + s * c_s.  Each output is one thread's k loop.
+// (bsel ? bsel[z] : z) * b_z; split s writes its partial sum at C + s * c_s.  Each output is one thread's k loop, summed
+// per K tile, then the tile sums in order.
 struct GemmArgs {
   const float* A; long long a_i, a_k, a_z;
   const float* B; long long b_k, b_j, b_z; const int* bsel;
@@ -60,6 +63,7 @@ __global__ void __launch_bounds__(256) gemm_f32(const GemmArgs g) {
       sB[kk][jj] = (gj < g.n && gk < k1) ? B[gk * g.b_k + gj * g.b_j] : 0.f;
     }
     __syncthreads();
+    float t[4][4] = {};
 #pragma unroll
     for (int kk = 0; kk < kGBK; ++kk) {
       const float4 a = *reinterpret_cast<const float4*>(&sA[kk][ti]);
@@ -68,9 +72,13 @@ __global__ void __launch_bounds__(256) gemm_f32(const GemmArgs g) {
 #pragma unroll
       for (int u = 0; u < 4; ++u)
 #pragma unroll
-        for (int v = 0; v < 4; ++v) acc[u][v] = fmaf(av[u], bv[v], acc[u][v]);
+        for (int v = 0; v < 4; ++v) t[u][v] = fmaf(av[u], bv[v], t[u][v]);
     }
     __syncthreads();
+#pragma unroll
+    for (int u = 0; u < 4; ++u)
+#pragma unroll
+      for (int v = 0; v < 4; ++v) acc[u][v] += t[u][v];
   }
 #pragma unroll
   for (int u = 0; u < 4; ++u)
@@ -88,13 +96,37 @@ __global__ void pl_reduce(const float* __restrict__ part, int nsplit, long long 
   dst[i] += v;
 }
 
-// dst[j] += sum_r src[r * ld + j] (r in order), j < n
+// sum over r < rows of f(r) in a fixed tree: runs of 8 rows, runs of 8 of those, of 8 of those, then in order.  About
+// 24 + rows / 512 roundings per sum instead of rows.  f is read 16 rows at a time, so 16 loads are in flight.
+template <class F>
+__device__ __forceinline__ float pl_tree_sum(int rows, F f) {
+  float v = 0.f;
+  for (int r3 = 0; r3 < rows; r3 += 512) {
+    float s2 = 0.f;
+    for (int r2 = r3; r2 < min(rows, r3 + 512); r2 += 64) {
+      float s1 = 0.f;
+      for (int r1 = r2; r1 < min(rows, r2 + 64); r1 += 16) {
+        float x[16];
+#pragma unroll
+        for (int u = 0; u < 16; ++u) x[u] = r1 + u < rows ? f(r1 + u) : 0.f;
+        float a = 0.f, b = 0.f;
+#pragma unroll
+        for (int u = 0; u < 8; ++u) { a += x[u]; b += x[8 + u]; }
+        s1 += a;
+        s1 += b;
+      }
+      s2 += s1;
+    }
+    v += s2;
+  }
+  return v;
+}
+
+// dst[j] += sum_r src[r * ld + j] (pl_tree_sum), j < n
 __global__ void pl_colsum(const float* __restrict__ src, int rows, int n, long long ld, float* __restrict__ dst) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n) return;
-  float v = 0.f;
-  for (int r = 0; r < rows; ++r) v += src[r * ld + j];
-  dst[j] += v;
+  dst[j] += pl_tree_sum(rows, [&](int r) { return src[r * ld + j]; });
 }
 
 // ------------------------------------------------------------------------------------ per-row phases (warp per row)
@@ -252,16 +284,15 @@ __global__ void pl_gather_x(const float* __restrict__ z, const float* __restrict
   x[i] = c < L ? z[static_cast<size_t>(r) * L + c] : emb[static_cast<size_t>(task[r]) * T + c - L];
 }
 
-// dst[t][c] += sum over rows r with task[r] == t (in order) of sum_i src_i[r][c], i over the three [rows, ld] sources
+// dst[t][c] += sum over rows r with task[r] == t (pl_tree_sum) of sum_i src_i[r][c], i over the three [rows, ld] sources
 __global__ void pl_emb_grad(const float* __restrict__ s0, const float* __restrict__ s1, const float* __restrict__ s2,
                             long long ld, const int* __restrict__ task, int rows, int tasks, int T, float* __restrict__ dst) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= tasks * T) return;
   const int t = i / T, cc = i % T;
-  float v = 0.f;
-  for (int r = 0; r < rows; ++r)
-    if (task[r] == t) v += (s0[r * ld + cc] + s1[r * ld + cc]) + s2[r * ld + cc];
-  dst[i] += v;
+  dst[i] += pl_tree_sum(rows, [&](int r) {
+    return task[r] == t ? (s0[r * ld + cc] + s1[r * ld + cc]) + s2[r * ld + cc] : 0.f;
+  });
 }
 
 // ------------------------------------------------------------------------------------ agent._update (world-model loss)

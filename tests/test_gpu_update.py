@@ -228,11 +228,16 @@ def _oracle(cfg, sd, x, dtype, split=False):
 
 
 RATIO_CASES = [("c1", {}, 3, 16), ("tiny-mt", {}, 3, 32), ("tiny", {"episodic": True}, 3, 32),
-               ("tiny", {"action_dim": 128, "num_bins": 256, "latent_dim": 8}, 2, 16)]
-RATIO_IDS = ["c1", "tiny-mt", "episodic", "corner"]
-# Measured, not yet explained: on the wgmma engine only, these miss the ratio rule by about 10x -- the episodic model's
-# termination.1 gradients at trained scale, and grad_norm of the corner (every gradient tensor of the corner passes).
-# The SIMT engine passes every quantity of every case.  strict: a fix makes these fail until the marks are removed.
+               ("tiny", {"action_dim": 128, "num_bins": 256, "latent_dim": 8}, 2, 16), ("c1", {}, 3, 256)]
+RATIO_IDS = ["c1", "tiny-mt", "episodic", "corner", "c1-b256"]
+# On the wgmma engine only, these miss the ratio rule by about 10x -- the episodic model's termination.1 gradients at
+# trained scale, and grad_norm of the corner (every gradient tensor of the corner passes).  The SIMT engine passes every
+# quantity of every case.  They are forward error amplified downstream, not the backward: tests/test_gpu_backward.py runs
+# the same models and batch shapes with the float64 reference anchored on the kernels' own tape, and on the wgmma engine
+# the backward passes with worst ratios 2.9 (episodic/mid), 2.1 (corner/init) and 2.9 (corner/mid), the taped forward
+# of each layer from the kernels' own input with 1.8, 2.2 and 2.1.  The wgmma engine's per-layer forward error is within
+# the rule; compounded through the rollout and the heads it is not, in these two quantities.  strict: a change that
+# makes them pass makes these fail until the marks are removed.
 RATIO_KNOWN = {("episodic", "mid", "tcgen05"): "termination.1 gradients", ("corner", "init", "tcgen05"): "grad_norm",
                ("corner", "mid", "tcgen05"): "grad_norm"}
 

@@ -59,13 +59,14 @@ def test_fixture_through_update_pi(engine, name, monkeypatch):
         assert float((got - w).abs().max()) <= 2.5 * agent.cfg.lr, k
 
 
-def qualifying_batch(cfg, sd, T, B, seed):
+def qualifying_batch(cfg, sd, T, B, seed, pool=256):
     """zs [T, B, L], task [B] | None, eps [T, B, A], qidx: rows where the float64 |log_pi| > 1e-2 and min(1 - a^2) > 1e-3
-    (the squash term and the entropy scale are ill-conditioned elsewhere; the same exclusion as row_mode_ratio_rule)."""
+    (the squash term and the entropy scale are ill-conditioned elsewhere; the same exclusion as row_mode_ratio_rule),
+    drawn from `pool` candidates per row."""
     import torch.nn.functional as F
     from oracle.wm_oracle import WMOracle
     g = torch.Generator().manual_seed(seed)
-    N = 256 * T * B                                               # candidate rows; column b takes task b % num_tasks
+    N = pool * T * B                                              # candidate rows; column b takes task b % num_tasks
     ntask = len(cfg.tasks) if cfg.multitask else 1
     zs = F.softmax(torch.randn(N, cfg.latent_dim // 8, 8, generator=g) * 3, dim=-1).reshape(N, -1)
     eps = torch.randn(N, cfg.action_dim, generator=g)
@@ -118,7 +119,7 @@ def oracle_pair(cfg, sd, zs, task, eps, qidx, drop=None, steps=1):
 
 
 RATIO_CASES = [("c1", {}, 4, 64), ("tiny-mt", {"task_dim": 5, "action_dims": [5, 1, 4, 2]}, 3, 32),
-               ("tiny", {"action_dim": 128, "num_bins": 256, "latent_dim": 8}, 2, 16)]
+               ("tiny", {"action_dim": 128, "num_bins": 256, "latent_dim": 8}, 2, 16), ("c1", {}, 4, 256)]
 
 
 # (case, level): at "mid" every one of the wide-head corner's 128 action dims would have to stay unsaturated for a row to
@@ -127,7 +128,8 @@ RATIO_PARAMS = [(c, lv) for c in RATIO_CASES for lv in ("init", "mid") if not (l
 
 
 @pytest.mark.parametrize("engine", ENGINES)
-@pytest.mark.parametrize("case,level", RATIO_PARAMS, ids=lambda c: c if isinstance(c, str) else c[0] + ("-corner" if c[1] else ""))
+@pytest.mark.parametrize("case,level", RATIO_PARAMS, ids=lambda c: c if isinstance(c, str) else c[0] + ("-corner" if c[1] else "")
+                         + ("-b256" if c[3] == 256 else ""))
 def test_ratio_rule_against_float64(engine, case, level, monkeypatch):
     wl, over, T, B = case
     cfg, sd = level_model(wl, level, **over)
@@ -137,7 +139,7 @@ def test_ratio_rule_against_float64(engine, case, level, monkeypatch):
     agent = make_agent(cfg, sd, engine)
     grads = {}
     info = run(agent, zs, task, eps, qidx, None, grads, monkeypatch)
-    tag = f"update_pi/{wl}{'-corner' if over else ''}/{level}/{engine}"
+    tag = f"update_pi/{wl}{'-corner' if over else ''}{'-b256' if B == 256 else ''}/{level}/{engine}"
     for q, k in (("pi_loss", info["pi_loss"]), ("pi_grad_norm", info["pi_grad_norm"])):
         key = "loss" if q == "pi_loss" else "grad_norm"
         ratio_rule(q, tag, k.reshape(1), yardstick(q, o32[key], o32s[key], o64[key]).reshape(1), o64[key].reshape(1))
