@@ -40,6 +40,8 @@ static int fail(int code, const char* fmt, ...) {
     if (_e != cudaSuccess)                                                                          \
       return fail(TDMPC2_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
   } while (0)
+// the check after each launch of a backward chain: its error, or an earlier kernel's, as TDMPC2_ERR_CUDA
+static int launch_ok() { CUDA_TRY(cudaGetLastError()); return 0; }
 
 static unsigned env_uint(const char* name, unsigned dflt) {
   const char* v = getenv(name);
@@ -756,28 +758,27 @@ extern "C" int tdmpc2_pixel_encode_backward(tdmpc2_pixel_encoder* e, const tdmpc
   auto dw = [&](int l, auto kern, int KK, const float* dy, int OH, const float* x, int64_t xp, int IC, int IH) -> int {
     const int ns = pixg_nsplit(IC, nc, KK, rows), cols = pixg_cols(IC, KK);
     kern<<<dim3(pixg_ctas_x(IC, nc, KK), ns), kPgThreads, 0, st>>>(dy, nc, OH, OH, x, xp, IC, IH, IH, rows, ns, part);
-    CUDA_TRY(cudaGetLastError());
+    if (const int rc = launch_ok()) return rc;
     pixg_reduce<<<blocks(static_cast<int64_t>(nc) * cols), kPgThreads, 0, st>>>(part, ns, nc, cols, grads->weight[l], grads->bias[l]);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
+    return launch_ok();
   };
   int rc;
   pixg_simnorm_back<<<blocks(rows * (L / e->d.simnorm_dim)), kPgThreads, 0, st>>>(z, dz, rows, L, e->d.simnorm_dim, dp4);
-  CUDA_TRY(cudaGetLastError());
+  if ((rc = launch_ok())) return rc;
   if ((rc = dw(3, pixg_dw<3, 1>, 9, dp4, kPixO4, tape + pix_tape_a3(nc), tp, nc, kPixO3))) return rc;
   pixg_dx<3, 1><<<blocks(rows * nc * kPixO3 * kPixO3), kPgThreads, 0, st>>>(dp4, nc, kPixO4, kPixO4, w->weight[3], tape + pix_tape_a3(nc),
                                                                             tp, nc, kPixO3, kPixO3, rows, dp3);
-  CUDA_TRY(cudaGetLastError());
+  if ((rc = launch_ok())) return rc;
   if ((rc = dw(2, pixg_dw<3, 2>, 9, dp3, kPixO3, tape + pix_tape_a2(nc), tp, nc, kPixO2))) return rc;
   pixg_dx<3, 2><<<blocks(rows * nc * kPixO2 * kPixO2), kPgThreads, 0, st>>>(dp3, nc, kPixO3, kPixO3, w->weight[2], tape + pix_tape_a2(nc),
                                                                             tp, nc, kPixO2, kPixO2, rows, dp2);
-  CUDA_TRY(cudaGetLastError());
+  if ((rc = launch_ok())) return rc;
   if ((rc = dw(1, pixg_dw<5, 2>, 25, dp2, kPixO2, tape, tp, nc, kPixO1))) return rc;
   pixg_dx<5, 2><<<blocks(rows * nc * kPixO1 * kPixO1), kPgThreads, 0, st>>>(dp2, nc, kPixO2, kPixO2, w->weight[1], tape, tp, nc, kPixO1,
                                                                             kPixO1, rows, dp1);
-  CUDA_TRY(cudaGetLastError());
+  if ((rc = launch_ok())) return rc;
   pixg_stage<<<blocks(rows * pix_stage_floats(C)), kPgThreads, 0, st>>>(frames, shift, grid_base, rows, C, img);
-  CUDA_TRY(cudaGetLastError());
+  if ((rc = launch_ok())) return rc;
   return dw(0, pixg_dw<7, 2>, 49, dp1, kPixO1, img, pix_stage_floats(C), C, kPixHW);
 }
 
@@ -1037,6 +1038,106 @@ extern "C" int tdmpc2_td_target(tdmpc2_planner* p, const float* next_z, const fl
   return launch(p, prm, stream_);
 }
 
+// ------------------------------------------------------------------------------------ backward chains (grad_kernels.cuh)
+// The number of row blocks a dW reduction over `rows` rows is split into: at most 8, of at least 256 rows each.
+static int dw_nsplit(size_t rows) { return std::max(1, std::min(8, static_cast<int>(rows / 256))); }
+
+// The launch context of a backward chain: its stream, and the split-K partials [nsplit, m n] of dweight.  Each member
+// issues its kernels in order, each followed by the launch check.
+struct Bwd {
+  cudaStream_t st;
+  float* part;
+  int nsplit;
+
+  int gemm(const GemmArgs& g, int batch) const {
+    gemm_f32<<<dim3((g.n + kGBN - 1) / kGBN, (g.m + kGBM - 1) / kGBM, batch * g.nsplit), 256, 0, st>>>(g);
+    return launch_ok();
+  }
+  // out [rows, n] = g [rows, k] W[:, :n] (W [k, ldw]), batched over `batch` heads (g, out strides; W by bsel)
+  int dinput(const float* g, long long k, const float* Wt, long long ldw, long long w_z, const int* bsel, int batch, long long n,
+             float* out, long long ldo, long long o_z, int rows) const {
+    return gemm(GemmArgs{g, k, 1, static_cast<long long>(rows) * k, Wt, ldw, 1, w_z, bsel, out, ldo, o_z, 0, rows,
+                         static_cast<int>(n), static_cast<int>(k), 1}, batch);
+  }
+  // dst [m, n] += src^T x over `rows` rows (src [rows, m], x [rows, n] with row pitch ldx), split-K partials summed in order
+  int dweight(const float* src, long long m, const float* x, long long n, long long ldx, int rows, float* dst) const {
+    const int rc = gemm(GemmArgs{src, 1, m, 0, x, ldx, 1, 0, nullptr, part, n, 0, m * n, static_cast<int>(m), static_cast<int>(n),
+                                 rows, nsplit}, 1);
+    if (rc) return rc;
+    pl_reduce<<<static_cast<int>((m * n + 255) / 256), 256, 0, st>>>(part, nsplit, m * n, m * n, dst);
+    return launch_ok();
+  }
+  // dst [n] += the column sums of src [rows, n] (row pitch ld)
+  int colsum(const float* src, int rows, long long n, long long ld, float* dst) const {
+    pl_colsum<<<static_cast<int>((n + 127) / 128), 128, 0, st>>>(src, rows, static_cast<int>(n), ld, dst);
+    return launch_ok();
+  }
+  // LayerNorm + Mish backward of a layer of width N, in place on g [batch, rows, N]: batch u reads row r's pre-LayerNorm
+  // values at tape + r pitch + off + u off_z, and the LayerNorm parameters and dropout scale of head hsel[u] (head 0
+  // without hsel).  dyn, dy and h (laid out like g) may be null.
+  int ln_back(const float* tape, int pitch, long long off, int rows, long long N, const tdmpc2_linear& lw, float* g, float* dyn,
+              float* dy, float* h, const float* drop = nullptr, int batch = 1, const int* hsel = nullptr, long long off_z = 0) const {
+    LnBackArgs a{};
+    a.tape = tape; a.pitch = pitch; a.off = static_cast<int>(off); a.off_z = off_z; a.g = g; a.out = g; a.ld = N; a.g_z = rows * N;
+    a.o_z = a.g_z; a.gamma = lw.ln_weight; a.beta = lw.ln_bias; a.hsel = hsel; a.drop = drop; a.dyn = dyn; a.dy = dy; a.h = h;
+    a.rows = rows; a.N = static_cast<int>(N);
+    pl_ln_back<<<dim3((rows + 7) / 8, batch), 256, 0, st>>>(a);
+    return launch_ok();
+  }
+  // LayerNorm + SimNorm (groups of V) backward of a layer of width N from dL/ds g [rows, N] to out; dyn and dy may be null
+  int ln_simnorm_back(const float* tape, int pitch, long long off, int rows, long long N, const tdmpc2_linear& lw, const float* g,
+                      float* out, float* dyn, float* dy, int V) const {
+    LnBackArgs a{};
+    a.tape = tape; a.pitch = pitch; a.off = static_cast<int>(off); a.g = g; a.out = out; a.ld = N; a.gamma = lw.ln_weight;
+    a.beta = lw.ln_bias; a.dyn = dyn; a.dy = dy; a.rows = rows; a.N = static_cast<int>(N);
+    pl_ln_simnorm_back<<<(rows + 7) / 8, 256, 0, st>>>(a, V);
+    return launch_ok();
+  }
+};
+
+// head_back's scratch, each [batch, rows, M]: dL/dpre of layers 1 and 0, and the dgamma / dbeta row terms and the
+// activation of the layer below (written only with parameter gradients)
+struct HeadWs {
+  float *g1, *g0, *dyn, *dy, *h;
+};
+
+// The backward of `batch` head MLPs (NormedLinear 0 and 1, then a plain Linear 2) over `rows` rows, from dL/dlogits
+// dl [batch, rows, nout].  Batch u is head hsel[u] (u without hsel) of the stacked weights lw; layer l's pre-LayerNorm
+// values of its row r are at tape + r pitch + off0 + l M + u off_z; drop is layer 0's dropout scale, or null.  With lg,
+// ADDS every layer's parameter gradients, reading layer 0's input x0 [rows, K0].  With dx, writes dL/dX [batch, rows, ldx]
+// of layer 0's input columns col .. col + nx.
+static int head_back(const Bwd& b, int rows, long long M, int batch, const int* hsel, const float* dl, long long nout,
+                     const tdmpc2_linear* lw, const tdmpc2_linear_grad* lg, const float* tape, int pitch, int off0, long long off_z,
+                     const float* drop, const float* x0, long long K0, long long col, long long nx, float* dx, long long ldx,
+                     const HeadWs& s) {
+  const long long RM = rows * M;
+  float *dyn = lg ? s.dyn : nullptr, *dy = lg ? s.dy : nullptr, *h = lg ? s.h : nullptr;
+  int rc;
+  if ((rc = b.dinput(dl, nout, lw[2].weight, M, nout * M, hsel, batch, M, s.g1, M, RM, rows)) ||
+      (rc = b.ln_back(tape, pitch, off0 + M, rows, M, lw[1], s.g1, dyn, dy, h, nullptr, batch, hsel, off_z)))
+    return rc;
+  for (int u = 0; lg && u < batch; ++u) {
+    const long long o = u * RM;
+    if ((rc = b.colsum(dyn + o, rows, M, M, lg[1].ln_weight + u * M)) || (rc = b.colsum(dy + o, rows, M, M, lg[1].ln_bias + u * M)) ||
+        (rc = b.dweight(dl + u * rows * nout, nout, h + o, M, M, rows, lg[2].weight + u * nout * M)) ||
+        (rc = b.colsum(dl + u * rows * nout, rows, nout, nout, lg[2].bias + u * nout)))
+      return rc;
+  }
+  if ((rc = b.dinput(s.g1, M, lw[1].weight, M, M * M, hsel, batch, M, s.g0, M, RM, rows)) ||
+      (rc = b.ln_back(tape, pitch, off0, rows, M, lw[0], s.g0, dyn, dy, h, drop, batch, hsel, off_z)))
+    return rc;
+  for (int u = 0; lg && u < batch; ++u) {
+    const long long o = u * RM;
+    if ((rc = b.colsum(dyn + o, rows, M, M, lg[0].ln_weight + u * M)) || (rc = b.colsum(dy + o, rows, M, M, lg[0].ln_bias + u * M)) ||
+        (rc = b.dweight(s.g1 + o, M, h + o, M, M, rows, lg[1].weight + u * M * M)) ||
+        (rc = b.colsum(s.g1 + o, rows, M, M, lg[1].bias + u * M)) ||
+        (rc = b.dweight(s.g0 + o, M, x0, K0, K0, rows, lg[0].weight + u * M * K0)) ||
+        (rc = b.colsum(s.g0 + o, rows, M, M, lg[0].bias + u * M)))
+      return rc;
+  }
+  return dx ? b.dinput(s.g0, M, lw[0].weight + col, K0, M * K0, hsel, batch, nx, dx, ldx, rows * ldx, rows) : 0;
+}
+
 // ------------------------------------------------------------------------------------ agent.update_pi (ROP_PI_LOSS + grad_kernels.cuh)
 static PiTape planner_tape(const tdmpc2_planner* p) {
   return pi_tape(p->d.mlp_dim, p->d.action_dim, pad_to(p->d.action_dim, 32), p->d.num_bins);
@@ -1052,13 +1153,12 @@ static PiWs pi_ws(const tdmpc2_planner* p, int rows) {
   const tdmpc2_dims& d = p->d;
   const size_t R = rows, M = d.mlp_dim, nb = d.num_bins, TA = d.task_dim + d.action_dim, LT = d.latent_dim + d.task_dim;
   PiWs w;
-  w.nsplit = std::max(1, std::min(8, rows / 256));
+  w.nsplit = dw_nsplit(R);
   size_t off = 0;
-  auto take = [&](size_t n) { const size_t o = off; off += (n + 63) / 64 * 64; return o; };
-  w.dl = take(2 * R * nb); w.gq = take(2 * R * M); w.gq2 = take(2 * R * M); w.dxq = take(2 * R * TA);
-  w.dlog = take(R * 2 * d.action_dim); w.gp = take(R * M); w.gp2 = take(R * M); w.dyn = take(R * M); w.dy = take(R * M);
-  w.hb = take(R * M); w.xb = take(R * LT); w.dxe = take(R * TA);
-  w.part = take(static_cast<size_t>(w.nsplit) * M * std::max({M, LT, static_cast<size_t>(2 * d.action_dim)}));
+  w.dl = take64(off, 2 * R * nb); w.gq = take64(off, 2 * R * M); w.gq2 = take64(off, 2 * R * M); w.dxq = take64(off, 2 * R * TA);
+  w.dlog = take64(off, R * 2 * d.action_dim); w.gp = take64(off, R * M); w.gp2 = take64(off, R * M); w.dyn = take64(off, R * M);
+  w.dy = take64(off, R * M); w.hb = take64(off, R * M); w.xb = take64(off, R * LT); w.dxe = take64(off, R * TA);
+  w.part = take64(off, static_cast<size_t>(w.nsplit) * M * std::max({M, LT, static_cast<size_t>(2 * d.action_dim)}));
   w.floats = off;
   return w;
 }
@@ -1090,13 +1190,6 @@ extern "C" int tdmpc2_pi_loss_forward(tdmpc2_planner* p, const float* z, const i
   return launch(p, prm, stream_);
 }
 
-static int gemm(const GemmArgs& g, int batch, cudaStream_t st) {
-  const dim3 grid((g.n + kGBN - 1) / kGBN, (g.m + kGBM - 1) / kGBM, batch * g.nsplit);
-  gemm_f32<<<grid, 256, 0, st>>>(g);
-  CUDA_TRY(cudaGetLastError());
-  return 0;
-}
-
 extern "C" int tdmpc2_pi_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* z,
                                        const int32_t* task, const float* eps, const int32_t* qidx, const float* dropout_mask,
                                        int T, int B, const float* scale, float entropy_coef, float rho,
@@ -1123,87 +1216,47 @@ extern "C" int tdmpc2_pi_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* 
   const PiTape tp = planner_tape(p);
   const PiWs L = pi_ws(p, R);
   float* ws = static_cast<float*>(workspace);
+  const Bwd bw{st, ws + L.part, L.nsplit};
   const long long M = d.mlp_dim, nb = d.num_bins, A = d.action_dim, Tq = d.task_dim, TA = Tq + A, Lz = d.latent_dim;
   const long long LT = Lz + Tq, D = Lz + Tq + A;
-  float *dl = ws + L.dl, *gq = ws + L.gq, *gq2 = ws + L.gq2, *dxq = ws + L.dxq, *dlog = ws + L.dlog, *gp = ws + L.gp,
-        *gp2 = ws + L.gp2, *dyn = ws + L.dyn, *dy = ws + L.dy, *hb = ws + L.hb, *xb = ws + L.xb, *dxe = ws + L.dxe,
-        *part = ws + L.part;
-  const dim3 rows8((R + 7) / 8), rows8x2((R + 7) / 8, 2);
-  const int* task_rows = d.task_dim > 0 ? task : nullptr;
-  auto colsum = [&](const float* src, long long n, long long ld, float* dst) -> int {
-    pl_colsum<<<static_cast<int>((n + 127) / 128), 128, 0, st>>>(src, R, static_cast<int>(n), ld, dst);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
-  };
-  // dst += src^T x [rows, n] over the rows, in nsplit row blocks summed in order
-  auto dweight = [&](const float* src, long long m, const float* x, long long n, long long ldx, float* dst) -> int {
-    GemmArgs g{src, 1, m, 0, x, ldx, 1, 0, nullptr, part, n, 0, m * n, static_cast<int>(m), static_cast<int>(n), R, L.nsplit};
-    int rc2 = gemm(g, 1, st);
-    if (rc2) return rc2;
-    pl_reduce<<<static_cast<int>((m * n + 255) / 256), 256, 0, st>>>(part, L.nsplit, m * n, m * n, dst);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
-  };
-  LnBackArgs lb{};
-  lb.tape = tape; lb.pitch = tp.pitch; lb.rows = R; lb.N = static_cast<int>(M); lb.ld = M;
+  float *dl = ws + L.dl, *dxq = ws + L.dxq, *dlog = ws + L.dlog, *xb = ws + L.xb, *dxe = ws + L.dxe;
 
-  // ---- the two Q heads: two-hot inverse -> layer 2 -> LN/Mish 1 -> layer 1 -> LN/Mish/dropout 0 -> [emb | a] columns
-  pl_q_head_back<<<rows8x2, 256, 0, st>>>(tape, tp.pitch, tp.q[0] + 2 * static_cast<int>(M), tp.q[1] + 2 * static_cast<int>(M), R,
-                                          static_cast<int>(nb), p->base.bins, scale, B, T, rho, dl);
-  CUDA_TRY(cudaGetLastError());
-  if ((rc = gemm(GemmArgs{dl, nb, 1, R * nb, w->qs[2].weight, M, 1, nb * M, qidx, gq, M, R * M, 0,
-                          R, static_cast<int>(M), static_cast<int>(nb), 1}, 2, st))) return rc;
-  lb.off = tp.q[0] + static_cast<int>(M); lb.off_z = tp.q[1] - tp.q[0]; lb.g = gq; lb.out = gq; lb.g_z = R * M;
-  lb.gamma = w->qs[1].ln_weight; lb.beta = w->qs[1].ln_bias; lb.hsel = qidx;
-  pl_ln_back<<<rows8x2, 256, 0, st>>>(lb);
-  CUDA_TRY(cudaGetLastError());
-  if ((rc = gemm(GemmArgs{gq, M, 1, R * M, w->qs[1].weight, M, 1, M * M, qidx, gq2, M, R * M, 0,
-                          R, static_cast<int>(M), static_cast<int>(M), 1}, 2, st))) return rc;
-  lb.off = tp.q[0]; lb.g = gq2; lb.out = gq2; lb.gamma = w->qs[0].ln_weight; lb.beta = w->qs[0].ln_bias; lb.drop = dropout_mask;
-  pl_ln_back<<<rows8x2, 256, 0, st>>>(lb);
-  CUDA_TRY(cudaGetLastError());
-  if ((rc = gemm(GemmArgs{gq2, M, 1, R * M, w->qs[0].weight + Lz, D, 1, M * D, qidx, dxq, TA, R * TA, 0,
-                          R, static_cast<int>(TA), static_cast<int>(M), 1}, 2, st))) return rc;
+  // ---- the two Q heads: two-hot inverse, then dX of their [emb | a] input columns (no parameter gradients: detached)
+  pl_q_head_back<<<dim3((R + 7) / 8, 2), 256, 0, st>>>(tape, tp.pitch, tp.q[0] + 2 * static_cast<int>(M), tp.q[1] + 2 * static_cast<int>(M),
+                                                       R, static_cast<int>(nb), p->base.bins, scale, B, T, rho, dl);
+  if ((rc = launch_ok()) ||
+      (rc = head_back(bw, R, M, 2, qidx, dl, nb, w->qs, nullptr, tape, tp.pitch, tp.q[0], tp.q[1] - tp.q[0], dropout_mask, nullptr,
+                      D, Lz, TA, dxq, TA, HeadWs{ws + L.gq, ws + L.gq2, nullptr, nullptr, nullptr})))
+    return rc;
 
-  // ---- the tanh-Gaussian head, then pi layers 2 -> 0 with their parameter gradients
+  // ---- the tanh-Gaussian head, then pi layers 2 -> 0 with their parameter gradients and, for multi-task models, dX of
+  // pi.0's embedding columns
   PiHeadArgs ph{};
   ph.tape = tape; ph.pitch = tp.pitch; ph.off_h = tp.pih; ph.Apad = pad_to(d.action_dim, 32);
-  ph.eps = eps; ph.task = task_rows; ph.masks = p->base.masks;
+  ph.eps = eps; ph.task = d.task_dim > 0 ? task : nullptr; ph.masks = p->base.masks;
   ph.da_q = dxq; ph.da_ld = TA; ph.da_z = R * TA; ph.a_off = static_cast<int>(Tq);
   ph.log_std_min = d.log_std_min; ph.log_std_dif = d.log_std_dif; ph.entropy_coef = entropy_coef; ph.rho = rho; ph.scale = scale;
   ph.rows = R; ph.A = d.action_dim; ph.Bsz = B; ph.Tsz = T; ph.dlog = dlog;
-  pl_pi_head_back<<<rows8, 256, 0, st>>>(ph);
-  CUDA_TRY(cudaGetLastError());
-  if ((rc = gemm(GemmArgs{dlog, 2 * A, 1, 0, w->pi[2].weight, M, 1, 0, nullptr, gp, M, 0, 0,
-                          R, static_cast<int>(M), static_cast<int>(2 * A), 1}, 1, st))) return rc;
-  lb.off = tp.pi1; lb.off_z = 0; lb.g = gp; lb.out = gp; lb.g_z = 0; lb.gamma = w->pi[1].ln_weight; lb.beta = w->pi[1].ln_bias;
-  lb.hsel = nullptr; lb.drop = nullptr; lb.dyn = dyn; lb.dy = dy; lb.h = hb;
-  pl_ln_back<<<rows8, 256, 0, st>>>(lb);                       // gp <- dL/dpre of pi.1; hb <- pi.1's activation
-  CUDA_TRY(cudaGetLastError());
-  if ((rc = colsum(dyn, M, M, gr->ln_weight[1])) || (rc = colsum(dy, M, M, gr->ln_bias[1]))) return rc;
-  if ((rc = dweight(dlog, 2 * A, hb, M, M, gr->weight[2])) || (rc = colsum(dlog, 2 * A, 2 * A, gr->bias[2]))) return rc;
-  if ((rc = gemm(GemmArgs{gp, M, 1, 0, w->pi[1].weight, M, 1, 0, nullptr, gp2, M, 0, 0,
-                          R, static_cast<int>(M), static_cast<int>(M), 1}, 1, st))) return rc;
-  lb.off = tp.pi0; lb.g = gp2; lb.out = gp2; lb.gamma = w->pi[0].ln_weight; lb.beta = w->pi[0].ln_bias;
-  pl_ln_back<<<rows8, 256, 0, st>>>(lb);                       // gp2 <- dL/dpre of pi.0; hb <- pi.0's activation
-  CUDA_TRY(cudaGetLastError());
-  if ((rc = colsum(dyn, M, M, gr->ln_weight[0])) || (rc = colsum(dy, M, M, gr->ln_bias[0]))) return rc;
-  if ((rc = dweight(gp, M, hb, M, M, gr->weight[1])) || (rc = colsum(gp, M, M, gr->bias[1]))) return rc;
-  const float* x = z;
+  pl_pi_head_back<<<(R + 7) / 8, 256, 0, st>>>(ph);
+  if ((rc = launch_ok())) return rc;
+  const float* x = z;     // pi.0's input [z | emb]
   if (Tq > 0) {
     pl_gather_x<<<static_cast<int>((R * LT + 255) / 256), 256, 0, st>>>(z, p->base.emb, task, R, static_cast<int>(Lz),
                                                                        static_cast<int>(Tq), xb);
-    CUDA_TRY(cudaGetLastError());
+    if ((rc = launch_ok())) return rc;
     x = xb;
   }
-  if ((rc = dweight(gp2, M, x, LT, LT, gr->weight[0])) || (rc = colsum(gp2, M, M, gr->bias[0]))) return rc;
+  const tdmpc2_linear_grad pg[3] = {{gr->weight[0], gr->bias[0], gr->ln_weight[0], gr->ln_bias[0]},
+                                    {gr->weight[1], gr->bias[1], gr->ln_weight[1], gr->ln_bias[1]},
+                                    {gr->weight[2], gr->bias[2], nullptr, nullptr}};
+  if ((rc = head_back(bw, R, M, 1, nullptr, dlog, 2 * A, w->pi, pg, tape, tp.pitch, tp.pi0, 0, nullptr, x, LT, Lz, Tq,
+                      Tq > 0 ? dxe : nullptr, TA, HeadWs{ws + L.gp, ws + L.gp2, ws + L.dyn, ws + L.dy, ws + L.hb})))
+    return rc;
   if (Tq > 0) {
     // the embedding enters pi.0's and both Q heads' layer-0 inputs: dL/demb of each row, scattered by task in row order
-    if ((rc = gemm(GemmArgs{gp2, M, 1, 0, w->pi[0].weight + Lz, LT, 1, 0, nullptr, dxe, TA, 0, 0,
-                            R, static_cast<int>(Tq), static_cast<int>(M), 1}, 1, st))) return rc;
     pl_emb_grad<<<static_cast<int>((d.num_tasks * Tq + 127) / 128), 128, 0, st>>>(dxe, dxq, dxq + R * TA, TA, task, R, d.num_tasks,
                                                                                 static_cast<int>(Tq), gr->task_emb);
-    CUDA_TRY(cudaGetLastError());
+    if ((rc = launch_ok())) return rc;
   }
   return 0;
 }
@@ -1247,7 +1300,7 @@ static WmWs wm_ws(const tdmpc2_planner* p, int H, int B) {
   const bool enc = p->num_enc > 0;
   const size_t E = enc ? d.enc_dim : 0, EL = enc ? std::max(E, L) : 0, OT = enc ? d.obs_dim + T : 0, BE = enc ? B : 0;
   WmWs w;
-  w.nsplit = std::max(1, std::min(8, static_cast<int>(R / 256)));
+  w.nsplit = dw_nsplit(R);
   size_t off = 0;
   w.dlr = take64(off, R * nb); w.dlq = take64(off, nq * R * nb); w.dlt = take64(off, R);
   w.gA = take64(off, nq * R * M); w.gB = take64(off, nq * R * M); w.dyn = take64(off, nq * R * M); w.dy = take64(off, nq * R * M);
@@ -1380,94 +1433,42 @@ static int wm_backward_impl(tdmpc2_planner* p, const tdmpc2_weights* w, const fl
   const WmTape tp = wm_tape(p, H, B);
   const WmWs W = wm_ws(p, H, B);
   float* ws = static_cast<float*>(workspace);
+  const Bwd bw{st, ws + W.part, W.nsplit};
   const int R = H * B, nq = d.num_q;
   const long long M = d.mlp_dim, nb = d.num_bins, A = d.action_dim, Tq = d.task_dim, Lz = d.latent_dim, E = d.enc_dim;
   const long long LT = Lz + Tq, D = Lz + Tq + A, OT = d.obs_dim + Tq;
   const float fH = static_cast<float>(H), fB = static_cast<float>(B);
   float* X = ws + W.xa;
   int* iota = reinterpret_cast<int*>(ws + W.iota);
-  auto ok = [&]() -> int { CUDA_TRY(cudaGetLastError()); return 0; };
-  auto colsum = [&](const float* src, int rows, long long n, long long ld, float* dst) -> int {
-    pl_colsum<<<static_cast<int>((n + 127) / 128), 128, 0, st>>>(src, rows, static_cast<int>(n), ld, dst);
-    return ok();
-  };
-  // dst [m, n] += src^T x over `rows` rows (src [rows, m], x [rows, n] with row pitch ldx), split-K partials summed in order
-  auto dweight = [&](const float* src, long long m, const float* x, long long n, long long ldx, int rows, float* dst) -> int {
-    GemmArgs g{src, 1, m, 0, x, ldx, 1, 0, nullptr, ws + W.part, n, 0, m * n, static_cast<int>(m), static_cast<int>(n), rows, W.nsplit};
-    int rc2 = gemm(g, 1, st);
-    if (rc2) return rc2;
-    pl_reduce<<<static_cast<int>((m * n + 255) / 256), 256, 0, st>>>(ws + W.part, W.nsplit, m * n, m * n, dst);
-    return ok();
-  };
-  // out [rows, n] = g [rows, k] W[:, :n] (W [k, ldw]), batched over `batch` heads (g, out strides; W by bsel)
-  auto dinput = [&](const float* g, long long k, const float* Wt, long long ldw, long long w_z, const int* bsel, int batch,
-                    long long n, float* out, long long ldo, long long o_z, int rows) -> int {
-    return gemm(GemmArgs{g, k, 1, static_cast<long long>(rows) * k, Wt, ldw, 1, w_z, bsel, out, ldo, o_z, 0, rows,
-                         static_cast<int>(n), static_cast<int>(k), 1}, batch, st);
-  };
-  // the three layers of a head MLP (NormedLinear 0, 1 and a plain Linear 2) from dL/dlogits dl [batch, R, nout]: parameter
-  // gradients of every layer (layer 0's input x0 [R, K0], row pitch ld0) and dX [batch, R, nx] of layer 0's first nx
-  // input columns (ld ldx)
-  auto head_back = [&](const float* dl, long long nout, const tdmpc2_linear* lw, const tdmpc2_linear_grad* lg, int batch,
-                       const float* tape_seg, int pitch, long long off_z, const float* drop, const float* x0, long long K0,
-                       long long ld0, long long nx, float* dx, long long ldx) -> int {
-    int rc2;
-    float *gA = ws + W.gA, *gB = ws + W.gB, *dyn = ws + W.dyn, *dy = ws + W.dy, *hb = ws + W.hb;
-    const long long RM = static_cast<long long>(R) * M;
-    const int* hs = batch > 1 ? iota : nullptr;
-    if ((rc2 = dinput(dl, nout, lw[2].weight, M, nout * M, hs, batch, M, gA, M, RM, R))) return rc2;
-    LnBackArgs lb{};
-    lb.tape = tape_seg; lb.pitch = pitch; lb.rows = R; lb.N = static_cast<int>(M); lb.ld = M; lb.off_z = off_z; lb.g_z = RM;
-    lb.o_z = RM; lb.hsel = hs; lb.dyn = dyn; lb.dy = dy; lb.h = hb;
-    lb.off = static_cast<int>(M); lb.g = gA; lb.out = gA; lb.gamma = lw[1].ln_weight; lb.beta = lw[1].ln_bias;
-    pl_ln_back<<<dim3((R + 7) / 8, batch), 256, 0, st>>>(lb);
-    if ((rc2 = ok())) return rc2;
-    for (int h = 0; h < batch; ++h) {
-      const long long o = h * RM;
-      if ((rc2 = colsum(dyn + o, R, M, M, lg[1].ln_weight + h * M)) || (rc2 = colsum(dy + o, R, M, M, lg[1].ln_bias + h * M)) ||
-          (rc2 = dweight(dl + h * R * nout, nout, hb + o, M, M, R, lg[2].weight + h * nout * M)) ||
-          (rc2 = colsum(dl + h * R * nout, R, nout, nout, lg[2].bias + h * nout)))
-        return rc2;
-    }
-    if ((rc2 = dinput(gA, M, lw[1].weight, M, M * M, hs, batch, M, gB, M, RM, R))) return rc2;
-    lb.off = 0; lb.g = gB; lb.out = gB; lb.gamma = lw[0].ln_weight; lb.beta = lw[0].ln_bias; lb.drop = drop;
-    pl_ln_back<<<dim3((R + 7) / 8, batch), 256, 0, st>>>(lb);
-    if ((rc2 = ok())) return rc2;
-    for (int h = 0; h < batch; ++h) {
-      const long long o = h * RM;
-      if ((rc2 = colsum(dyn + o, R, M, M, lg[0].ln_weight + h * M)) || (rc2 = colsum(dy + o, R, M, M, lg[0].ln_bias + h * M)) ||
-          (rc2 = dweight(gA + o, M, hb + o, M, M, R, lg[1].weight + h * M * M)) || (rc2 = colsum(gA + o, R, M, M, lg[1].bias + h * M)) ||
-          (rc2 = dweight(gB + o, M, x0, K0, ld0, R, lg[0].weight + h * M * K0)) || (rc2 = colsum(gB + o, R, M, M, lg[0].bias + h * M)))
-        return rc2;
-    }
-    return dinput(gB, M, lw[0].weight, K0, M * K0, hs, batch, nx, dx, ldx, static_cast<long long>(R) * ldx, R);
-  };
+  const HeadWs hw{ws + W.gA, ws + W.gB, ws + W.dyn, ws + W.dy, ws + W.hb};
 
   pl_iota<<<1, 32 * ((nq + 31) / 32), 0, st>>>(iota, nq);
-  if ((rc = ok())) return rc;
+  if ((rc = launch_ok())) return rc;
   // X = [zs[:H] | emb | action]: the layer-0 input of the dynamics, reward and Q heads (z columns first)
   pl_gather_xa<<<static_cast<int>((R * D + 255) / 256), 256, 0, st>>>(zs, p->base.emb, task, action, R, static_cast<int>(Lz),
                                                                      static_cast<int>(Tq), static_cast<int>(A), X);
-  if ((rc = ok())) return rc;
+  if ((rc = launch_ok())) return rc;
 
   // ---- 1. the heads, all H B rows at once: Q (batched over heads), reward, termination
   pl_soft_ce_back<<<dim3((R + 7) / 8, nq), 256, 0, st>>>(q_logits, static_cast<long long>(R) * nb, R, static_cast<int>(nb), td_target,
                                                          cf->vmin, cf->vmax, cf->bin_size, cf->value / (fH * nq * fB), cf->rho, B,
                                                          ws + W.dlq);
-  if ((rc = ok())) return rc;
-  if ((rc = head_back(ws + W.dlq, nb, w->qs, gr->qs, nq, tape + tp.q, tp.p_q, 2 * M, dropout_mask, X, D, D, LT, ws + W.dxq, LT)))
+  if ((rc = launch_ok()) ||
+      (rc = head_back(bw, R, M, nq, iota, ws + W.dlq, nb, w->qs, gr->qs, tape + tp.q, tp.p_q, 0, 2 * M, dropout_mask, X, D, 0, LT,
+                      ws + W.dxq, LT, hw)))
     return rc;
   pl_soft_ce_back<<<dim3((R + 7) / 8, 1), 256, 0, st>>>(reward_logits, 0, R, static_cast<int>(nb), reward, cf->vmin, cf->vmax,
                                                         cf->bin_size, cf->reward / (fH * fB), cf->rho, B, ws + W.dlr);
-  if ((rc = ok())) return rc;
-  if ((rc = head_back(ws + W.dlr, nb, w->reward, gr->reward, 1, tape + tp.rew, tp.p_rew, 0, nullptr, X, D, D, LT, ws + W.dxr, LT)))
+  if ((rc = launch_ok()) ||
+      (rc = head_back(bw, R, M, 1, nullptr, ws + W.dlr, nb, w->reward, gr->reward, tape + tp.rew, tp.p_rew, 0, 0, nullptr, X, D, 0,
+                      LT, ws + W.dxr, LT, hw)))
     return rc;
   if (d.episodic) {
     pl_bce_back<<<(R + 255) / 256, 256, 0, st>>>(term_logits, terminated, R, cf->termination / (fH * fB), ws + W.dlt);
-    if ((rc = ok())) return rc;
     // termination reads [z_{t+1}] alone: its layer-0 input is zs[1:], a contiguous [R, L] block
-    if ((rc = head_back(ws + W.dlt, 1, w->termination, gr->termination, 1, tape + tp.term, tp.p_term, 0, nullptr,
-                        zs + static_cast<size_t>(B) * Lz, Lz, Lz, Lz, ws + W.dxt, Lz)))
+    if ((rc = launch_ok()) ||
+        (rc = head_back(bw, R, M, 1, nullptr, ws + W.dlt, 1, w->termination, gr->termination, tape + tp.term, tp.p_term, 0, 0,
+                        nullptr, zs + static_cast<size_t>(B) * Lz, Lz, 0, Lz, ws + W.dxt, Lz, hw)))
       return rc;
   }
 
@@ -1477,72 +1478,55 @@ static int wm_backward_impl(tdmpc2_planner* p, const tdmpc2_weights* w, const fl
   za.dxd = ws + W.dxd; za.ld = LT; za.dxt = d.episodic ? ws + W.dxt : nullptr; za.ldt = Lz;
   za.cons = cf->consistency * 2.f / (fH * fB * static_cast<float>(Lz)); za.rho = cf->rho; za.H = H; za.Bsz = B;
   za.L = static_cast<int>(Lz); za.dz = ws + W.dz;
-  const int dz_blocks = static_cast<int>((B * Lz + 255) / 256), b8 = (B + 7) / 8;
+  const int dz_blocks = static_cast<int>((B * Lz + 255) / 256);
   for (int t = H; t >= 1; --t) {
     za.t = t;
     pl_dz_step<<<dz_blocks, 256, 0, st>>>(za);
-    if ((rc = ok())) return rc;
+    if ((rc = launch_ok())) return rc;
     const size_t r0 = static_cast<size_t>(t - 1) * B;
     const float* tseg = tape + tp.dyn + r0 * tp.p_dyn;
-    LnBackArgs lb{};
-    lb.tape = tseg; lb.pitch = tp.p_dyn; lb.rows = B; lb.off = static_cast<int>(2 * M); lb.N = static_cast<int>(Lz); lb.ld = Lz;
-    lb.g = ws + W.dz; lb.out = ws + W.dp2 + r0 * Lz; lb.gamma = w->dynamics[2].ln_weight; lb.beta = w->dynamics[2].ln_bias;
-    lb.dyn = ws + W.dyn2 + r0 * Lz; lb.dy = ws + W.dy2 + r0 * Lz;
-    pl_ln_simnorm_back<<<b8, 256, 0, st>>>(lb, d.simnorm_dim);
-    if ((rc = ok())) return rc;
-    if ((rc = dinput(ws + W.dp2 + r0 * Lz, Lz, w->dynamics[2].weight, M, 0, nullptr, 1, M, ws + W.dp1 + r0 * M, M, 0, B))) return rc;
-    lb.off = static_cast<int>(M); lb.N = static_cast<int>(M); lb.ld = M; lb.g = lb.out = ws + W.dp1 + r0 * M;
-    lb.gamma = w->dynamics[1].ln_weight; lb.beta = w->dynamics[1].ln_bias;
-    lb.dyn = ws + W.dyn1 + r0 * M; lb.dy = ws + W.dy1 + r0 * M; lb.h = ws + W.h1 + r0 * M;
-    pl_ln_back<<<b8, 256, 0, st>>>(lb);
-    if ((rc = ok())) return rc;
-    if ((rc = dinput(ws + W.dp1 + r0 * M, M, w->dynamics[1].weight, M, 0, nullptr, 1, M, ws + W.dp0 + r0 * M, M, 0, B))) return rc;
-    lb.off = 0; lb.g = lb.out = ws + W.dp0 + r0 * M; lb.gamma = w->dynamics[0].ln_weight; lb.beta = w->dynamics[0].ln_bias;
-    lb.dyn = ws + W.dyn0 + r0 * M; lb.dy = ws + W.dy0 + r0 * M; lb.h = ws + W.h0 + r0 * M;
-    pl_ln_back<<<b8, 256, 0, st>>>(lb);
-    if ((rc = ok())) return rc;
-    if ((rc = dinput(ws + W.dp0 + r0 * M, M, w->dynamics[0].weight, D, 0, nullptr, 1, LT, ws + W.dxd + r0 * LT, LT, 0, B))) return rc;
+    float *dp2 = ws + W.dp2 + r0 * Lz, *dp1 = ws + W.dp1 + r0 * M, *dp0 = ws + W.dp0 + r0 * M;
+    if ((rc = bw.ln_simnorm_back(tseg, tp.p_dyn, 2 * M, B, Lz, w->dynamics[2], ws + W.dz, dp2, ws + W.dyn2 + r0 * Lz,
+                                 ws + W.dy2 + r0 * Lz, d.simnorm_dim)) ||
+        (rc = bw.dinput(dp2, Lz, w->dynamics[2].weight, M, 0, nullptr, 1, M, dp1, M, 0, B)) ||
+        (rc = bw.ln_back(tseg, tp.p_dyn, M, B, M, w->dynamics[1], dp1, ws + W.dyn1 + r0 * M, ws + W.dy1 + r0 * M, ws + W.h1 + r0 * M)) ||
+        (rc = bw.dinput(dp1, M, w->dynamics[1].weight, M, 0, nullptr, 1, M, dp0, M, 0, B)) ||
+        (rc = bw.ln_back(tseg, tp.p_dyn, 0, B, M, w->dynamics[0], dp0, ws + W.dyn0 + r0 * M, ws + W.dy0 + r0 * M, ws + W.h0 + r0 * M)) ||
+        (rc = bw.dinput(dp0, M, w->dynamics[0].weight, D, 0, nullptr, 1, LT, ws + W.dxd + r0 * LT, LT, 0, B)))
+      return rc;
   }
   za.t = 0;
   pl_dz_step<<<dz_blocks, 256, 0, st>>>(za);
-  if ((rc = ok())) return rc;
+  if ((rc = launch_ok())) return rc;
 
   // ---- 3. the dynamics' parameter gradients: one reduction over all H B taped rows per layer
   const tdmpc2_linear_grad* gd = gr->dynamics;
-  if ((rc = dweight(ws + W.dp2, Lz, ws + W.h1, M, M, R, gd[2].weight)) || (rc = colsum(ws + W.dp2, R, Lz, Lz, gd[2].bias)) ||
-      (rc = colsum(ws + W.dyn2, R, Lz, Lz, gd[2].ln_weight)) || (rc = colsum(ws + W.dy2, R, Lz, Lz, gd[2].ln_bias)) ||
-      (rc = dweight(ws + W.dp1, M, ws + W.h0, M, M, R, gd[1].weight)) || (rc = colsum(ws + W.dp1, R, M, M, gd[1].bias)) ||
-      (rc = colsum(ws + W.dyn1, R, M, M, gd[1].ln_weight)) || (rc = colsum(ws + W.dy1, R, M, M, gd[1].ln_bias)) ||
-      (rc = dweight(ws + W.dp0, M, X, D, D, R, gd[0].weight)) || (rc = colsum(ws + W.dp0, R, M, M, gd[0].bias)) ||
-      (rc = colsum(ws + W.dyn0, R, M, M, gd[0].ln_weight)) || (rc = colsum(ws + W.dy0, R, M, M, gd[0].ln_bias)))
+  if ((rc = bw.dweight(ws + W.dp2, Lz, ws + W.h1, M, M, R, gd[2].weight)) || (rc = bw.colsum(ws + W.dp2, R, Lz, Lz, gd[2].bias)) ||
+      (rc = bw.colsum(ws + W.dyn2, R, Lz, Lz, gd[2].ln_weight)) || (rc = bw.colsum(ws + W.dy2, R, Lz, Lz, gd[2].ln_bias)) ||
+      (rc = bw.dweight(ws + W.dp1, M, ws + W.h0, M, M, R, gd[1].weight)) || (rc = bw.colsum(ws + W.dp1, R, M, M, gd[1].bias)) ||
+      (rc = bw.colsum(ws + W.dyn1, R, M, M, gd[1].ln_weight)) || (rc = bw.colsum(ws + W.dy1, R, M, M, gd[1].ln_bias)) ||
+      (rc = bw.dweight(ws + W.dp0, M, X, D, D, R, gd[0].weight)) || (rc = bw.colsum(ws + W.dp0, R, M, M, gd[0].bias)) ||
+      (rc = bw.colsum(ws + W.dyn0, R, M, M, gd[0].ln_weight)) || (rc = bw.colsum(ws + W.dy0, R, M, M, gd[0].ln_bias)))
     return rc;
 
   if (latent) CUDA_TRY(cudaMemcpyAsync(dz0, ws + W.dz, static_cast<size_t>(B) * Lz * 4, cudaMemcpyDeviceToDevice, st));
   // ---- 4. dz_0 through the encoder: the SimNorm layer, then the Mish layers down to layer 0 (input [obs | emb])
   if (!latent) {
     const int ne = p->num_enc;
+    const float* te = tape + tp.enc;
     float *cur = ws + W.ea, *nxt = ws + W.eb;
-    LnBackArgs lb{};
-    lb.tape = tape + tp.enc; lb.pitch = tp.p_enc; lb.rows = B; lb.off = static_cast<int>((ne - 1) * E); lb.N = static_cast<int>(Lz);
-    lb.ld = Lz; lb.g = ws + W.dz; lb.out = cur; lb.gamma = w->enc[ne - 1].ln_weight; lb.beta = w->enc[ne - 1].ln_bias;
-    lb.dyn = ws + W.edyn; lb.dy = ws + W.edy;
-    pl_ln_simnorm_back<<<b8, 256, 0, st>>>(lb, d.simnorm_dim);
-    if ((rc = ok())) return rc;
-    if ((rc = colsum(ws + W.edyn, B, Lz, Lz, gr->enc[ne - 1].ln_weight)) || (rc = colsum(ws + W.edy, B, Lz, Lz, gr->enc[ne - 1].ln_bias)) ||
-        (rc = colsum(cur, B, Lz, Lz, gr->enc[ne - 1].bias)))
+    if ((rc = bw.ln_simnorm_back(te, tp.p_enc, (ne - 1) * E, B, Lz, w->enc[ne - 1], ws + W.dz, cur, ws + W.edyn, ws + W.edy,
+                                 d.simnorm_dim)) ||
+        (rc = bw.colsum(ws + W.edyn, B, Lz, Lz, gr->enc[ne - 1].ln_weight)) ||
+        (rc = bw.colsum(ws + W.edy, B, Lz, Lz, gr->enc[ne - 1].ln_bias)) || (rc = bw.colsum(cur, B, Lz, Lz, gr->enc[ne - 1].bias)))
       return rc;
     long long n_cur = Lz;
     for (int i = ne - 2; i >= 0; --i) {
-      if ((rc = dinput(cur, n_cur, w->enc[i + 1].weight, E, 0, nullptr, 1, E, nxt, E, 0, B))) return rc;
-      LnBackArgs le{};
-      le.tape = tape + tp.enc; le.pitch = tp.p_enc; le.rows = B; le.off = static_cast<int>(i * E); le.N = static_cast<int>(E); le.ld = E;
-      le.g = le.out = nxt; le.gamma = w->enc[i].ln_weight; le.beta = w->enc[i].ln_bias;
-      le.dyn = ws + W.edyn; le.dy = ws + W.edy; le.h = ws + W.eh;
-      pl_ln_back<<<b8, 256, 0, st>>>(le);
-      if ((rc = ok())) return rc;
-      if ((rc = dweight(cur, n_cur, ws + W.eh, E, E, B, gr->enc[i + 1].weight)) ||
-          (rc = colsum(ws + W.edyn, B, E, E, gr->enc[i].ln_weight)) || (rc = colsum(ws + W.edy, B, E, E, gr->enc[i].ln_bias)) ||
-          (rc = colsum(nxt, B, E, E, gr->enc[i].bias)))
+      if ((rc = bw.dinput(cur, n_cur, w->enc[i + 1].weight, E, 0, nullptr, 1, E, nxt, E, 0, B)) ||
+          (rc = bw.ln_back(te, tp.p_enc, i * E, B, E, w->enc[i], nxt, ws + W.edyn, ws + W.edy, ws + W.eh)) ||
+          (rc = bw.dweight(cur, n_cur, ws + W.eh, E, E, B, gr->enc[i + 1].weight)) ||
+          (rc = bw.colsum(ws + W.edyn, B, E, E, gr->enc[i].ln_weight)) || (rc = bw.colsum(ws + W.edy, B, E, E, gr->enc[i].ln_bias)) ||
+          (rc = bw.colsum(nxt, B, E, E, gr->enc[i].bias)))
         return rc;
       std::swap(cur, nxt);
       n_cur = E;
@@ -1551,28 +1535,26 @@ static int wm_backward_impl(tdmpc2_planner* p, const tdmpc2_weights* w, const fl
     if (Tq > 0) {
       pl_gather_x<<<static_cast<int>((B * OT + 255) / 256), 256, 0, st>>>(obs0, p->base.emb, task, B, d.obs_dim, static_cast<int>(Tq),
                                                                          ws + W.ex);
-      if ((rc = ok())) return rc;
+      if ((rc = launch_ok())) return rc;
       xe = ws + W.ex;
     }
-    if ((rc = dweight(cur, n_cur, xe, OT, OT, B, gr->enc[0].weight))) return rc;
-    if (Tq > 0 && (rc = dinput(cur, n_cur, w->enc[0].weight + d.obs_dim, OT, 0, nullptr, 1, Tq, ws + W.exe + Lz, LT, 0, B)))
+    if ((rc = bw.dweight(cur, n_cur, xe, OT, OT, B, gr->enc[0].weight)) ||
+        (Tq > 0 && (rc = bw.dinput(cur, n_cur, w->enc[0].weight + d.obs_dim, OT, 0, nullptr, 1, Tq, ws + W.exe + Lz, LT, 0, B))))
       return rc;
   }
-  {
-    if (Tq > 0) {
-      // ---- 5. the task embedding: encoder layer 0 (without the latent variant), dynamics layer 0, reward layer 0, each Q
-      // head's layer 0, in order
-      CUDA_TRY(cudaMemsetAsync(ws + W.zero, 0, static_cast<size_t>(R) * LT * 4, st));
-      const float* z0 = ws + W.zero;
-      const dim3 eg(static_cast<int>((d.num_tasks * Tq + 127) / 128));
-      if (!latent) pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.exe + Lz, z0, z0, LT, task, B, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
-      pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.dxd + Lz, z0, z0, LT, task, R, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
-      pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.dxr + Lz, z0, z0, LT, task, R, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
-      for (int h = 0; h < nq; ++h)
-        pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.dxq + h * static_cast<long long>(R) * LT + Lz, z0, z0, LT, task, R, d.num_tasks,
-                                        static_cast<int>(Tq), gr->task_emb);
-      if ((rc = ok())) return rc;
-    }
+  if (Tq > 0) {
+    // ---- 5. the task embedding: encoder layer 0 (without the latent variant), dynamics layer 0, reward layer 0, each Q
+    // head's layer 0, in order
+    CUDA_TRY(cudaMemsetAsync(ws + W.zero, 0, static_cast<size_t>(R) * LT * 4, st));
+    const float* z0 = ws + W.zero;
+    const dim3 eg(static_cast<int>((d.num_tasks * Tq + 127) / 128));
+    if (!latent) pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.exe + Lz, z0, z0, LT, task, B, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
+    pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.dxd + Lz, z0, z0, LT, task, R, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
+    pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.dxr + Lz, z0, z0, LT, task, R, d.num_tasks, static_cast<int>(Tq), gr->task_emb);
+    for (int h = 0; h < nq; ++h)
+      pl_emb_grad<<<eg, 128, 0, st>>>(ws + W.dxq + h * static_cast<long long>(R) * LT + Lz, z0, z0, LT, task, R, d.num_tasks,
+                                      static_cast<int>(Tq), gr->task_emb);
+    if ((rc = launch_ok())) return rc;
   }
   return 0;
 }
