@@ -35,13 +35,14 @@
 extern "C" {
 #endif
 
-#define TDMPC2_B200_ABI_VERSION 8   /* 2: tdmpc2_weights.termination, dims.episodic = 1 accepted; 3: a persisting-L2 knob;
+#define TDMPC2_B200_ABI_VERSION 9   /* 2: tdmpc2_weights.termination, dims.episodic = 1 accepted; 3: a persisting-L2 knob;
                                        4: tdmpc2_planner_set_passes (declared non-parity fast mode), reduction-segment knobs, engine query;
                                        5: pixel encoder (tdmpc2_pixel_*), tdmpc2_plan_prologue_latent, dims.num_enc_layers = 0;
                                        6: tdmpc2_plan_iter_rng (declared non-parity in-kernel noise), tdmpc2_debug_rng;
                                        7: world-model methods on a flat batch (tdmpc2_wm_*, tdmpc2_td_target), target Q blob, then
                                           agent.update_pi, agent._update of state and pixel models, the replay buffer's sampler;
-                                       8: removed engines 2-4, the engine query, the L2 and reduction-segment knobs; one tdmpc2_pixel_encode */
+                                       8: removed engines 2-4, the engine query, the L2 and reduction-segment knobs; one tdmpc2_pixel_encode;
+                                       9: the _latent calls folded in: tdmpc2_plan_prologue's z, tdmpc2_wm_loss_* with obs0 NULL and dz0 */
 #define TDMPC2_MAX_ENC_LAYERS 8
 
 typedef enum tdmpc2_status {
@@ -144,16 +145,14 @@ int tdmpc2_pack_weights(tdmpc2_planner* p, const tdmpc2_weights* w, void* stream
 /* ---- the hot path -------------------------------------------------------- */
 /* Replaces tdmpc2.py:153-170: z = encode(obs, task); the P policy-prior
  * trajectories; mean/std initialisation incl. the warm start from _prev_mean.
- *   obs [E, obs_dim]; task [E] int32 or NULL (single-task); t0 [E] uint8;
+ *   obs [E, obs_dim] or z [E, L]: exactly one is non-NULL (else TDMPC2_ERR_INVALID).  z is the latent given, in place
+ *   of encode(obs, task): models without a state encoder (dims.num_enc_layers = 0; cfg.obs == 'rgb': z comes from
+ *   tdmpc2_pixel_encode) pass z, and obs on such a planner is TDMPC2_ERR_STATE;
+ *   task [E] int32 or NULL (single-task); t0 [E] uint8;
  *   prev_mean [E, H, A]; noise_prior [E, H, P, A] (draw 1 of SURVEY 8(a)). */
-int tdmpc2_plan_prologue(tdmpc2_planner* p, const float* obs, const int32_t* task,
+int tdmpc2_plan_prologue(tdmpc2_planner* p, const float* obs, const float* z, const int32_t* task,
                          const uint8_t* t0, const float* prev_mean,
                          const float* noise_prior, void* stream);
-/* The same with the latent given: z [E, L] replaces encode(obs, task).  For models without a state encoder
- * (dims.num_enc_layers = 0; cfg.obs == 'rgb': z comes from tdmpc2_pixel_encode). */
-int tdmpc2_plan_prologue_latent(tdmpc2_planner* p, const float* z, const int32_t* task,
-                                const uint8_t* t0, const float* prev_mean,
-                                const float* noise_prior, void* stream);
 
 /* DECLARED NON-PARITY throughput mode of tdmpc2_plan_iter: the two large noise tensors (tdmpc2.py:176, world_model.py:156) are
  * generated inside the kernel -- Philox4x32-10 + Box-Muller under rng_state = {seed, plan counter} (device memory, uint64[2];
@@ -313,14 +312,14 @@ int tdmpc2_pi_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const fl
                             const float* eps, const int32_t* qidx, const float* dropout_mask, int T, int B, const float* scale,
                             float entropy_coef, float rho, const tdmpc2_pi_grads* grads, void* workspace, void* stream);
 
-/* ---- agent._update: the world model's loss (tdmpc2.py:259-313), state observations ------------------------------
+/* ---- agent._update: the world model's loss (tdmpc2.py:259-313), state and pixel observations --------------------
  * forward: the latent rollout of a [H + 1, B] batch (row r of a [H, B] batch is t B + b), as row launches that also
  * write the caller-owned tape [tape_bytes] (the pre-LayerNorm row of every LayerNorm layer, DESIGN section 4.4):
  *   encode(obs0 [B, obs_dim]) -> zs[0]; next(zs[t], action[t]) -> zs[t + 1] for t < H, written in place into
  *   zs [H + 1, B, L]; Q 'all' on (zs[:H], action) with dropout_mask (NULL: eval mode; else [num_q, H B, mlp_dim] of
  *   mask / (1 - p) on each head's layer 0) -> q_logits [num_q, H B, num_bins]; reward(zs[:H], action) -> reward_logits
  *   [H B, num_bins]; episodic models: termination(zs[1:]) -> term_logits [H B] (else NULL).
- *   task: NULL (single-task) or [H B] per-row task indices.  Pixel models (no state encoder): TDMPC2_ERR_UNSUPPORTED.
+ *   task: NULL (single-task) or [H B] per-row task indices.  Pixel models pass obs0 = NULL (below).
  * backward: from the tape, the forward's inputs and outputs, next_z [H, B, L] (encode(obs[1:])), reward / td_target /
  *   terminated [H B] and the loss coefficients, ADDS dL/dparameter of
  *     consistency * sum_t rho^t mse(zs[t+1], next_z[t]) / H + reward * sum_t rho^t soft_ce(reward logits, r_t).mean() / H
@@ -356,21 +355,13 @@ int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const fl
                             const float* action, const int32_t* task, const float* dropout_mask, int H, int B,
                             const float* zs, const float* q_logits, const float* reward_logits, const float* term_logits,
                             const float* next_z, const float* reward, const float* td_target, const float* terminated,
-                            const tdmpc2_wm_loss_coefs* coefs, const tdmpc2_wm_grads* grads, void* workspace, void* stream);
-/* Planners without a state encoder (pixel models, num_enc_layers = 0) get TDMPC2_ERR_UNSUPPORTED from the two calls above;
- * they use these.  _latent forward: zs[0] ([B, L]) is the caller's, written by a taped tdmpc2_pixel_encode; the rest as
- * tdmpc2_wm_loss_forward.  _latent backward: as tdmpc2_wm_loss_backward without the state encoder (grads->enc and
- * w->enc are not read), and dL/dz_0 [B, L] is written to dz0, for tdmpc2_pixel_encode_backward.  tape_bytes and
- * workspace_bytes answer for both variants. */
-int tdmpc2_wm_loss_forward_latent(tdmpc2_planner* p, const float* action, const int32_t* task, const float* dropout_mask,
-                                  int H, int B, float* zs, float* q_logits, float* reward_logits, float* term_logits,
-                                  float* tape, void* stream);
-int tdmpc2_wm_loss_backward_latent(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* action,
-                                   const int32_t* task, const float* dropout_mask, int H, int B, const float* zs,
-                                   const float* q_logits, const float* reward_logits, const float* term_logits,
-                                   const float* next_z, const float* reward, const float* td_target, const float* terminated,
-                                   const tdmpc2_wm_loss_coefs* coefs, const tdmpc2_wm_grads* grads, float* dz0,
-                                   void* workspace, void* stream);
+                            const tdmpc2_wm_loss_coefs* coefs, const tdmpc2_wm_grads* grads, float* dz0, void* workspace,
+                            void* stream);
+/* obs0 NULL: z_0 comes from elsewhere (pixel models, num_enc_layers = 0: a taped tdmpc2_pixel_encode of obs[0]).  The
+ * forward then reads zs[0] ([B, L]) as the caller wrote it and skips the encoder; the backward skips the state encoder
+ * (grads->enc and w->enc are not read) and writes dL/dz_0 [B, L] to dz0, for tdmpc2_pixel_encode_backward.  Valid on
+ * any planner.  dz0 must be non-NULL exactly when obs0 is NULL, else TDMPC2_ERR_INVALID.  A non-NULL obs0 on a planner
+ * without a state encoder: TDMPC2_ERR_UNSUPPORTED.  tape_bytes and workspace_bytes answer for both uses. */
 
 /* ---- replay buffer: Buffer.sample (common/buffer.py:93-115, torchrl SliceSampler with strict_length) -------------
  * One launch gathers B slices of H + 1 consecutive steps from circular [capacity, ...] storages into the layout of

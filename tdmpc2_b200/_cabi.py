@@ -12,13 +12,13 @@ LIB_PATH = os.environ.get("TDMPC2_B200_LIB") or os.path.join(HERE, "libtdmpc2_b2
 MAX_ENC_LAYERS = 8
 ENGINE_TCGEN05, ENGINE_SIMT = 0, 1     # tdmpc2_engine
 Q_ALL, Q_MIN, Q_AVG = 0, 1, 2   # tdmpc2_q_return
-ABI_VERSION = 8            # TDMPC2_B200_ABI_VERSION of include/tdmpc2_b200.h this binding was written against
+ABI_VERSION = 9            # TDMPC2_B200_ABI_VERSION of include/tdmpc2_b200.h this binding was written against
 
 # every symbol include/tdmpc2_b200.h declares
 SYMBOLS = [
     "tdmpc2_abi_version", "tdmpc2_last_error", "tdmpc2_planner_create", "tdmpc2_planner_destroy",
     "tdmpc2_planner_packed_bytes", "tdmpc2_planner_workspace_bytes", "tdmpc2_planner_bind",
-    "tdmpc2_planner_set_engine", "tdmpc2_planner_set_passes", "tdmpc2_pack_weights", "tdmpc2_plan_prologue", "tdmpc2_plan_prologue_latent",
+    "tdmpc2_planner_set_engine", "tdmpc2_planner_set_passes", "tdmpc2_pack_weights", "tdmpc2_plan_prologue",
     "tdmpc2_pixel_encoder_create", "tdmpc2_pixel_encoder_destroy", "tdmpc2_pixel_encoder_workspace_bytes", "tdmpc2_pixel_encode", "tdmpc2_plan_iter", "tdmpc2_plan_iter_rng", "tdmpc2_debug_rng",
     "tdmpc2_plan_epilogue", "tdmpc2_plan_get_state", "tdmpc2_estimate_value", "tdmpc2_debug_layer",
     "tdmpc2_planner_layer_count", "tdmpc2_planner_launch_count", "tdmpc2_planner_set_profile",
@@ -27,8 +27,7 @@ SYMBOLS = [
     "tdmpc2_td_target", "tdmpc2_pi_loss_tape_bytes", "tdmpc2_pi_loss_workspace_bytes", "tdmpc2_pi_loss_forward",
     "tdmpc2_pi_loss_backward", "tdmpc2_wm_loss_tape_bytes", "tdmpc2_wm_loss_workspace_bytes", "tdmpc2_wm_loss_forward",
     "tdmpc2_wm_loss_backward", "tdmpc2_pixel_encode_tape_bytes",
-    "tdmpc2_pixel_backward_workspace_bytes", "tdmpc2_pixel_encode_backward", "tdmpc2_wm_loss_forward_latent",
-    "tdmpc2_wm_loss_backward_latent", "tdmpc2_buffer_sample",
+    "tdmpc2_pixel_backward_workspace_bytes", "tdmpc2_pixel_encode_backward", "tdmpc2_buffer_sample",
 ]
 
 
@@ -120,8 +119,7 @@ def load():
     lib.tdmpc2_planner_set_engine.argtypes = [vp, C.c_int]
     lib.tdmpc2_planner_set_passes.argtypes = [vp, C.c_int]
     lib.tdmpc2_pack_weights.argtypes = [vp, C.POINTER(Weights), vp]
-    lib.tdmpc2_plan_prologue.argtypes = [vp, vp, vp, vp, vp, vp, vp]
-    lib.tdmpc2_plan_prologue_latent.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.tdmpc2_plan_prologue.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     lib.tdmpc2_pixel_encoder_create.argtypes = [C.POINTER(PixelDims), C.POINTER(vp)]
     lib.tdmpc2_pixel_encoder_destroy.argtypes = [vp]
     lib.tdmpc2_pixel_encoder_destroy.restype = None
@@ -157,14 +155,11 @@ def load():
     lib.tdmpc2_wm_loss_workspace_bytes.argtypes = [vp, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
     lib.tdmpc2_wm_loss_forward.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
     lib.tdmpc2_wm_loss_backward.argtypes = [vp, C.POINTER(Weights), vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp,
-                                            vp, vp, C.POINTER(WmLossCoefs), C.POINTER(WmGrads), vp, vp]
+                                            vp, vp, C.POINTER(WmLossCoefs), C.POINTER(WmGrads), vp, vp, vp]
     lib.tdmpc2_pixel_encode_tape_bytes.argtypes = [vp, i64, C.POINTER(C.c_size_t)]
     lib.tdmpc2_pixel_backward_workspace_bytes.argtypes = [vp, i64, C.POINTER(C.c_size_t)]
     lib.tdmpc2_pixel_encode_backward.argtypes = [vp, C.POINTER(ConvWeights), vp, vp, vp, i64, vp, vp, vp, C.POINTER(ConvGrads),
                                                  vp, vp]
-    lib.tdmpc2_wm_loss_forward_latent.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
-    lib.tdmpc2_wm_loss_backward_latent.argtypes = [vp, C.POINTER(Weights), vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp,
-                                                   vp, vp, vp, C.POINTER(WmLossCoefs), C.POINTER(WmGrads), vp, vp, vp]
     lib.tdmpc2_buffer_sample.argtypes = [C.POINTER(BufferField), C.c_int, i64, vp, vp, i64, vp, vp, C.c_int, C.c_int, vp]
     _lib = lib
     return lib

@@ -267,7 +267,7 @@ extern "C" int tdmpc2_planner_create(const tdmpc2_dims* dims, tdmpc2_planner** o
     return static_cast<int>(p->layers.size()) - 1;
   };
   // encoder: mlp(obs+T, n_hidden*[enc_dim], L, act=SimNorm)  (layers.py:157-159); num_enc_layers == 0: the model has no
-  // state encoder (pixel observations: tdmpc2_pixel_encode + tdmpc2_plan_prologue_latent supply the latent)
+  // state encoder (pixel observations: tdmpc2_pixel_encode supplies the latent, tdmpc2_plan_prologue's z)
   p->num_enc = d.num_enc_layers == 0 ? 0 : n_hidden + 1;
   p->li_enc = static_cast<int>(p->layers.size());
   if (p->num_enc > 0) { int k = d.obs_dim + T; for (int i = 0; i < n_hidden; ++i) { add(k, d.enc_dim, true); k = d.enc_dim; } add(k, L, true); }
@@ -571,13 +571,14 @@ static int ready(tdmpc2_planner* p) {
 }
 
 // obs != nullptr: z = encode(obs, task) through the state encoder; z_in != nullptr: the latent is given (pixel models)
-static int prologue_impl(tdmpc2_planner* p, const float* obs, const float* z_in, const int32_t* task, const uint8_t* t0,
-                         const float* prev_mean, const float* noise_prior, void* stream_) {
+extern "C" int tdmpc2_plan_prologue(tdmpc2_planner* p, const float* obs, const float* z_in, const int32_t* task, const uint8_t* t0,
+                                    const float* prev_mean, const float* noise_prior, void* stream_) {
+  if (!obs == !z_in) return fail(TDMPC2_ERR_INVALID, "exactly one of obs and z must be non-NULL");
   int rc = ready(p);
   if (rc) return rc;
   const tdmpc2_dims& d = p->d;
-  if ((!obs && !z_in) || !t0 || !prev_mean) return fail(TDMPC2_ERR_INVALID, "null argument");
-  if (obs && p->num_enc == 0) return fail(TDMPC2_ERR_STATE, "this planner was created without a state encoder (num_enc_layers = 0): use tdmpc2_plan_prologue_latent");
+  if (!t0 || !prev_mean) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (obs && p->num_enc == 0) return fail(TDMPC2_ERR_STATE, "this planner was created without a state encoder (num_enc_layers = 0): pass z, not obs");
   if (d.task_dim > 0 && !task) return fail(TDMPC2_ERR_INVALID, "multi-task model needs task indices");
   if (d.num_pi_trajs > 0 && !noise_prior) return fail(TDMPC2_ERR_INVALID, "noise_prior is required when num_pi_trajs > 0");
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
@@ -614,17 +615,6 @@ static int prologue_impl(tdmpc2_planner* p, const float* obs, const float* z_in,
     if ((rc = launch(p, prm, st))) return rc;
   }
   return 0;
-}
-
-extern "C" int tdmpc2_plan_prologue(tdmpc2_planner* p, const float* obs, const int32_t* task, const uint8_t* t0,
-                                    const float* prev_mean, const float* noise_prior, void* stream_) {
-  if (!obs) return fail(TDMPC2_ERR_INVALID, "null argument");
-  return prologue_impl(p, obs, nullptr, task, t0, prev_mean, noise_prior, stream_);
-}
-extern "C" int tdmpc2_plan_prologue_latent(tdmpc2_planner* p, const float* z, const int32_t* task, const uint8_t* t0,
-                                           const float* prev_mean, const float* noise_prior, void* stream_) {
-  if (!z) return fail(TDMPC2_ERR_INVALID, "null argument");
-  return prologue_impl(p, nullptr, z, task, t0, prev_mean, noise_prior, stream_);
 }
 
 // ------------------------------------------------------------------------------------ pixel encoder (cfg.obs == 'rgb')
@@ -1326,8 +1316,8 @@ static int wm_dims_ok(const tdmpc2_planner* p, int H, int B) {
 }
 static int wm_needs_encoder(const tdmpc2_planner* p) {
   if (p->num_enc == 0)
-    return fail(TDMPC2_ERR_UNSUPPORTED, "this planner has no state encoder (pixel model): use tdmpc2_wm_loss_forward_latent / "
-                                        "tdmpc2_wm_loss_backward_latent with a taped tdmpc2_pixel_encode / tdmpc2_pixel_encode_backward");
+    return fail(TDMPC2_ERR_UNSUPPORTED, "this planner has no state encoder (pixel model): pass obs0 = NULL, with zs[0] from a taped "
+                                        "tdmpc2_pixel_encode and dz0 for tdmpc2_pixel_encode_backward");
   return 0;
 }
 
@@ -1347,13 +1337,14 @@ extern "C" int tdmpc2_wm_loss_workspace_bytes(const tdmpc2_planner* p, int H, in
   return 0;
 }
 
-// latent: zs[0] is the caller's (the pixel encoder wrote it), and the ENCODE launch is skipped
-static int wm_forward_impl(tdmpc2_planner* p, bool latent, const float* obs0, const float* action, const int32_t* task,
-                           const float* dropout_mask, int H, int B, float* zs, float* q_logits, float* reward_logits,
-                           float* term_logits, float* tape, void* stream_) {
+// obs0 == nullptr (latent): zs[0] is the caller's (the pixel encoder wrote it), and the ENCODE launch is skipped
+extern "C" int tdmpc2_wm_loss_forward(tdmpc2_planner* p, const float* obs0, const float* action, const int32_t* task,
+                                      const float* dropout_mask, int H, int B, float* zs, float* q_logits, float* reward_logits,
+                                      float* term_logits, float* tape, void* stream_) {
+  const bool latent = obs0 == nullptr;
   int rc = rows_ready(p, B);
   if (rc || (rc = wm_dims_ok(p, H, B)) || (!latent && (rc = wm_needs_encoder(p))) || (rc = need_task(p, task))) return rc;
-  if ((!latent && !obs0) || !action || !zs || !q_logits || !reward_logits || !tape) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (!action || !zs || !q_logits || !reward_logits || !tape) return fail(TDMPC2_ERR_INVALID, "null argument");
   if (p->d.episodic && !term_logits) return fail(TDMPC2_ERR_INVALID, "episodic model needs term_logits");
   const tdmpc2_dims& d = p->d;
   const int R = H * B;
@@ -1388,32 +1379,22 @@ static int wm_forward_impl(tdmpc2_planner* p, bool latent, const float* obs0, co
   return 0;
 }
 
-extern "C" int tdmpc2_wm_loss_forward(tdmpc2_planner* p, const float* obs0, const float* action, const int32_t* task,
-                                      const float* dropout_mask, int H, int B, float* zs, float* q_logits, float* reward_logits,
-                                      float* term_logits, float* tape, void* stream_) {
-  return wm_forward_impl(p, false, obs0, action, task, dropout_mask, H, B, zs, q_logits, reward_logits, term_logits, tape, stream_);
-}
-
-extern "C" int tdmpc2_wm_loss_forward_latent(tdmpc2_planner* p, const float* action, const int32_t* task,
-                                             const float* dropout_mask, int H, int B, float* zs, float* q_logits,
-                                             float* reward_logits, float* term_logits, float* tape, void* stream_) {
-  return wm_forward_impl(p, true, nullptr, action, task, dropout_mask, H, B, zs, q_logits, reward_logits, term_logits, tape, stream_);
-}
-
 static bool lin_ok(const tdmpc2_linear& l, bool ln) { return l.weight && l.bias && (!ln || (l.ln_weight && l.ln_bias)); }
 static bool grad_ok(const tdmpc2_linear_grad& g, bool ln) { return g.weight && g.bias && (!ln || (g.ln_weight && g.ln_bias)); }
 
-// dz0 != nullptr (latent): step 4 (the state encoder) is skipped and dL/dz_0 [B, L] is copied to dz0 instead
-static int wm_backward_impl(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* obs0,
-                            const float* action, const int32_t* task, const float* dropout_mask, int H, int B,
-                            const float* zs, const float* q_logits, const float* reward_logits, const float* term_logits,
-                            const float* next_z, const float* reward, const float* td_target, const float* terminated,
-                            const tdmpc2_wm_loss_coefs* cf, const tdmpc2_wm_grads* gr, float* dz0, void* workspace, void* stream_) {
-  const bool latent = dz0 != nullptr;
+// obs0 == nullptr (latent): step 4 (the state encoder) is skipped and dL/dz_0 [B, L] is copied to dz0 instead
+extern "C" int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* obs0,
+                                       const float* action, const int32_t* task, const float* dropout_mask, int H, int B,
+                                       const float* zs, const float* q_logits, const float* reward_logits, const float* term_logits,
+                                       const float* next_z, const float* reward, const float* td_target, const float* terminated,
+                                       const tdmpc2_wm_loss_coefs* cf, const tdmpc2_wm_grads* gr, float* dz0, void* workspace,
+                                       void* stream_) {
+  const bool latent = obs0 == nullptr;
   int rc = rows_ready(p, B);
   if (rc || (rc = wm_dims_ok(p, H, B)) || (!latent && (rc = wm_needs_encoder(p))) || (rc = need_task(p, task))) return rc;
+  if (latent != (dz0 != nullptr)) return fail(TDMPC2_ERR_INVALID, "dz0 must be non-NULL exactly when obs0 is NULL");
   const tdmpc2_dims& d = p->d;
-  if (!w || !tape || (!latent && !obs0) || !action || !zs || !q_logits || !reward_logits || !next_z || !reward || !td_target || !cf || !gr ||
+  if (!w || !tape || !action || !zs || !q_logits || !reward_logits || !next_z || !reward || !td_target || !cf || !gr ||
       !workspace)
     return fail(TDMPC2_ERR_INVALID, "null argument");
   if (d.episodic && (!term_logits || !terminated)) return fail(TDMPC2_ERR_INVALID, "episodic model needs term_logits and terminated");
@@ -1557,26 +1538,6 @@ static int wm_backward_impl(tdmpc2_planner* p, const tdmpc2_weights* w, const fl
     if ((rc = launch_ok())) return rc;
   }
   return 0;
-}
-
-extern "C" int tdmpc2_wm_loss_backward(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* obs0,
-                                       const float* action, const int32_t* task, const float* dropout_mask, int H, int B,
-                                       const float* zs, const float* q_logits, const float* reward_logits, const float* term_logits,
-                                       const float* next_z, const float* reward, const float* td_target, const float* terminated,
-                                       const tdmpc2_wm_loss_coefs* cf, const tdmpc2_wm_grads* gr, void* workspace, void* stream_) {
-  return wm_backward_impl(p, w, tape, obs0, action, task, dropout_mask, H, B, zs, q_logits, reward_logits, term_logits, next_z,
-                          reward, td_target, terminated, cf, gr, nullptr, workspace, stream_);
-}
-
-extern "C" int tdmpc2_wm_loss_backward_latent(tdmpc2_planner* p, const tdmpc2_weights* w, const float* tape, const float* action,
-                                              const int32_t* task, const float* dropout_mask, int H, int B, const float* zs,
-                                              const float* q_logits, const float* reward_logits, const float* term_logits,
-                                              const float* next_z, const float* reward, const float* td_target,
-                                              const float* terminated, const tdmpc2_wm_loss_coefs* cf, const tdmpc2_wm_grads* gr,
-                                              float* dz0, void* workspace, void* stream_) {
-  if (!dz0) return fail(TDMPC2_ERR_INVALID, "null argument");
-  return wm_backward_impl(p, w, tape, nullptr, action, task, dropout_mask, H, B, zs, q_logits, reward_logits, term_logits, next_z,
-                          reward, td_target, terminated, cf, gr, dz0, workspace, stream_);
 }
 
 // ------------------------------------------------------------------------------------ replay buffer: Buffer.sample

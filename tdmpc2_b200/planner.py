@@ -329,11 +329,18 @@ class Planner:
                 t.record_stream(stream)
 
     # ------------------------------------------------------------------ hot path
-    def prologue(self, obs, task, t0, prev_mean, noise_prior) -> None:
-        self._keep = [obs, task, t0, prev_mean, noise_prior]
+    def prologue(self, obs, task, t0, prev_mean, noise_prior, z=None) -> None:
+        """obs [E, obs_dim], or obs None and z [E, L] the latent given in place of encode(obs) (pixel models)."""
+        self._keep = [obs, z, task, t0, prev_mean, noise_prior]
         with torch.cuda.device(self.device):
-            _cabi.check(self.lib.tdmpc2_plan_prologue(self.h, _ptr(obs), _ptr(task), _ptr(t0), _ptr(prev_mean),
+            _cabi.check(self.lib.tdmpc2_plan_prologue(self.h, _ptr(obs), _ptr(z), _ptr(task), _ptr(t0), _ptr(prev_mean),
                                                       _ptr(noise_prior), self._stream()))
+
+    def _prologue_obs(self, obs, shift, task, t0, prev_mean, noise_prior) -> None:
+        """prologue() on the planning chain's observations: pixel models encode the frames (ShiftAug shifts `shift`) into
+        the static pix_z that a captured graph reads, and pass that as z."""
+        z = self.encode_pixel_rows(obs, shift, out=self.pix_z) if self.rgb else None
+        self.prologue(None if self.rgb else obs, task, t0, prev_mean, noise_prior, z=z)
 
     def encode_pixel_rows(self, frames, shift, out=None) -> torch.Tensor:
         """z = encode(obs) for any number of pixel frames in one launch: frames [R, C, 64, 64] (any dtype, values 0..255),
@@ -380,12 +387,6 @@ class Planner:
                                                               R, _ptr(tape), _ptr(z), _ptr(dz), C.byref(G), _ptr(ws),
                                                               self._stream()))
 
-    def prologue_latent(self, z, task, t0, prev_mean, noise_prior) -> None:
-        self._keep = [z, task, t0, prev_mean, noise_prior]
-        with torch.cuda.device(self.device):
-            _cabi.check(self.lib.tdmpc2_plan_prologue_latent(self.h, _ptr(z), _ptr(task), _ptr(t0), _ptr(prev_mean),
-                                                             _ptr(noise_prior), self._stream()))
-
     def iterate(self, noise_r, noise_pi, qidx, values_out=None, elite_idx_out=None) -> None:
         with torch.cuda.device(self.device):
             _cabi.check(self.lib.tdmpc2_plan_iter(self.h, _ptr(noise_r), _ptr(noise_pi), _ptr(qidx),
@@ -417,10 +418,7 @@ class Planner:
     def _launch_chain(self, obs, task, t0, prev_mean, noise: Noise, action, new_mean, tr=None) -> None:
         """prologue -> I x iter -> epilogue on the current stream (10 launches for I = 6)."""
         cfg, E, dev = self.cfg, self.E, self.device
-        if self.rgb:
-            self.prologue_latent(self.encode_pixel_rows(obs, noise.shift, out=self.pix_z), task, t0, prev_mean, noise.prior)
-        else:
-            self.prologue(obs, task, t0, prev_mean, noise.prior)
+        self._prologue_obs(obs, noise.shift, task, t0, prev_mean, noise.prior)
         if tr is not None:
             st = self.get_state()
             tr["z"], tr["pi_actions"] = st["z"], st["pi_actions"]
@@ -521,10 +519,7 @@ class Planner:
             for t in range(H if P > 0 else 0):                                        # tdmpc2.py:153
                 nz.prior[0, t] = torch.randn(P, A, **kw)
             main.wait_event(side.record_event())
-        if self.rgb:
-            self.prologue_latent(self.encode_pixel_rows(obs, nz.shift, out=self.pix_z), task, t0, prev_mean, nz.prior)
-        else:
-            self.prologue(obs, task, t0, prev_mean, nz.prior)
+        self._prologue_obs(obs, nz.shift, task, t0, prev_mean, nz.prior)
         for it in range(I):
             with torch.cuda.stream(side):
                 nz.r[it, 0] = torch.randn(H, N - P, A, **kw)                          # tdmpc2.py:175
@@ -674,30 +669,22 @@ class Planner:
                                                          _ptr(qidx), _ptr(drop), T, B, _ptr(scale), float(entropy_coef),
                                                          float(rho), C.byref(G), _ptr(ws), self._stream()))
 
-    def wm_loss_forward(self, obs0, action, task, drop, H, B):
+    def wm_loss_forward(self, obs0, action, task, drop, H, B, zs=None):
         """agent._update's taped forward: obs0 [B, obs_dim], action [H B, A], task [H B] | None, drop [num_q, H B, M] | None
         -> tape, zs [H + 1, B, L], Q logits [num_q, H B, num_bins], reward logits [H B, num_bins], termination logits
-        [H B, 1] (episodic models) or None."""
+        [H B, 1] (episodic models) or None.  obs0 None: z_0 is the caller's, in zs[0] of the given zs ([H + 1, B, L] fp32
+        contiguous, filled in place; pixel models: encode_pixel_rows_taped(..., out=zs[0]))."""
+        if obs0 is None and zs is None:
+            raise ValueError("wm_loss_forward without obs0 needs zs, with z_0 in zs[0]")
         cfg, R = self.cfg, H * B
         tape = self._scratch(self.lib.tdmpc2_wm_loss_tape_bytes, self.h, H, B)
-        zs = self._rows_out(H + 1, B, cfg.latent_dim)
+        if zs is None:
+            zs = self._rows_out(H + 1, B, cfg.latent_dim)
         ql, rl = self._rows_out(cfg.num_q, R, cfg.num_bins), self._rows_out(R, cfg.num_bins)
         tl = self._rows_out(R, 1) if cfg.episodic else None
         with torch.cuda.device(self.device):
             _cabi.check(self.lib.tdmpc2_wm_loss_forward(self.h, _ptr(obs0), _ptr(action), _ptr(task), _ptr(drop), H, B, _ptr(zs),
                                                         _ptr(ql), _ptr(rl), _ptr(tl), _ptr(tape), self._stream()))
-        return tape, zs, ql, rl, tl
-
-    def wm_loss_forward_latent(self, zs, action, task, drop, H, B):
-        """wm_loss_forward for a latent z_0 the caller wrote into zs[0] (pixel models: encode_pixel_rows_taped(..., out=zs[0])):
-        zs [H + 1, B, L] fp32 contiguous, filled in place -> tape, zs, Q logits, reward logits, termination logits | None."""
-        cfg, R = self.cfg, H * B
-        tape = self._scratch(self.lib.tdmpc2_wm_loss_tape_bytes, self.h, H, B)
-        ql, rl = self._rows_out(cfg.num_q, R, cfg.num_bins), self._rows_out(R, cfg.num_bins)
-        tl = self._rows_out(R, 1) if cfg.episodic else None
-        with torch.cuda.device(self.device):
-            _cabi.check(self.lib.tdmpc2_wm_loss_forward_latent(self.h, _ptr(action), _ptr(task), _ptr(drop), H, B, _ptr(zs),
-                                                               _ptr(ql), _ptr(rl), _ptr(tl), _ptr(tape), self._stream()))
         return tape, zs, ql, rl, tl
 
     def _wm_loss_structs(self, tensor, grads):
@@ -722,30 +709,19 @@ class Planner:
         return W, G, cf
 
     def wm_loss_backward(self, tensor, tape, obs0, action, task, drop, H, B, zs, ql, rl, tl, next_z, reward, td_target,
-                         terminated, grads):
+                         terminated, grads) -> Optional[torch.Tensor]:
         """Adds dL/dparameter of _update's world-model loss to `grads` (.grad tensors by state-dict key: `_encoder.state.*`,
         `_dynamics.*`, `_reward.*`, `_termination.*`, `_Qs.params.*`, `_task_emb.weight`).  `tensor(key)` returns the
-        model's fp32 tensor of a state-dict key."""
+        model's fp32 tensor of a state-dict key.  obs0 None (z_0 was the caller's): the state encoder is skipped
+        (`_encoder.*` of `grads` is not touched) and dL/dz_0 [B, L] is returned, for pixel_encode_backward; else None."""
         W, G, cf = self._wm_loss_structs(tensor, grads)
         ws = self._scratch(self.lib.tdmpc2_wm_loss_workspace_bytes, self.h, H, B)
+        dz0 = self._rows_out(B, self.cfg.latent_dim) if obs0 is None else None
         with torch.cuda.device(self.device):
             _cabi.check(self.lib.tdmpc2_wm_loss_backward(
                 self.h, C.byref(W), _ptr(tape), _ptr(obs0), _ptr(action), _ptr(task), _ptr(drop), H, B, _ptr(zs), _ptr(ql),
                 _ptr(rl), _ptr(tl), _ptr(next_z), _ptr(reward), _ptr(td_target), _ptr(terminated), C.byref(cf), C.byref(G),
-                _ptr(ws), self._stream()))
-
-    def wm_loss_backward_latent(self, tensor, tape, action, task, drop, H, B, zs, ql, rl, tl, next_z, reward, td_target,
-                                terminated, grads) -> torch.Tensor:
-        """wm_loss_backward without the state encoder (`_encoder.*` of `grads` is not touched) -> dL/dz_0 [B, L], for
-        pixel_encode_backward."""
-        W, G, cf = self._wm_loss_structs(tensor, grads)
-        ws = self._scratch(self.lib.tdmpc2_wm_loss_workspace_bytes, self.h, H, B)
-        dz0 = self._rows_out(B, self.cfg.latent_dim)
-        with torch.cuda.device(self.device):
-            _cabi.check(self.lib.tdmpc2_wm_loss_backward_latent(
-                self.h, C.byref(W), _ptr(tape), _ptr(action), _ptr(task), _ptr(drop), H, B, _ptr(zs), _ptr(ql), _ptr(rl),
-                _ptr(tl), _ptr(next_z), _ptr(reward), _ptr(td_target), _ptr(terminated), C.byref(cf), C.byref(G), _ptr(dz0),
-                _ptr(ws), self._stream()))
+                _ptr(dz0), _ptr(ws), self._stream()))
         return dz0
 
     def estimate_value(self, z, actions, task, noise_pi, qidx):

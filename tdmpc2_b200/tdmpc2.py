@@ -304,7 +304,7 @@ class TDMPC2(torch.nn.Module):
         run as taped row launches (tdmpc2_wm_loss_forward), the backward chain of grad_kernels.cuh ADDS the gradients of
         the world-model loss to `.grad` as autograd would; then torch's clip_grad_norm_ and optim.step(), update_pi on the
         detached latents, and the Polyak update of the target Q ensemble.  Pixel models encode obs[0] with a taped conv
-        forward into zs[0] (a taped tdmpc2_pixel_encode, tdmpc2_wm_loss_forward_latent), and dL/dz_0 runs through the conv
+        forward into zs[0] (a taped tdmpc2_pixel_encode; the loss calls get obs0 = NULL), and dL/dz_0 runs through the conv
         backward of pixel_grad_kernels.cuh into `.grad` of `_encoder.rgb.*`.
         Draws from self.generator in the reference's order: pixel models' ShiftAug shifts of obs[1:] (H draws of (B, 2)),
         the TD target's pi noise and Q pair (`td_eps` [H, B, A], `td_qidx` [2]), pixel models' shift of obs[0], the
@@ -397,12 +397,12 @@ class TDMPC2(torch.nn.Module):
         # latent rollout and heads (tdmpc2.py:269-285), on the kernels with a tape
         pl = self.planner
         act_rows = action.reshape(H * B, A)
+        obs0, zs = obs[0], None
         if rgb:
             zs = torch.empty(H + 1, B, L, device=dev, dtype=torch.float32)
             _, pix_tape = pl.encode_pixel_rows_taped(obs[0], shift0, out=zs[0])
-            tape, zs, ql, rl, tl = pl.wm_loss_forward_latent(zs, act_rows, taskv, drop, H, B)
-        else:
-            tape, zs, ql, rl, tl = pl.wm_loss_forward(obs[0], act_rows, taskv, drop, H, B)
+            obs0 = None
+        tape, zs, ql, rl, tl = pl.wm_loss_forward(obs0, act_rows, taskv, drop, H, B, zs=zs)
         rho = torch.pow(cfg.rho, torch.arange(H, device=dev, dtype=torch.float32))
         consistency_loss = (F.mse_loss(zs[1:], next_z, reduction="none").mean(dim=(1, 2)) * rho).sum() / H
         reward_loss = (_soft_ce(rl.view(H, B, -1), reward, cfg).mean(dim=(1, 2)) * rho).sum() / H
@@ -422,13 +422,10 @@ class TDMPC2(torch.nn.Module):
             if p.grad is None:
                 p.grad = torch.zeros_like(p)
         grads = {k: p.grad for k, p in zip(self._wm_keys, params)}
+        dz0 = pl.wm_loss_backward(self.model.tensor, tape, obs0, act_rows, taskv, drop, H, B, zs, ql, rl, tl, next_z, reward,
+                                  td_targets, terminated, grads)
         if rgb:
-            dz0 = pl.wm_loss_backward_latent(self.model.tensor, tape, act_rows, taskv, drop, H, B, zs, ql, rl, tl, next_z,
-                                             reward, td_targets, terminated, grads)
             pl.pixel_encode_backward(self.model.tensor, pix_tape, obs[0], shift0, zs[0], dz0, grads)
-        else:
-            pl.wm_loss_backward(self.model.tensor, tape, obs[0], act_rows, taskv, drop, H, B, zs, ql, rl, tl, next_z, reward,
-                                td_targets, terminated, grads)
         grad_norm = torch.nn.utils.clip_grad_norm_([p for p in self.model.parameters() if p.grad is not None],
                                                    cfg.grad_clip_norm)
         self.optim.step()

@@ -272,17 +272,14 @@ def wm_kernels(cfg, sd, engine, x, H, B):
     dv = lambda t: None if t is None else t.to(DEV).contiguous()
     taskv = agent.model._task_rows(pl, dv(x["task"]), (H, B))
     act, drop = dv(x["action"]).reshape(R, A), dv(x["drop"]).reshape(nq, R, -1)
-    latent = x["z0"] is not None
-    if latent:
+    obs0, zs = dv(x["obs0"]), None
+    if obs0 is None:
         zs = torch.empty(H + 1, B, cfg.latent_dim, device=DEV)
         zs[0] = dv(x["z0"])
-        tape, zs, ql, rl, tl = pl.wm_loss_forward_latent(zs, act, taskv, drop, H, B)
-    else:
-        tape, zs, ql, rl, tl = pl.wm_loss_forward(dv(x["obs0"]), act, taskv, drop, H, B)
+    tape, zs, ql, rl, tl = pl.wm_loss_forward(obs0, act, taskv, drop, H, B, zs=zs)
     grads = {k: torch.zeros_like(agent.model.tensor(k)) for k in agent._wm_keys}
-    args = (agent.model.tensor, tape) + (() if latent else (dv(x["obs0"]),)) + (
-        act, taskv, drop, H, B, zs, ql, rl, tl, dv(x["next_z"]), dv(x["reward"]), dv(x["td"]), dv(x["terminated"]), grads)
-    dz0 = pl.wm_loss_backward_latent(*args) if latent else pl.wm_loss_backward(*args)
+    dz0 = pl.wm_loss_backward(agent.model.tensor, tape, obs0, act, taskv, drop, H, B, zs, ql, rl, tl, dv(x["next_z"]),
+                              dv(x["reward"]), dv(x["td"]), dv(x["terminated"]), grads)
     torch.cuda.synchronize()
     values = decode_wm_tape(cfg, sd, tape, zs, ql, rl, tl, H, B)
     return values, {k: v.cpu() for k, v in grads.items()}, None if dz0 is None else dz0.cpu()

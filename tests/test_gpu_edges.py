@@ -187,6 +187,61 @@ def test_only_the_two_engines_are_accepted():
     assert Planner(cfg, 1, "cuda:0", engine="simt").iter_engine == "simt"
 
 
+def test_obs_or_latent_rules_of_prologue_and_world_model_loss():
+    """The prologue takes exactly one of obs and z; the world-model loss backward takes dz0 exactly when obs0 is NULL.
+    Both other combinations are TDMPC2_ERR_INVALID on every planner.  A pixel planner refuses obs (prologue:
+    TDMPC2_ERR_STATE) and obs0 (loss forward and backward: TDMPC2_ERR_UNSUPPORTED).  Valid calls still return 0."""
+    import ctypes as C
+    from tdmpc2_b200.planner import _ptr
+    from tdmpc2_b200.tdmpc2 import TDMPC2
+    H, B = 2, 4
+    for wl in ("tiny", "tiny-rgb"):
+        cfg = workload(wl, num_envs=1)
+        agent = TDMPC2(cfg, device="cuda:0")
+        agent.model.load_state_dict(synth_state_dict(cfg, seed=27, perturb=True))
+        pl, lib, rgb = agent.planner, agent.planner.lib, wl == "tiny-rgb"
+        g = torch.Generator().manual_seed(8)
+        obs_shape = tuple(cfg.obs_shape["rgb"]) if rgb else (cfg.obs_shape["state"][0],)
+        obs = torch.rand(B, *obs_shape, generator=g).cuda()
+        z = torch.softmax(torch.randn(B, cfg.latent_dim // cfg.simnorm_dim, cfg.simnorm_dim, generator=g), -1).reshape(B, -1).cuda()
+        t0, prev = torch.ones(1, dtype=torch.uint8, device="cuda"), torch.zeros(1, cfg.horizon, cfg.action_dim, device="cuda")
+        prior = torch.randn(1, cfg.horizon, cfg.num_pi_trajs, cfg.action_dim, generator=g).cuda()
+
+        def prologue(o, zz):
+            return lib.tdmpc2_plan_prologue(pl.h, _ptr(o), _ptr(zz), None, _ptr(t0), _ptr(prev), _ptr(prior), pl._stream())
+        assert prologue(obs[:1], z[:1]) == -1 and prologue(None, None) == -1, wl
+        assert b"exactly one of obs and z" in lib.tdmpc2_last_error()
+        if rgb:
+            assert prologue(obs[:1], None) == -4 and b"pass z, not obs" in lib.tdmpc2_last_error()
+        assert prologue(None if rgb else obs[:1], z[:1] if rgb else None) == 0, wl
+
+        act = (torch.rand(H * B, cfg.action_dim, generator=g) * 2 - 1).cuda()
+        zs = torch.empty(H + 1, B, cfg.latent_dim, device="cuda")
+        zs[0] = z
+        tape, zs, ql, rl, tl = pl.wm_loss_forward(None if rgb else obs, act, None, None, H, B, zs=zs)
+        next_z, rew, td, term = zs[1:].clone(), torch.rand(H * B, 1).cuda(), torch.rand(H * B, 1).cuda(), torch.zeros(H * B, 1).cuda()
+        grads = {k: torch.zeros_like(agent.model.tensor(k)) for k in agent._wm_keys}
+        W, G, cf = pl._wm_loss_structs(agent.model.tensor, grads)
+        ws = pl._scratch(lib.tdmpc2_wm_loss_workspace_bytes, pl.h, H, B)
+        dz0 = torch.empty(B, cfg.latent_dim, device="cuda")
+
+        def backward(o, d):
+            return lib.tdmpc2_wm_loss_backward(pl.h, C.byref(W), _ptr(tape), _ptr(o), _ptr(act), None, None, H, B, _ptr(zs),
+                                               _ptr(ql), _ptr(rl), _ptr(tl), _ptr(next_z), _ptr(rew), _ptr(td), _ptr(term),
+                                               C.byref(cf), C.byref(G), _ptr(d), _ptr(ws), pl._stream())
+        assert backward(None, None) == -1 and b"dz0 must be non-NULL exactly when obs0 is NULL" in lib.tdmpc2_last_error()
+        if rgb:
+            fwd = lib.tdmpc2_wm_loss_forward(pl.h, _ptr(obs), _ptr(act), None, None, H, B, _ptr(zs), _ptr(ql), _ptr(rl),
+                                             _ptr(tl), _ptr(tape), pl._stream())
+            assert fwd == -5 and b"no state encoder" in lib.tdmpc2_last_error()
+            assert backward(obs, None) == -5 and backward(obs, dz0) == -5
+        else:
+            assert backward(obs, dz0) == -1 and b"dz0 must be non-NULL" in lib.tdmpc2_last_error()
+            assert backward(obs, None) == 0
+        assert backward(None, dz0) == 0, wl
+        torch.cuda.synchronize()
+
+
 @pytest.mark.parametrize("wl", ["tiny", "tiny-mt", "tiny-rgb"])
 def test_one_environment_paths_agree_bit_for_bit(wl):
     """One environment per act() (the reference's call shape) has three host paths: draws interleaved with the launches

@@ -230,7 +230,7 @@ def test_taped_z_bit_identical_and_zs0():
     H, B = x["action"].shape[:2]
     zs = torch.empty(H + 1, B, cfg.latent_dim, device=DEV)
     pl.encode_pixel_rows_taped(x["obs"][0], x["shift"][0], out=zs[0])
-    pl.wm_loss_forward_latent(zs, x["action"].reshape(H * B, -1).contiguous(), None, None, H, B)
+    pl.wm_loss_forward(None, x["action"].reshape(H * B, -1).contiguous(), None, None, H, B, zs=zs)
     assert torch.equal(zs[0], agent.model.encode(x["obs"][0], None, shift=x["shift"][0]))
     assert torch.equal(zs[1], agent.model.next(zs[0], x["action"][0], None))
 
@@ -252,10 +252,10 @@ def test_deterministic_and_accumulates(engine):
         _, ptape = pl.encode_pixel_rows_taped(x["obs"][0], x["shift"][0], out=zs[0])
         act = x["action"].reshape(H * B, -1).contiguous()
         drop = x["drop"].reshape(cfg.num_q, H * B, -1).contiguous()
-        tape, zs, ql, rl, tl = pl.wm_loss_forward_latent(zs, act, None, drop, H, B)
+        tape, zs, ql, rl, tl = pl.wm_loss_forward(None, act, None, drop, H, B, zs=zs)
         grads = {k: (torch.zeros_like(agent.model.tensor(k)) if pre is None else pre[k].clone().to(DEV)) for k in agent._wm_keys}
-        dz0 = pl.wm_loss_backward_latent(agent.model.tensor, tape, act, None, drop, H, B, zs, ql, rl, tl, next_z.contiguous(),
-                                         x["reward"].contiguous(), td.contiguous(), x["terminated"].contiguous(), grads)
+        dz0 = pl.wm_loss_backward(agent.model.tensor, tape, None, act, None, drop, H, B, zs, ql, rl, tl, next_z.contiguous(),
+                                  x["reward"].contiguous(), td.contiguous(), x["terminated"].contiguous(), grads)
         pl.pixel_encode_backward(agent.model.tensor, ptape, x["obs"][0], x["shift"][0], zs[0], dz0, grads)
         torch.cuda.synchronize()
         return {k: v.cpu() for k, v in grads.items()}

@@ -47,7 +47,7 @@ def test_single_pixel_encode_call_exported():
     assert "tdmpc2_pixel_encode" in _cabi.SYMBOLS and hasattr(lib, "tdmpc2_pixel_encode")
     for old in ("tdmpc2_pixel_encode_rows", "tdmpc2_pixel_encode_taped"):     # ABI 8 merged them into tdmpc2_pixel_encode
         assert old not in _cabi.SYMBOLS and not hasattr(lib, old), old
-    assert lib.tdmpc2_abi_version() == _cabi.ABI_VERSION == 8
+    assert lib.tdmpc2_abi_version() == _cabi.ABI_VERSION == 9
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")

@@ -79,11 +79,14 @@ def lib():
     return _cabi.load()
 
 
-def test_world_model_entry_points_exported_by_abi_8(lib):
+def test_world_model_entry_points_exported_by_abi_9(lib):
     from tdmpc2_b200 import _cabi
-    assert _cabi.ABI_VERSION == 8 and lib.tdmpc2_abi_version() == 8
+    assert _cabi.ABI_VERSION == 9 and lib.tdmpc2_abi_version() == 9
     for s in NEW_SYMBOLS:
         assert s in _cabi.SYMBOLS and hasattr(lib, s), s
+    # ABI 9 folded these into tdmpc2_plan_prologue (z) and tdmpc2_wm_loss_forward / _backward (obs0 = NULL, dz0)
+    for old in ("tdmpc2_plan_prologue_latent", "tdmpc2_wm_loss_forward_latent", "tdmpc2_wm_loss_backward_latent"):
+        assert old not in _cabi.SYMBOLS and not hasattr(lib, old), old
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
