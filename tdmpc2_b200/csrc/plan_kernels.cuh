@@ -184,8 +184,7 @@ __device__ __forceinline__ LayerRec layer_rec(const LayerDev& l) {
 // What a layer's epilogue has to do besides the activation itself.
 struct EpiArgs {
   int kind;                 // Epi
-  int dstbuf;               // LN kinds: plane destination buffer (or -1)
-  int dst_col0;
+  int dstbuf;               // LN kinds: plane destination buffer (or -1), written from column 0
   float* out_f32;           // LN kinds / RAW: optional fp32 row output
   int out_pitch;
   const int* rowmap;        // smem [128]: output row of each tile row (or -1), for out_f32
@@ -238,6 +237,17 @@ __device__ __forceinline__ float4 lds128(const float* p) {   // p must point int
   float4 r;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];\n" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "r"(ptx::smem_u32(p)));
   return r;
+}
+// Four consecutive floats of a global row: one 16-byte access when v4 (p 16-byte aligned), else four scalar ones.
+__device__ __forceinline__ float4 ld_quad(const float* p, bool v4) {
+  return v4 ? *reinterpret_cast<const float4*>(p) : make_float4(p[0], p[1], p[2], p[3]);
+}
+__device__ __forceinline__ void st_quad(float* p, bool v4, const float* y) {
+  if (v4) {
+    *reinterpret_cast<float4*>(p) = make_float4(y[0], y[1], y[2], y[3]);
+  } else {
+    p[0] = y[0]; p[1] = y[1]; p[2] = y[2]; p[3] = y[3];
+  }
 }
 // Diagnostics (cycle counters per role, clock stamps per layer of CTA 0) exist only in builds with -DTDMPC2_PROF
 // (tdmpc2_b200.build.build_variant("prof", ["TDMPC2_PROF=1"]), loaded through TDMPC2_B200_LIB): in the product build
@@ -529,6 +539,24 @@ __device__ __forceinline__ float simnorm_lane(float y, bool valid) {
   t += __shfl_xor_sync(0xffffffffu, t, 4);
   return valid ? __fdiv_rn(e, t) : 0.f;
 }
+// The same SimNorm on a 512-wide row's layout (rows_ln_act): y = 4 contiguous columns of a lane, a group of 8 columns is
+// lanes 2 k, 2 k + 1.  The sum pairs like simnorm_lane's butterfly, (e0 + e1) + (e2 + e3) in the lane and then the
+// partner's half, and the max is order-free, so the result is bit-identical to simnorm_lane's.
+__device__ __forceinline__ void simnorm_quad(float* y) {
+  float m = fmaxf(fmaxf(y[0], y[1]), fmaxf(y[2], y[3]));
+  m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+  float e[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) e[i] = expf(y[i] - m);
+  float t = (e[0] + e[1]) + (e[2] + e[3]);
+  t += __shfl_xor_sync(0xffffffffu, t, 1);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) y[i] = __fdiv_rn(e[i], t);
+}
+
+__device__ __forceinline__ float tree_sum8(const float (&t)[8]) {
+  return ((t[0] + t[1]) + (t[2] + t[3])) + ((t[4] + t[5]) + (t[6] + t[7]));
+}
 
 constexpr int kLnRegCols = 16;   // columns per lane of a 512-wide row
 constexpr int kLnBatch = 8;      // columns per lane that the output pass carries through activation and stores at once
@@ -539,7 +567,9 @@ constexpr int kLnBatch = 8;      // columns per lane that the output pass carrie
 // kStageCols-float buffers there.  While the warp works on row r from one, cp.async (L2 only, no registers held) copies
 // row r + kWarps of raw into the other.
 constexpr int kStageCols = 512;
-static_assert(kWarps * 2 * kStageCols * 4 <= kStages * kStageBytes, "row staging buffers");
+// A 512-wide LayerNorm row phase also stages its layer's bias | gamma | beta (3 x 512 floats) there, past the row buffers.
+constexpr int kLnParamOff = kWarps * 2 * kStageCols;   // floats from stage_base
+static_assert((kLnParamOff + 3 * kStageCols) * 4 <= kStages * kStageBytes, "row staging buffers and LayerNorm parameters");
 __device__ __forceinline__ float* row_stage(const Ctx& c, int i) {
   return reinterpret_cast<float*>(c.stage_base) + (c.warp * 2 + (i & 1)) * kStageCols;
 }
@@ -579,17 +609,20 @@ __device__ __forceinline__ void mish_batch(float (&y)[kLnBatch]) {
   for (int u = 0; u < kLnBatch; ++u) y[u] = y[u] > 20.f ? y[u] : y[u] * q[u];
 }
 
-// LayerNorm (+ Mish | SimNorm) over raw rows; one warp per row, lane-strided columns (lane + 32 j).  raw is written by
-// this kernel's GEMM and read with ld.global.cg; bias / gamma / beta are read-only for the kernel's lifetime and go
-// through the read-only path (__ldg).  The output pass works on batches of kLnBatch columns per lane: every load of a
-// batch is issued before its first store (the stores go through pointers that may alias raw as far as the compiler
-// knows), and the batch's activations are independent chains that overlap.
-//   - 512-wide rows (every hidden layer of the 5M model): raw is read once, through the staging buffers, so that the next
-//     row's copy overlaps this row's work; the 16 values per lane stay in registers from the statistics through the
-//     output pass.  (Holding the next row in registers instead spills it: the row phase shares the kernel's 168.)
-//   - other widths: raw is read once per statistic and once in the output pass.  (Statistics loads in guarded batches
-//     of kLnBatch were measured slower on c3's 1792-wide rows than these loops, which ptxas unrolls with unguarded loads.)
-// Every column's value is the same expression in the same order in both paths: same bits.
+// LayerNorm (+ Mish | SimNorm) over raw rows; one warp per row.  raw is written by this kernel's GEMM; bias / gamma /
+// beta are read-only for the kernel's lifetime.  The output pass works on batches of kLnBatch columns per lane: every
+// load of a batch is issued before its first store (the stores go through pointers that may alias raw as far as the
+// compiler knows), and the batch's activations are independent chains that overlap.
+//   - 512-wide rows (every hidden layer of the 5M model): each lane owns 4 contiguous columns of each 128-column slab,
+//     so that the row, bias, gamma and beta are read with 16-byte shared loads (the row through the staging buffers,
+//     so that the next row's copy overlaps this row's work; the parameters staged once per layer) and each plane gets
+//     one 8-byte store per slab.  The 16 values per lane stay in registers from the statistics through the output
+//     pass.  (Holding the next row in registers instead spills it: the row phase shares the kernel's 168.)
+//   - other widths: lane-strided columns (lane + 32 j), raw read with ld.global.cg once per statistic and once in the
+//     output pass, the parameters through the read-only path (__ldg).  (Statistics loads in guarded batches of kLnBatch
+//     were measured slower on c3's 1792-wide rows than these loops, which ptxas unrolls with unguarded loads.)
+// Each column's normalised value, activation and split are the same expressions in both paths; the mean and variance
+// add the columns in an order set by the lane mapping (in the 512-wide path, a balanced tree per lane).
 // ROWS (ROP_PI_LOSS): the pre-LayerNorm value is multiplied by the dropout scale ea.drop (Q layer 0, train mode) and
 // stored to the tape ea.tape; compiled out of the planning instantiations.
 template <bool ROWS>
@@ -613,8 +646,8 @@ __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const L
         if (j0 + u < ncolj) y[u] = simnorm_lane(y[u], c.lane + 32 * (j0 + u) < N);
     }
     if (dhi) {
-      __half* hi = dhi + static_cast<size_t>(r) * pitch + ea.dst_col0;
-      __half* lo = dlo + static_cast<size_t>(r) * pitch + ea.dst_col0;
+      __half* hi = dhi + static_cast<size_t>(r) * pitch;
+      __half* lo = dlo + static_cast<size_t>(r) * pitch;
 #pragma unroll
       for (int u = 0; u < kLnBatch; ++u) {
         const int col = c.lane + 32 * (j0 + u);
@@ -632,45 +665,106 @@ __device__ __forceinline__ void rows_ln_act(const PlanParams& P, Ctx& c, const L
     }
   };
   if (N == 32 * kLnRegCols) {
-    // Rows arrive through the warp's staging buffers (see stage_row): row r + kWarps is copied while row r is computed.
+    // Lane l owns columns 128 q + 4 l + i (q, i = 0..3): x[4 q + i].  Rows arrive through the warp's staging buffers (see
+    // stage_row): row r + kWarps is copied while row r is computed.  The layer's bias | gamma | beta go to smem once,
+    // while the warps' first rows are in flight.
+    static_assert(3 * kStageCols == 4 * kThreads, "LayerNorm parameter copy: 4 floats per thread");
+    static_assert(kKch % 4 == 0, "plane rows (KpadX / KpadH, multiples of kKch) keep 4-column groups 8-byte aligned");
+    // (the lane index is re-read here: per-thread offsets derived from c.lane or threadIdx.x are otherwise computed at
+    // kernel start and held, or spilled, through the GEMMs)
+    const int lane = static_cast<int>(ptx::lane_id());
+    const int c0 = 4 * lane;
+    float* prm = reinterpret_cast<float*>(c.stage_base) + kLnParamOff;
     stage_row(P, c, c.warp, N, row_stage(c, 0));
+    {
+      const int t = 32 * c.warp + lane, a = t / (kStageCols / 4);   // thread t copies floats 4 t .. 4 t + 3
+      const float* src = (a == 0 ? bias : a == 1 ? lg : lb) + 4 * (t % (kStageCols / 4));
+      const float4 v = ld_quad(src, (reinterpret_cast<uintptr_t>(src) & 15) == 0);
+      *reinterpret_cast<float4*>(prm + 4 * t) = v;
+    }
+    __syncthreads();
     for (int r = c.warp, i = 0; r < kTileM; r += kWarps, ++i) {
       const float* row = stage_advance(P, c, r, i, N);
       float x[kLnRegCols];
 #pragma unroll
-      for (int j = 0; j < kLnRegCols; ++j) x[j] = row[c.lane + 32 * j];
+      for (int q = 0; q < 4; ++q) {
+        const float4 v = lds128(row + 128 * q + c0), b = lds128(prm + 128 * q + c0);
+        x[4 * q] = fmaf(v.x, inv_scale, b.x);
+        x[4 * q + 1] = fmaf(v.y, inv_scale, b.y);
+        x[4 * q + 2] = fmaf(v.z, inv_scale, b.z);
+        x[4 * q + 3] = fmaf(v.w, inv_scale, b.w);
+      }
       const bool live = ROWS && ea.rowmap[r] >= 0;
-      const float* drow = live && ea.drop ? ea.drop + static_cast<size_t>(ea.rowmap[r]) * N : nullptr;
-      float s = 0.f;
+      if (ROWS && live && ea.drop) {
+        const float* drow = ea.drop + static_cast<size_t>(ea.rowmap[r]) * N;
+        const bool v4 = (reinterpret_cast<uintptr_t>(drow) & 15) == 0;
 #pragma unroll
-      for (int j = 0; j < kLnRegCols; ++j) {
-        x[j] = fmaf(x[j], inv_scale, __ldg(bias + c.lane + 32 * j));
-        if (ROWS && drow) x[j] *= drow[c.lane + 32 * j];
-        s += x[j];
+        for (int q = 0; q < 4; ++q) {
+          const float4 d = ld_quad(drow + 128 * q + c0, v4);
+          x[4 * q] *= d.x; x[4 * q + 1] *= d.y; x[4 * q + 2] *= d.z; x[4 * q + 3] *= d.w;
+        }
       }
       if (ROWS && live && ea.tape) {
         float* trow = ea.tape + static_cast<size_t>(ea.rowmap[r]) * P.tape_pitch;
+        const bool v4 = (reinterpret_cast<uintptr_t>(trow) & 15) == 0;
 #pragma unroll
-        for (int j = 0; j < kLnRegCols; ++j) trow[c.lane + 32 * j] = x[j];
+        for (int q = 0; q < 4; ++q) st_quad(trow + 128 * q + c0, v4, x + 4 * q);
       }
-      const float mean = warp_sum(s) * invN;
-      float sq = 0.f;
+      // the lane's 16 terms of each statistic are added as a balanced tree (4 roundings deep instead of 15): an error in
+      // the mean or the variance shifts or scales the whole row alike
+      float t[kLnRegCols / 2];
 #pragma unroll
-      for (int j = 0; j < kLnRegCols; ++j) {
-        const float d = x[j] - mean;
-        sq = fmaf(d, d, sq);
+      for (int j = 0; j < kLnRegCols / 2; ++j) t[j] = x[2 * j] + x[2 * j + 1];
+      const float mean = warp_sum(tree_sum8(t)) * invN;
+#pragma unroll
+      for (int j = 0; j < kLnRegCols / 2; ++j) {
+        const float d0 = x[2 * j] - mean, d1 = x[2 * j + 1] - mean;
+        t[j] = fmaf(d0, d0, d1 * d1);
       }
-      const float var = warp_sum(sq) * invN;
+      const float var = warp_sum(tree_sum8(t)) * invN;
       const float rstd = 1.f / sqrtf(var + 1e-5f);   // nn.LayerNorm eps (layers.py:101)
+      const int orow = ea.rowmap ? ea.rowmap[r] : r;
+      float* o = ea.out_f32 && orow >= 0 ? ea.out_f32 + static_cast<size_t>(orow) * ea.out_pitch : nullptr;
+      const bool o4 = (reinterpret_cast<uintptr_t>(o) & 15) == 0;
 #pragma unroll
       for (int j0 = 0; j0 < kLnRegCols; j0 += kLnBatch) {
-        float y[kLnBatch];
+        float y[kLnBatch];   // slabs q0, q0 + 1
+        const int q0 = j0 / 4;
 #pragma unroll
-        for (int u = 0; u < kLnBatch; ++u) {
-          const int col = c.lane + 32 * (j0 + u);
-          y[u] = (x[j0 + u] - mean) * rstd * __ldg(lg + col) + __ldg(lb + col);
+        for (int s4 = 0; s4 < kLnBatch / 4; ++s4) {
+          const float4 g = lds128(prm + kStageCols + 128 * (q0 + s4) + c0);
+          const float4 b = lds128(prm + 2 * kStageCols + 128 * (q0 + s4) + c0);
+          const float* xs = x + j0 + 4 * s4;
+          float* ys = y + 4 * s4;
+          ys[0] = (xs[0] - mean) * rstd * g.x + b.x;
+          ys[1] = (xs[1] - mean) * rstd * g.y + b.y;
+          ys[2] = (xs[2] - mean) * rstd * g.z + b.z;
+          ys[3] = (xs[3] - mean) * rstd * g.w + b.w;
         }
-        act_store(y, j0, r);
+        if (ea.kind == EPI_LN_MISH) {
+          mish_batch(y);
+        } else {
+#pragma unroll
+          for (int s4 = 0; s4 < kLnBatch / 4; ++s4) simnorm_quad(y + 4 * s4);
+        }
+#pragma unroll
+        for (int s4 = 0; s4 < kLnBatch / 4; ++s4) {
+          const int col = 128 * (q0 + s4) + c0;
+          if (dhi) {
+            uint32_t hw[2], lw[2];
+#pragma unroll
+            for (int p = 0; p < 2; ++p) {
+              __half h0, l0, h1, l1;
+              split_f(y[4 * s4 + 2 * p], h0, l0);
+              split_f(y[4 * s4 + 2 * p + 1], h1, l1);
+              hw[p] = static_cast<uint32_t>(__half_as_ushort(h0)) | (static_cast<uint32_t>(__half_as_ushort(h1)) << 16);
+              lw[p] = static_cast<uint32_t>(__half_as_ushort(l0)) | (static_cast<uint32_t>(__half_as_ushort(l1)) << 16);
+            }
+            __stcg(reinterpret_cast<uint2*>(dhi + static_cast<size_t>(r) * pitch + col), make_uint2(hw[0], hw[1]));
+            __stcg(reinterpret_cast<uint2*>(dlo + static_cast<size_t>(r) * pitch + col), make_uint2(lw[0], lw[1]));
+          }
+          if (o) st_quad(o + col, o4, y + 4 * s4);
+        }
       }
       __syncwarp();   // every lane has read buffer i before the next iteration refills it
     }
@@ -1207,7 +1301,7 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
 
     for (int sidx = 0; sidx < nsteps; ++sidx) {
       EpiArgs ea;
-      ea.kind = EPI_LN_MISH; ea.dstbuf = -1; ea.dst_col0 = 0; ea.out_f32 = nullptr; ea.out_pitch = 0; ea.rowmap = nullptr;
+      ea.kind = EPI_LN_MISH; ea.dstbuf = -1; ea.out_f32 = nullptr; ea.out_pitch = 0; ea.rowmap = nullptr;
       ea.head = 0; ea.disc = 0.f; ea.tile = tile; ea.eps_base = nullptr; ea.eps_rows = 0; ea.act_out = nullptr; ea.t_out = 0;
       ea.tape = nullptr; ea.drop = nullptr;
       int li, src;
@@ -1383,7 +1477,7 @@ __global__ void __launch_bounds__(kThreads, 1) plan_kernel(const __grid_constant
         } else if (mlp == 0) {                 // reward (world_model.py:123-130) + two_hot_inv
           ea.kind = EPI_TWOHOT; ea.head = HEAD_REWARD; ea.disc = dpow[t];
         } else if (mlp == 1) {                 // z <- next(z, a)  (world_model.py:114-121)
-          ea.kind = EPI_LN_SIMNORM; ea.dstbuf = BUF_X; ea.dst_col0 = 0;
+          ea.kind = EPI_LN_SIMNORM; ea.dstbuf = BUF_X;
         } else if (mlp == 2) {                 // a = pi(z)  (world_model.py:144-174) -> X action columns
           ea.kind = EPI_PI;
           if (P.mode == MODE_PRIOR) {          // eps = noise_prior[e, t, p, :]

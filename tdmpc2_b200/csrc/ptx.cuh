@@ -81,6 +81,11 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void* p, size_t bytes) {
 
 // ------------------------------------------------------------------ cp.async (per-thread asynchronous copies)
 // 16 bytes global -> shared through L2 only (.cg); completion is tracked per thread in commit groups.
+__device__ __forceinline__ uint32_t lane_id() {
+  uint32_t l;
+  asm volatile("mov.u32 %0, %%laneid;\n" : "=r"(l));
+  return l;
+}
 __device__ __forceinline__ void cp_async_16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }
