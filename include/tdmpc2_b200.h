@@ -14,12 +14,13 @@
  *   - all device memory is CALLER-OWNED (torch tensors in the Python host):
  *     contiguous, 256-byte aligned; the library never allocates device memory;
  *   - all work is enqueued on the caller's `stream` (a cudaStream_t passed as
- *     void*); no host synchronisation, except in create/bind/pack which are
- *     set-up calls;
+ *     void*); no host synchronisation, except in create/bind/pack and the
+ *     model file's upload, which are set-up calls;
  *   - fp32 tensors, int32 task / q-head indices, uint8 flags, int64 elite
  *     indices (torch.topk's dtype);
  *   - there is NO CPU fallback: every call fails with TDMPC2_ERR_NO_DEVICE
- *     unless the current device is sm_90 (H100).
+ *     unless the current device is sm_90 (H100); only the model file's
+ *     open / dims / device_bytes run on the host alone.
  *
  * Batched semantics (new in this build): a leading environment axis E.  Each
  * environment is one independent reference _plan call (own obs, task, t0,
@@ -42,7 +43,9 @@ extern "C" {
                                        7: world-model methods on a flat batch (tdmpc2_wm_*, tdmpc2_td_target), target Q blob, then
                                           agent.update_pi, agent._update of state and pixel models, the replay buffer's sampler;
                                        8: removed engines 2-4, the engine query, the L2 and reduction-segment knobs; one tdmpc2_pixel_encode;
-                                       9: the _latent calls folded in: tdmpc2_plan_prologue's z, tdmpc2_wm_loss_* with obs0 NULL and dz0 */
+                                       9: the _latent calls folded in: tdmpc2_plan_prologue's z, tdmpc2_wm_loss_* with obs0 NULL and dz0;
+                                          then added, no existing call or struct changed: the model file (tdmpc2_model_file_*),
+                                          tdmpc2_plan_draws, tdmpc2_act */
 #define TDMPC2_MAX_ENC_LAYERS 8
 
 typedef enum tdmpc2_status {
@@ -236,6 +239,67 @@ int tdmpc2_plan_get_state(tdmpc2_planner* p, float* mean, float* std, float* z,
 int tdmpc2_estimate_value(tdmpc2_planner* p, const float* z, const float* actions,
                           const int32_t* task, const float* noise_pi, const int32_t* qidx,
                           float* value_out, void* stream);
+
+/* ---- planning from a plain C host: the model file and one call per plan --------------------------------------------
+ * The model file is what agent.export(fp) writes (tdmpc2_b200/export.py): safetensors layout (8-byte little-endian header
+ * length, JSON header, raw little-endian data), fp32 tensors under the reference's state-dict keys plus tdmpc2.bins,
+ * tdmpc2.discount [num_tasks] (F64) and, for pixel models, tdmpc2.grid_base [64]; __metadata__ holds format
+ * "tdmpc2_b200.model", version "1", obs "state" | "rgb", every tdmpc2_dims field and, for pixel models, the
+ * pixel.{in_channels, num_channels, simnorm_dim} of tdmpc2_pixel_dims, all as strings.
+ *   open: host only (no device needed).  Reads the file and checks it: a truncated file, a header length past the end of
+ *     the file, a dtype other than F32 (F64 for tdmpc2.discount), overlapping or out-of-range data_offsets, a wrong format
+ *     or version, a missing tensor or a shape that disagrees with the dims are TDMPC2_ERR_INVALID, with the reason in
+ *     tdmpc2_last_error().
+ *   dims: the file's dims (num_envs = the exporting cfg's), pixel dims (pixel may be NULL) and whether it is a pixel model.
+ *   device_bytes / upload: dims may differ from the file's in num_envs and the planning block (num_samples, num_pi_trajs,
+ *     num_elites, horizon, iterations, temperature, min_std, max_std); any other difference is TDMPC2_ERR_INVALID.  upload
+ *     copies the tensors into the caller-owned device_buf (device_bytes, 256-byte aligned) and fills w (for
+ *     tdmpc2_pack_weights; discount_pow [num_tasks, dims->horizon + 1] computed as the Python planner does) and, for pixel
+ *     models, conv and grid_base (NULL for state models).  Synchronous: it returns when the copy is done. */
+typedef struct tdmpc2_model_file tdmpc2_model_file;
+int tdmpc2_model_file_open(const char* path, tdmpc2_model_file** out);
+void tdmpc2_model_file_close(tdmpc2_model_file* f);
+int tdmpc2_model_file_dims(const tdmpc2_model_file* f, tdmpc2_dims* dims, tdmpc2_pixel_dims* pixel, int32_t* is_pixel);
+int tdmpc2_model_file_device_bytes(const tdmpc2_model_file* f, const tdmpc2_dims* dims, size_t* out);
+int tdmpc2_model_file_upload(const tdmpc2_model_file* f, const tdmpc2_dims* dims, void* device_buf, tdmpc2_weights* w,
+                             tdmpc2_conv_weights* conv, const float** grid_base, void* stream);
+
+/* DECLARED NON-PARITY, like tdmpc2_plan_iter_rng: the small draws of one plan on the device, under rng_state = {seed, plan
+ * counter} (device memory, read, not advanced), each kind on a Philox stream of its own (0x80000000 + k, far above the
+ * iteration streams 2 * it and 2 * it + 1); element i of a draw is component i % 4 of Philox group i / 4:
+ *   noise_prior [E, H, P, A]  k = 0: standard normals (Box-Muller, as the iterations' noise); NULL when P == 0
+ *   qidx [I, E, 2] int32      k = 1: per (iteration, env) row r the indices of the two smallest of num_q uniform words
+ *                             (groups r ceil(num_q / 4) ..), smallest first: randperm(num_q)[:2]'s law
+ *   expo [E, K]               k = 2: -log(u), u in (0, 1] (24-bit)
+ *   noise_final [E, A]        k = 3: standard normals; not drawn (may be NULL) when eval_mode != 0
+ *   shift [E, 2]              k = 4: floor(7 u), u in [0, 1), as floats (ShiftAug's randint(0, 7)); NULL: not drawn
+ * One launch, no allocation, no host synchronisation.  Not torch's streams: the values differ from torch's draws. */
+int tdmpc2_plan_draws(tdmpc2_planner* p, const uint64_t* rng_state, int eval_mode, float* noise_prior, int32_t* qidx,
+                      float* expo, float* noise_final, float* shift, void* stream);
+
+/* One whole plan per call, every random number drawn on the device (DECLARED NON-PARITY, like tdmpc2_plan_iter_rng).  In
+ * order on `stream`: rng_state[1] += 1; tdmpc2_plan_draws into scratch; pixel models: tdmpc2_pixel_encode of frames with
+ * the drawn shifts into scratch; tdmpc2_plan_prologue; iterations x tdmpc2_plan_iter_rng; tdmpc2_plan_epilogue (no
+ * exploration noise in eval mode).  From a fresh {seed, 0} this follows the sequence the Python planner's rng = 'philox'
+ * mode follows with rng_seed = seed, when its small draws are tdmpc2_plan_draws' at the same counter.  The counter lives
+ * in device memory, so one captured call replays with fresh noise every time.  No allocation, no host synchronisation.
+ * Needs the tensor-core engine (TDMPC2_ERR_UNSUPPORTED on the SIMT engine).  State models pass e = NULL and obs; pixel
+ * models (a planner with num_enc_layers = 0) pass e, its workspace, conv, frames and grid_base. */
+typedef struct tdmpc2_act_args {
+  const float* obs;          /* [E, obs_dim] state models, else NULL                         */
+  const float* frames;       /* [E, C, 64, 64] in 0..255 for pixel models, else NULL         */
+  const int32_t* task;       /* [E] or NULL (single-task)                                    */
+  const uint8_t* t0;         /* [E]                                                          */
+  int32_t eval_mode;
+  uint64_t* rng_state;       /* device {seed, plan counter}                                  */
+  float* prev_mean;          /* [E, H, A]: read by the prologue, overwritten by the epilogue */
+  float* action_out;         /* [E, A]                                                       */
+  const float* grid_base;    /* pixel models                                                 */
+} tdmpc2_act_args;
+/* scratch: caller-owned device memory (256-byte aligned) of this many bytes; e NULL for state models */
+int tdmpc2_act_scratch_bytes(const tdmpc2_planner* p, const tdmpc2_pixel_encoder* e, size_t* out);
+int tdmpc2_act(tdmpc2_planner* p, tdmpc2_pixel_encoder* e, void* enc_workspace, const tdmpc2_conv_weights* conv,
+               const tdmpc2_act_args* a, void* scratch, void* stream);
 
 /* ---- world-model methods on a flat batch of rows ------------------------------
  * The training-side and analysis calls of the reference's WorldModel (world_model.py:103-216) and TDMPC2._td_target

@@ -28,6 +28,8 @@ SYMBOLS = [
     "tdmpc2_pi_loss_backward", "tdmpc2_wm_loss_tape_bytes", "tdmpc2_wm_loss_workspace_bytes", "tdmpc2_wm_loss_forward",
     "tdmpc2_wm_loss_backward", "tdmpc2_pixel_encode_tape_bytes",
     "tdmpc2_pixel_backward_workspace_bytes", "tdmpc2_pixel_encode_backward", "tdmpc2_buffer_sample",
+    "tdmpc2_model_file_open", "tdmpc2_model_file_close", "tdmpc2_model_file_dims", "tdmpc2_model_file_device_bytes",
+    "tdmpc2_model_file_upload", "tdmpc2_plan_draws", "tdmpc2_act_scratch_bytes", "tdmpc2_act",
 ]
 
 
@@ -83,6 +85,11 @@ class WmLossCoefs(C.Structure):
 class BufferField(C.Structure):    # tdmpc2_buffer_field: one field of a Buffer.sample gather
     _fields_ = [("storage", C.c_void_p), ("out", C.c_void_p), ("row_bytes", C.c_int64), ("first_step", C.c_int32),
                 ("steps", C.c_int32), ("host", C.c_int32)]
+
+
+class ActArgs(C.Structure):       # tdmpc2_act_args
+    _fields_ = [("obs", C.c_void_p), ("frames", C.c_void_p), ("task", C.c_void_p), ("t0", C.c_void_p), ("eval_mode", C.c_int32),
+                ("rng_state", C.c_void_p), ("prev_mean", C.c_void_p), ("action_out", C.c_void_p), ("grid_base", C.c_void_p)]
 
 
 class CabiError(RuntimeError):
@@ -161,6 +168,15 @@ def load():
     lib.tdmpc2_pixel_encode_backward.argtypes = [vp, C.POINTER(ConvWeights), vp, vp, vp, i64, vp, vp, vp, C.POINTER(ConvGrads),
                                                  vp, vp]
     lib.tdmpc2_buffer_sample.argtypes = [C.POINTER(BufferField), C.c_int, i64, vp, vp, i64, vp, vp, C.c_int, C.c_int, vp]
+    lib.tdmpc2_model_file_open.argtypes = [C.c_char_p, C.POINTER(vp)]
+    lib.tdmpc2_model_file_close.argtypes = [vp]
+    lib.tdmpc2_model_file_close.restype = None
+    lib.tdmpc2_model_file_dims.argtypes = [vp, C.POINTER(Dims), C.POINTER(PixelDims), C.POINTER(i32)]
+    lib.tdmpc2_model_file_device_bytes.argtypes = [vp, C.POINTER(Dims), C.POINTER(C.c_size_t)]
+    lib.tdmpc2_model_file_upload.argtypes = [vp, C.POINTER(Dims), vp, C.POINTER(Weights), C.POINTER(ConvWeights), C.POINTER(vp), vp]
+    lib.tdmpc2_plan_draws.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, vp, vp]
+    lib.tdmpc2_act_scratch_bytes.argtypes = [vp, vp, C.POINTER(C.c_size_t)]
+    lib.tdmpc2_act.argtypes = [vp, vp, vp, C.POINTER(ConvWeights), C.POINTER(ActArgs), vp, vp]
     _lib = lib
     return lib
 

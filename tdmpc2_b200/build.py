@@ -17,6 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libtdmpc2_b200.so")
 STAMP = LIB + ".stamp"
 SOURCES = ["api.cu", "plan_kernels.cuh", "grad_kernels.cuh", "pixel_encoder.cuh", "pixel_grad_kernels.cuh", "buffer_kernels.cuh", "ptx.cuh", "rng.cuh",
+           "draw_kernels.cuh", "model_file.cuh",
            os.path.join("..", "..", "include", "tdmpc2_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]

@@ -20,6 +20,7 @@
 #include "pixel_encoder.cuh"
 #include "pixel_grad_kernels.cuh"
 #include "buffer_kernels.cuh"
+#include "draw_kernels.cuh"
 
 using namespace tdmpc2;
 
@@ -52,6 +53,8 @@ static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; 
 // a workspace / tape segment of n floats at `off`, the next one starting on a 64-float boundary
 static size_t take64(size_t& off, size_t n) { const size_t o = off; off += (n + 63) / 64 * 64; return o; }
 static inline int pad_to(int x, int a) { return (x + a - 1) / a * a; }
+
+#include "model_file.cuh"
 
 // ------------------------------------------------------------------------------------ pack kernels
 __global__ void absmax_kernel(const float* __restrict__ w, size_t n, unsigned* slot) {
@@ -816,6 +819,102 @@ extern "C" int tdmpc2_debug_rng(const uint64_t* rng_state, uint32_t stream, uint
       reinterpret_cast<const unsigned long long*>(rng_state), stream, group0, ngroups, out);
   CUDA_TRY(cudaGetLastError());
   return 0;
+}
+
+// The small draws of one plan (draw_kernels.cuh), every kind in one launch.
+extern "C" int tdmpc2_plan_draws(tdmpc2_planner* p, const uint64_t* rng_state, int eval_mode, float* noise_prior, int32_t* qidx,
+                                 float* expo, float* noise_final, float* shift, void* stream_) {
+  if (!p) return fail(TDMPC2_ERR_INVALID, "null planner");
+  const tdmpc2_dims& d = p->d;
+  if (!rng_state || !qidx || !expo || (d.num_pi_trajs > 0 && !noise_prior) || (!eval_mode && !noise_final))
+    return fail(TDMPC2_ERR_INVALID, "null argument");
+  const long long E = d.num_envs, H = d.horizon, A = d.action_dim;
+  DrawParams P{};
+  P.state = reinterpret_cast<const unsigned long long*>(rng_state);
+  P.prior = d.num_pi_trajs > 0 ? noise_prior : nullptr;
+  P.n_prior = E * H * d.num_pi_trajs * A;
+  P.qidx = qidx;
+  P.q_rows = static_cast<long long>(d.iterations) * E;
+  P.num_q = d.num_q;
+  P.expo = expo;
+  P.n_expo = E * d.num_elites;
+  P.final_ = eval_mode ? nullptr : noise_final;
+  P.n_final = E * A;
+  P.shift = shift;
+  P.n_shift = E * 2;
+  const long long work = std::max({(P.n_prior + 3) / 4, P.q_rows, (P.n_expo + 3) / 4, (P.n_final + 3) / 4, (P.n_shift + 3) / 4});
+  const unsigned blocks = static_cast<unsigned>(std::max<long long>(1, std::min<long long>((work + 255) / 256, 1024)));
+  plan_draws_kernel<<<dim3(blocks, kDrawKinds), 256, 0, static_cast<cudaStream_t>(stream_)>>>(P);
+  CUDA_TRY(cudaGetLastError());
+  p->launches += 1;
+  return 0;
+}
+
+// tdmpc2_act's scratch: the draws and, for pixel models, the encoded latent
+struct ActScratch {
+  size_t prior, qidx, expo, final_, shift, z, bytes;
+};
+static ActScratch act_scratch(const tdmpc2_dims& d, bool pixel) {
+  const size_t E = d.num_envs, H = d.horizon, A = d.action_dim;
+  ActScratch s{};
+  size_t off = 0;
+  auto take = [&](size_t n) { const size_t o = off; off = align_up(off + n, 256); return o; };
+  s.prior = take(E * H * std::max(d.num_pi_trajs, 1) * A * 4);
+  s.qidx = take(static_cast<size_t>(d.iterations) * E * 2 * 4);
+  s.expo = take(E * d.num_elites * 4);
+  s.final_ = take(E * A * 4);
+  s.shift = take(E * 2 * 4);
+  s.z = pixel ? take(E * d.latent_dim * 4) : 0;
+  s.bytes = off;
+  return s;
+}
+
+extern "C" int tdmpc2_act_scratch_bytes(const tdmpc2_planner* p, const tdmpc2_pixel_encoder* e, size_t* out) {
+  if (!p || !out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  *out = act_scratch(p->d, e != nullptr).bytes;
+  return 0;
+}
+
+extern "C" int tdmpc2_act(tdmpc2_planner* p, tdmpc2_pixel_encoder* e, void* enc_workspace, const tdmpc2_conv_weights* conv,
+                          const tdmpc2_act_args* a, void* scratch, void* stream_) {
+  int rc = ready(p);
+  if (rc) return rc;
+  if (!a || !scratch || !a->t0 || !a->rng_state || !a->prev_mean || !a->action_out) return fail(TDMPC2_ERR_INVALID, "null argument");
+  if (reinterpret_cast<uintptr_t>(scratch) & 255) return fail(TDMPC2_ERR_INVALID, "scratch must be 256-byte aligned");
+  if (p->engine == TDMPC2_ENGINE_SIMT) return fail(TDMPC2_ERR_UNSUPPORTED, "in-kernel noise needs a tensor-core engine");
+  const tdmpc2_dims& d = p->d;
+  const bool pixel = p->num_enc == 0;
+  if (pixel) {
+    if (!e || !enc_workspace || !conv || !a->frames || !a->grid_base)
+      return fail(TDMPC2_ERR_INVALID, "a planner without a state encoder acts on frames: e, enc_workspace, conv, frames and grid_base are needed");
+    if (16 * e->d.num_channels != d.latent_dim) return fail(TDMPC2_ERR_INVALID, "the pixel encoder's latent is not the planner's latent_dim");
+  } else if (e || !a->obs) {
+    return fail(TDMPC2_ERR_INVALID, "a state model acts on obs, with no pixel encoder");
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  unsigned long long* state = reinterpret_cast<unsigned long long*>(a->rng_state);
+  rng_advance_kernel<<<1, 1, 0, st>>>(state);
+  CUDA_TRY(cudaGetLastError());
+  p->launches += 1;
+  const ActScratch s = act_scratch(d, pixel);
+  unsigned char* base = static_cast<unsigned char*>(scratch);
+  float* prior = d.num_pi_trajs > 0 ? reinterpret_cast<float*>(base + s.prior) : nullptr;
+  int32_t* qidx = reinterpret_cast<int32_t*>(base + s.qidx);
+  float* expo = reinterpret_cast<float*>(base + s.expo);
+  float* fin = a->eval_mode ? nullptr : reinterpret_cast<float*>(base + s.final_);
+  float* shift = pixel ? reinterpret_cast<float*>(base + s.shift) : nullptr;
+  if ((rc = tdmpc2_plan_draws(p, a->rng_state, a->eval_mode, prior, qidx, expo, fin, shift, stream_))) return rc;
+  float* z = nullptr;
+  if (pixel) {
+    z = reinterpret_cast<float*>(base + s.z);
+    if ((rc = tdmpc2_pixel_encode(e, enc_workspace, conv, a->frames, shift, a->grid_base, d.num_envs, z, nullptr, stream_))) return rc;
+    p->launches += 1;
+  }
+  if ((rc = tdmpc2_plan_prologue(p, pixel ? nullptr : a->obs, z, a->task, a->t0, a->prev_mean, prior, stream_))) return rc;
+  for (int it = 0; it < d.iterations; ++it)
+    if ((rc = tdmpc2_plan_iter_rng(p, a->rng_state, it, qidx + static_cast<size_t>(it) * d.num_envs * 2, nullptr, nullptr, stream_)))
+      return rc;
+  return tdmpc2_plan_epilogue(p, expo, fin, a->action_out, a->prev_mean, nullptr, stream_);
 }
 
 extern "C" int tdmpc2_plan_epilogue(tdmpc2_planner* p, const float* expo, const float* noise_final, float* action_out,

@@ -22,13 +22,15 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
   return c;
 }
 
-// state[0] = seed, state[1] = plan counter (device memory: the launch chain is replayed as a CUDA graph, so the per-plan
-// value must not be a kernel argument)
-__device__ __forceinline__ float4 rng_normal4(const unsigned long long* __restrict__ state, uint32_t stream, unsigned long long group) {
+// The raw Philox output of counter (group, stream, plan counter) under the seed.  state[0] = seed, state[1] = plan counter
+// (device memory: the launch chain is replayed as a CUDA graph, so the per-plan value must not be a kernel argument)
+__device__ __forceinline__ uint4 rng_bits4(const unsigned long long* __restrict__ state, uint32_t stream, unsigned long long group) {
   const unsigned long long seed = state[0], plan = state[1];
-  const uint4 u = philox4x32_10(make_uint4(static_cast<uint32_t>(group), static_cast<uint32_t>(group >> 32), stream,
-                                           static_cast<uint32_t>(plan)),
-                                make_uint2(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32) ^ static_cast<uint32_t>(plan >> 32)));
+  return philox4x32_10(make_uint4(static_cast<uint32_t>(group), static_cast<uint32_t>(group >> 32), stream, static_cast<uint32_t>(plan)),
+                       make_uint2(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32) ^ static_cast<uint32_t>(plan >> 32)));
+}
+__device__ __forceinline__ float4 rng_normal4(const unsigned long long* __restrict__ state, uint32_t stream, unsigned long long group) {
+  const uint4 u = rng_bits4(state, stream, group);
   // Box-Muller: u1 in (0, 1], u2 in [0, 1)
   const float u1a = (static_cast<float>(u.x >> 8) + 1.0f) * (1.0f / 16777216.0f), u2a = static_cast<float>(u.y >> 8) * (1.0f / 16777216.0f);
   const float u1b = (static_cast<float>(u.z >> 8) + 1.0f) * (1.0f / 16777216.0f), u2b = static_cast<float>(u.w >> 8) * (1.0f / 16777216.0f);
@@ -39,6 +41,14 @@ __device__ __forceinline__ float4 rng_normal4(const unsigned long long* __restri
   return make_float4(ra * ca, ra * sa, rb * cb, rb * sb);
 }
 __device__ __forceinline__ float rng_pick(const float4& g, int i) { return i == 0 ? g.x : i == 1 ? g.y : i == 2 ? g.z : g.w; }
+
+// Four uniforms in [0, 1): the top 24 bits of each word, so every value is an exact fp32 multiple of 2^-24.
+__device__ __forceinline__ float4 rng_uniform4(const unsigned long long* __restrict__ state, uint32_t stream, unsigned long long group) {
+  const uint4 u = rng_bits4(state, stream, group);
+  const float s = 1.0f / 16777216.0f;
+  return make_float4(static_cast<float>(u.x >> 8) * s, static_cast<float>(u.y >> 8) * s, static_cast<float>(u.z >> 8) * s,
+                     static_cast<float>(u.w >> 8) * s);
+}
 
 // diagnostics / tests: out[4 g .. 4 g + 3] = the four normals of group g
 __global__ void rng_debug_kernel(const unsigned long long* state, uint32_t stream, unsigned long long group0, int ngroups, float* out) {

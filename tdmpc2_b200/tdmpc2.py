@@ -110,6 +110,13 @@ class TDMPC2(torch.nn.Module):
         self.model.load_state_dict(state_dict)
         self._weights_dirty = True
 
+    def export(self, fp):
+        """Write the model file a C or C++ host plans from (tdmpc2_model_file_open, include/tdmpc2_b200.h): the weights
+        acting reads, as fp32 safetensors, with the planner's dims as metadata (export.py).  Load a legacy checkpoint with
+        `load` first.  Needs no GPU."""
+        from .export import export_model
+        export_model(self.model.state_dict(), self.cfg, fp)
+
     # ------------------------------------------------------------------ inference API
     @torch.no_grad()
     def act(self, obs, t0=False, eval_mode=False, task=None):
