@@ -1,7 +1,7 @@
 """The DECLARED NON-PARITY throughput mode with in-kernel noise (tdmpc2_plan_iter_rng, csrc/rng.cuh): the generator's
 statistics, and that every consumer of an element -- the per-step action pass and the MPPI refit that re-derives the elites'
 actions -- regenerates the same value (the refit mean recomputed on the host from the dumped stream must match the kernel's).
-There is no oracle comparison: the oracle consumes torch's draws.  Run on an H100: pytest -m gpu."""
+The float64 comparison of the generator and of philox plans is tests/test_gpu_philox_plan.py.  Run on an H100: pytest -m gpu."""
 import ctypes as C
 
 import pytest
