@@ -1,9 +1,11 @@
 """Shared helpers for parity tests (tolerances are written where they are used)."""
 import ast
+import ctypes as C
 import math
 import os
 
 import numpy as np
+import pytest
 import torch
 
 from tdmpc2_b200.config import workload
@@ -161,6 +163,15 @@ def print_ratio_table():
             print(f"{q:18s} {case:34s} {r:7.2f} {n:9d} {x:9d}")
 
 
+@pytest.fixture(scope="module", autouse=True)
+def ratio_table():
+    """Imported by name into a test module: OBSERVED starts empty for the module, and its table is printed after the
+    module's last test (pytest -s)."""
+    OBSERVED.clear()
+    yield
+    print_ratio_table()
+
+
 def ratio_rule(q, case, k, o32, o64, keep=None, need=0.5):
     """Asserts the ratio rule on the elements `keep` (default: all; at least the fraction `need` of them) and records
     the observed ratio."""
@@ -193,11 +204,58 @@ def level_model(wl, level, **over):
     return cfg, with_target_blend(cfg, sd, 107)
 
 
-def agent_for(cfg, sd, engine):
+def agent_for(cfg, sd, engine="tcgen05"):
     from tdmpc2_b200.tdmpc2 import TDMPC2
     agent = TDMPC2(cfg, device=DEV, engine=engine)
     agent.model.load_state_dict(sd)
     return agent
+
+
+def planner_for(cfg, E, engine, sd):
+    """A Planner for E environments on `engine` (None: the default engine) with `sd` packed."""
+    from tdmpc2_b200.planner import Planner
+    pl = Planner(cfg, E, DEV, engine=engine)
+    pl.pack(sd)
+    return pl
+
+
+def cuda_stream():
+    return torch.cuda.current_stream().cuda_stream
+
+
+def draw_planner(E, N, P, K, H, A, I, num_q):
+    """(library, planner handle, Dims) of a bare planner of these draw counts, made only for tdmpc2_plan_draws: no weights
+    are bound (the caller destroys the handle)."""
+    from tdmpc2_b200 import _cabi
+    lib = _cabi.load()
+    d = _cabi.Dims(num_envs=E, num_samples=N, num_pi_trajs=P, num_elites=K, horizon=H, iterations=I, obs_dim=8, action_dim=A,
+                   latent_dim=64, mlp_dim=64, enc_dim=64, num_enc_layers=2, task_dim=0, num_tasks=1, num_q=num_q, num_bins=101,
+                   simnorm_dim=8, episodic=0, temperature=0.5, min_std=0.05, max_std=2.0, log_std_min=-10.0, log_std_dif=12.0)
+    p = C.c_void_p()
+    _cabi.check(lib.tdmpc2_planner_create(C.byref(d), C.byref(p)))
+    return lib, p, d
+
+
+SENTINEL = 1234.5
+
+
+def plan_draws(h, state, d, eval_mode=False, pixel=False, sentinel=False):
+    """tdmpc2_plan_draws of planner handle h (Dims d) at rng `state` -> (prior, qidx, expo, final, shift) on the host
+    (final None in eval mode, shift None without pixels); with `sentinel` the buffers the call must not write (prior
+    when P = 0, final in eval mode) are passed filled with SENTINEL and returned too."""
+    from tdmpc2_b200 import _cabi
+    E, H, P, A, I, K = d.num_envs, d.horizon, d.num_pi_trajs, d.action_dim, d.iterations, d.num_elites
+    f32 = dict(device=DEV, dtype=torch.float32)
+    prior = torch.full((E, H, max(P, 1) if sentinel else P, A), SENTINEL, **f32)
+    final = torch.full((E, A), SENTINEL, **f32) if (sentinel or not eval_mode) else None
+    qidx = torch.full((I, E, 2), -7, device=DEV, dtype=torch.int32)
+    expo = torch.full((E, K), SENTINEL, **f32)
+    shift = torch.full((E, 2), SENTINEL, **f32) if pixel else None
+    pt = lambda t: None if t is None or t.numel() == 0 else t.data_ptr()
+    _cabi.check(_cabi.load().tdmpc2_plan_draws(h, state.data_ptr(), int(eval_mode), pt(prior), qidx.data_ptr(),
+                                               expo.data_ptr(), pt(final), pt(shift), cuda_stream()))
+    torch.cuda.synchronize()
+    return tuple(None if t is None else t.cpu() for t in (prior, qidx, expo, final, shift))
 
 
 def symlog(x):
@@ -286,6 +344,9 @@ def layer_list(cfg):
     for h in range(cfg.num_q):
         for i in range(3):
             out.append((li, f"_Qs.params.{i}", h, i < 2, False)); li += 1
+    if cfg.episodic:                                   # appended last by the packer (include/tdmpc2_b200.h)
+        for i in range(3):
+            out.append((li, f"_termination.{i}", None, i < 2, False)); li += 1
     return out
 
 
@@ -295,10 +356,8 @@ def fused_layer_ratio_rule(cfg, sd, engine, case):
     |k - y64| <= c * 2^-22 * sum_k |W_nk| |x_k| + 2^-23 |b_n| + 2^-25 / 2^k * sum_{k: W_nk tiny} |x_k|
     (c = LINEAR_C; the last term is the declared subnormal-lo limit, SUBNORMAL_LO) and the ratio rule; LayerNorm + Mish /
     SimNorm outputs obey the ratio rule.  Returns the layers compared: (prefix, head, output width, epilogue)."""
-    from tdmpc2_b200.planner import Planner
     F = torch.nn.functional
-    pl = Planner(cfg, 2, DEV, engine=engine)
-    pl.pack(sd)
+    pl = planner_for(cfg, 2, engine, sd)
     g = torch.Generator().manual_seed(0)
     compared = []
     for (li, prefix, head, has_ln, simnorm) in layer_list(cfg):
@@ -345,16 +404,17 @@ def fused_layer_ratio_rule(cfg, sd, engine, case):
     return compared
 
 
-def to_gpu_noise(n):
+def to_gpu_noise(n, eval_mode=False):
+    """The planner.Noise on the GPU of an oracle PlanNoise (no final draw in eval mode; ShiftAug's shift for pixels)."""
     from tdmpc2_b200.planner import Noise
-    return Noise.from_env_major(n.prior, n.r, n.pi, n.qidx, n.expo, n.final, device=DEV)
+    return Noise.from_env_major(n.prior, n.r, n.pi, n.qidx, n.expo, None if eval_mode else n.final, device=DEV,
+                                shift=n.shift)
 
 
 def plan_three_ways(cfg, sd, engine, E, seed, warm=False):
     """One plan() by the kernels and by the fp32 and float64 oracles on the same inputs and noise.  Every environment
     starts afresh (t0), or with `warm` the odd ones are warm-started from a random previous mean."""
     from oracle.plan_oracle import draw_noise as oracle_noise, plan_oracle
-    from tdmpc2_b200.planner import Planner
     obs = trained_obs(cfg, E, seed)
     task = [(2 * i + 1) % len(cfg.tasks) for i in range(E)] if cfg.multitask else None
     noise = oracle_noise(cfg, 40 + seed, E)
@@ -365,111 +425,115 @@ def plan_three_ways(cfg, sd, engine, E, seed, warm=False):
         prev = 0.3 * torch.randn(E, cfg.horizon, cfg.action_dim, generator=torch.Generator().manual_seed(seed))
     w32 = plan_oracle(cfg, sd, obs, task=task, t0=t0.bool().tolist(), prev_mean=prev, noise=noise)
     w64 = plan_oracle(cfg, sd, obs, task=task, t0=t0.bool().tolist(), prev_mean=prev, noise=noise, dtype=torch.float64)
-    pl = Planner(cfg, E, DEV, engine=engine)
-    pl.pack(sd)
+    pl = planner_for(cfg, E, engine, sd)
     taskv = torch.tensor(task, dtype=torch.int32, device=DEV) if task is not None else None
     action, new_mean, tr = pl.plan(obs.to(DEV), taskv, t0.to(DEV), prev.to(DEV), to_gpu_noise(noise), trace=True)
     torch.cuda.synchronize()
     return {k: v.cpu() for k, v in tr.items()}, action.cpu(), new_mean.cpu(), w32, w64, noise
 
 
-def compare_plans(cfg, case, tr, action, new_mean, w32, w64, noise, pool_envs=False):
-    """Values by the ratio rule per (env, iteration); top-k indices exact where float64's sorted values are separated
-    by more than twice the allowed value error; refit mean / std within 1e-4 plus the value error they inherit, and
-    the action within 1e-4 plus what it inherits from the refits, while the elite set is unambiguous
-    (helpers.compare_with_oracle's logic).  `pool_envs`: the ratio rule takes its maximum over every environment's
-    values of an iteration at once (for a handful of samples per environment, where a maximum over one environment's
-    values says nothing about fp32's error).  Returns counters."""
-    E, K = tr["values"].shape[0], cfg.num_elites
-    n = dict(values=0, topk=0, refit=0, clamped=0, dominated=0, actions=0)
-    wmax, clamped = refit_stats(cfg, w64)
-    keep_all = w64.term_margin > TERM_MARGIN if cfg.episodic else torch.ones_like(w64.values, dtype=torch.bool)
-    pooled = [ratio_rule("plan values", case, tr["values"][:, it], w32.values[:, it], w64.values[:, it],
-                         keep_all[:, it]) for it in range(cfg.iterations)] if pool_envs else None
-    for e in range(E):
-        clean = True
-        stable = None
-        tols = []
+# ------------------------------------------------------------------------------------------ the plan-versus-oracle walk
+def _walk_plan(cfg, tr, action, new_mean, want, noise, envs, value_tol=None, ratio=None, gap=None, keep=None,
+               pool_envs=False):
+    """What "the plan matches the oracle" means.  The kernel's trace `tr` (plan(trace=True)), `action` and `new_mean` of
+    the environments `envs` (rows of the kernel's batch) against oracle PlanTrace rows 0 .. len(envs) - 1 (`want`) and
+    their PlanNoise `noise`.  Per environment, iteration by iteration:
+
+      * values, by one of two criteria: `value_tol` = (atol, rtol), |k - o| <= atol + rtol |o|, an allowed value error of
+        atol + rtol max|o|; or `ratio` = (case, w32), the ratio rule against `want` as float64 and `w32` as the fp32
+        oracle, its bound the allowed error (`pool_envs`: its maximum runs over every environment's values of an
+        iteration at once, for a handful of samples per environment, where one environment's maximum says nothing);
+      * only the samples of `keep` (bool [len(envs), I, N], default all: for episodic samples within TERM_MARGIN of the
+        termination decision); the environment stops being compared at the first iteration with a sample outside it
+        (a flipped termination may change the elite set);
+      * top-k indices exact at the sorted positions separated from both neighbours by more than `gap` (default twice
+        the allowed value error); the environment stops being compared at the first iteration whose k-th and (k+1)-th
+        values are not (the elite SET is ambiguous).  With K == N every sample is an elite: always separated;
+      * refit mean and std within 1e-4 (the north-star tolerance) plus, under the ratio rule, T dv sigma: what a value
+        error dv passes on through the refit weights exp(T (v - v_max)) (Cauchy-Schwarz with sum(w) = 1; sigma the
+        elites' std).
+
+    An environment compared through every iteration then has its new mean held to the last refit's tolerance; where the
+    winning Gumbel logit leads the runner-up by more than 1e-3 (under the ratio rule also only where the picked sorted
+    position is stable, so that it names the same sample) its pick is exact and its action -- the picked elite's first
+    action clamp(mu + sigma eps), drawn from the second-to-last refit, plus sigma eps_final from the last one -- within
+    1e-4 plus each refit's allowance scaled by the noise it meets.  Returns counters of what was compared."""
+    assert (value_tol is None) != (ratio is None), "one value criterion: value_tol=(atol, rtol) or ratio=(case, w32)"
+    K = cfg.num_elites
+    tr = {q: tr[q].detach().cpu() for q in ("values", "elite_idx", "iter_mean", "iter_std", "pick")}
+    action, new_mean = action.detach().cpu(), new_mean.detach().cpu()
+    keep = torch.ones_like(want.values, dtype=torch.bool) if keep is None else keep
+    n = dict(values=0, topk=0, refit=0, clamped=0, dominated=0, means=0, actions=0)
+    wmax, clamped = refit_stats(cfg, want)
+    if ratio is not None:
+        case, w32 = ratio
+        pooled = [ratio_rule("plan values", case, tr["values"][envs, it], w32.values[:, it], want.values[:, it],
+                             keep[:, it]) for it in range(cfg.iterations)] if pool_envs else None
+    for j, e in enumerate(envs):
+        clean, tols = True, []
         for it in range(cfg.iterations):
-            v64 = w64.values[e, it]
-            keep = keep_all[e, it]
-            if pooled:
-                allowed = pooled[it]
+            v, kept = want.values[j, it], keep[j, it]
+            if ratio is None:
+                atol, rtol = value_tol
+                err = (tr["values"][e, it].double() - v.double()).abs()
+                ok = (err <= atol + rtol * v.double().abs()) | ~kept
+                assert bool(ok.all()), f"values env={e} it={it}: err {float(err[kept].max()):.3e}"
+                allowed = atol + rtol * float(v.abs().max())
             else:
-                allowed = ratio_rule("plan values", case, tr["values"][e, it], w32.values[e, it], v64, keep)
-            n["values"] += int(keep.sum())
-            if not bool(keep.all()):
-                clean = False                           # a flipped termination may change the elite set
-                break
-            gap = 2 * allowed
-            stable = stable_positions(v64, K, gap)
-            assert torch.equal(tr["elite_idx"][e, it][stable], w64.elite_idx[e, it][stable]), f"top-k {case} env={e} it={it}"
-            n["topk"] += int(stable.sum())
-            if not bool(boundary_separated(v64, K, gap)):
+                allowed = pooled[it] if pool_envs else ratio_rule("plan values", case, tr["values"][e, it],
+                                                                  w32.values[j, it], v, kept)
+            n["values"] += int(kept.sum())
+            if not bool(kept.all()):
                 clean = False
                 break
-            # The refit weights exp(T (v - v_max)) pass a value error dv on to the mean and the std as at most
-            # T dv sigma (Cauchy-Schwarz with sum(w) = 1; sigma = the elites' std): on top of the 1e-4 north-star tolerance
-            tol = 1e-4 + cfg.temperature * allowed * w64.iter_std[e, it]
-            tols.append(float((tol - 1e-4).max()))
+            gap_it = 2 * allowed if gap is None else gap
+            stable = stable_positions(v, K, gap_it)
+            assert torch.equal(tr["elite_idx"][e, it][stable], want.elite_idx[j, it][stable]), f"top-k env={e} it={it}"
+            n["topk"] += int(stable.sum())
+            if not bool(boundary_separated(v, K, gap_it)):
+                clean = False
+                break
+            extra = 0.0 if ratio is None else cfg.temperature * allowed * want.iter_std[j, it].double()
+            tol = 1e-4 + extra
+            tols.append(float((tol - 1e-4).max()) if ratio is not None else 0.0)
             for q in ("iter_mean", "iter_std"):
-                err = (tr[q][e, it].double() - getattr(w64, q)[e, it]).abs()
-                assert bool((err <= tol).all()), f"{q} {case} env={e} it={it}: {float(err.max()):.2e}"
+                err = (tr[q][e, it].double() - getattr(want, q)[j, it].double()).abs()
+                assert bool((err <= tol).all()), f"{q} env={e} it={it}: {float(err.max()):.2e}"
             n["refit"] += 1
-            n["clamped"] += int(clamped[e, it])
-            n["dominated"] += int(wmax[e, it] > 0.9)
-        if clean:
-            assert bool(((new_mean[e].double() - w64.mean[e]).abs() <= tol).all())
-            logits = w64.score[e].log() - noise.expo[e].double().log()
-            top2 = _top_k_plus_one(logits, 1)               # one elite: its pick is never ambiguous
-            # the pick is a position in the sorted elite list: it names the same sample only where that order is stable
-            if float(top2[0] - top2[1]) > 1e-3 and bool(stable[int(w64.pick[e])]):
-                assert int(tr["pick"][e]) == int(w64.pick[e])
-                # The action is the picked elite's first action clamp(mu + sigma eps), drawn from the second-to-last
-                # refit, plus sigma eps_final from the last refit: each refit's value-induced error reaches the action
-                # scaled by the noise it meets (1e-4 alone when the values are exact)
-                eps_r = float(noise.r[e, -1].abs().max()) if noise.r[e, -1].numel() else 0.0
-                eps_f = float(noise.final[e].abs().max()) if noise.final is not None else 0.0
-                tol_a = 1e-4 + (tols[-2] if len(tols) > 1 else 0.0) * (1 + eps_r) + tols[-1] * eps_f
-                err = float((action[e].double() - w64.action[e]).abs().max())
-                assert err <= tol_a, f"action {case} env={e}: {err:.2e} > {tol_a:.2e}"
-                n["actions"] += 1
+            n["clamped"] += int(clamped[j, it])
+            n["dominated"] += int(wmax[j, it] > 0.9)
+        if not clean:
+            continue
+        err = (new_mean[e].double() - want.mean[j].double()).abs()
+        assert bool((err <= tol).all()), f"mean env={e}: {float(err.max()):.2e}"
+        n["means"] += 1
+        logits = want.score[j].log() - noise.expo[j].to(want.score.dtype).log()
+        top2 = _top_k_plus_one(logits, 1)               # one elite: its pick is never ambiguous
+        if float(top2[0] - top2[1]) > 1e-3 and (ratio is None or bool(stable[int(want.pick[j])])):
+            assert int(tr["pick"][e]) == int(want.pick[j]), f"pick env={e}: {int(tr['pick'][e])} != {int(want.pick[j])}"
+            eps_r = float(noise.r[j, -1].abs().max()) if noise.r[j, -1].numel() else 0.0
+            eps_f = float(noise.final[j].abs().max()) if noise.final is not None else 0.0
+            tol_a = 1e-4 + (tols[-2] if len(tols) > 1 else 0.0) * (1 + eps_r) + tols[-1] * eps_f
+            err = float((action[e].double() - want.action[j].double()).abs().max())
+            assert err <= tol_a, f"action env={e}: {err:.2e} > {tol_a:.2e}"
+            n["actions"] += 1
     return n
 
 
-def compare_with_oracle(cfg, tr, action, new_mean, want, on, envs, value_atol=5e-5, value_rtol=1e-5, gap=None):
-    """Kernel trace of environments `envs` (rows of the big batch) against oracle rows 0..len(envs)-1.
-    values: |got - want| <= value_atol + value_rtol * |want| (the tolerance of tests/test_gpu_parity.py: fp32 round-off
-    level -- the fp32 oracle itself is only that close to float64); top-k indices exact where the oracle's sorted values
-    are separated by > gap (default 2 x the value tolerance at that magnitude, at least 1e-4); refit mean/std and final
+def compare_plans(cfg, case, tr, action, new_mean, w32, w64, noise, pool_envs=False):
+    """Every environment of a plan against the fp32 (w32) and float64 (w64) oracles by the ratio rule (_walk_plan); for
+    episodic models the samples whose termination logit is within TERM_MARGIN of the decision are not compared."""
+    keep = w64.term_margin > TERM_MARGIN if cfg.episodic else None
+    return _walk_plan(cfg, tr, action, new_mean, w64, noise, list(range(tr["values"].shape[0])), ratio=(case, w32),
+                      keep=keep, pool_envs=pool_envs)
+
+
+def compare_with_oracle(cfg, tr, action, new_mean, want, on, envs, value_atol=5e-5, value_rtol=1e-5, gap=None, keep=None):
+    """Kernel trace of environments `envs` (rows of the big batch) against oracle rows 0..len(envs)-1 (_walk_plan):
+    values |got - want| <= value_atol + value_rtol * |want| (default: the fp32 round-off level of tests/test_gpu_parity.py
+    -- the fp32 oracle itself is only that close to float64); top-k indices exact where the oracle's sorted values are
+    separated by > gap (default 2 x the value tolerance at the iteration's largest |value|); refit mean / std, new mean and
     action within 1e-4 (north-star tolerance) while the elite set is unambiguous.  Returns counters so that callers can
     assert that the comparisons really ran."""
-    K = cfg.num_elites
-    n = dict(values=0, topk=0, refit=0, actions=0, max_value_err=0.0)
-    for j, e in enumerate(envs):
-        clean = True
-        for it in range(cfg.iterations):
-            v_got, v_want = tr["values"][e, it].cpu(), want.values[j, it]
-            err = float((v_got - v_want).abs().max())
-            n["max_value_err"] = max(n["max_value_err"], err)
-            assert torch.allclose(v_got, v_want, atol=value_atol, rtol=value_rtol), f"values env={e} it={it} err={err:.3e}"
-            n["values"] += v_want.numel()
-            gap_it = gap if gap is not None else max(1e-4, 2 * (value_atol + value_rtol * float(v_want.abs().max())))
-            stable = stable_positions(v_want, K, gap_it)
-            assert torch.equal(tr["elite_idx"][e, it].cpu()[stable], want.elite_idx[j, it][stable]), f"top-k env={e} it={it}"
-            n["topk"] += int(stable.sum())
-            if not bool(boundary_separated(v_want, K, gap_it)):
-                clean = False
-                break
-            assert torch.allclose(tr["iter_mean"][e, it].cpu(), want.iter_mean[j, it], atol=1e-4, rtol=0), f"mean env={e} it={it}"
-            assert torch.allclose(tr["iter_std"][e, it].cpu(), want.iter_std[j, it], atol=1e-4, rtol=0), f"std env={e} it={it}"
-            n["refit"] += 1
-        if clean:
-            assert torch.allclose(new_mean[e].cpu(), want.mean[j], atol=1e-4, rtol=0)
-            logits = want.score[j].log() - on.expo[j].log()
-            top2 = torch.topk(logits, 2).values
-            if float(top2[0] - top2[1]) > 1e-3:
-                assert int(tr["pick"][e].cpu()) == int(want.pick[j])
-                assert torch.allclose(action[e].cpu(), want.action[j], atol=1e-4, rtol=0), f"action env={e}"
-                n["actions"] += 1
-    return n
+    return _walk_plan(cfg, tr, action, new_mean, want, on, list(envs), value_tol=(value_atol, value_rtol), gap=gap,
+                      keep=keep)

@@ -20,7 +20,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from helpers import DEV, OBSERVED, level_model, print_ratio_table, ratio_rule, trained_obs
+from helpers import DEV, level_model, ratio_rule, trained_obs
+from helpers import ratio_table  # noqa: F401 (autouse: this module's ratio table)
 from oracle.pi_oracle import PI_KEYS, update_pi_oracle
 from oracle.update_oracle import Tape, update_oracle
 from test_gpu_shape_envelope import CASES as ENVELOPE, shape
@@ -31,13 +32,6 @@ pytestmark = pytest.mark.gpu
 ENGINES = ["simt", "tcgen05"]
 LEVELS = ["init", "mid"]
 GBK = 16                 # kGBK: gemm_f32's K tile
-
-
-@pytest.fixture(scope="module", autouse=True)
-def ratio_table():
-    OBSERVED.clear()
-    yield
-    print_ratio_table()
 
 
 # ------------------------------------------------------------------------------------ shape arithmetic (api.cu)

@@ -12,19 +12,16 @@ import pytest
 import torch
 from scipy import stats
 
+from helpers import cuda_stream, draw_planner, plan_draws, planner_for
 from tdmpc2_b200 import _cabi
 from tdmpc2_b200.config import workload
 from tdmpc2_b200.export import export_model
-from tdmpc2_b200.planner import Planner, alloc_noise, discount_table
+from tdmpc2_b200.planner import alloc_noise, discount_table
 from tdmpc2_b200.synth import synth_state_dict
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CASES = {"c1": ("c1", {}), "tiny-mt": ("tiny-mt", {}), "episodic": ("tiny", {"episodic": True}), "tiny-rgb": ("tiny-rgb", {})}
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def _model(case, E, tmp_path, **over):
@@ -61,8 +58,8 @@ class CModel:
         _cabi.check(lib.tdmpc2_model_file_device_bytes(self.f, C.byref(self.d), C.byref(nb))); self.buf = u8(nb.value)
         self.W, self.conv, self.grid = _cabi.Weights(), _cabi.ConvWeights(), C.c_void_p()
         _cabi.check(lib.tdmpc2_model_file_upload(self.f, C.byref(self.d), self.buf.data_ptr(), C.byref(self.W), C.byref(self.conv),
-                                                 C.byref(self.grid), _stream()))
-        _cabi.check(lib.tdmpc2_pack_weights(self.p, C.byref(self.W), _stream()))
+                                                 C.byref(self.grid), cuda_stream()))
+        _cabi.check(lib.tdmpc2_pack_weights(self.p, C.byref(self.W), cuda_stream()))
         self.enc, self.enc_ws = None, None
         if self.pixel:
             self.enc = C.c_void_p()
@@ -96,24 +93,11 @@ class CModel:
         a.t0, a.eval_mode, a.rng_state = t0.data_ptr(), int(bool(eval_mode)), self.rng_state.data_ptr()
         a.prev_mean, a.action_out, a.grid_base = self.prev_mean.data_ptr(), self.action.data_ptr(), self.grid.value
         return self.lib.tdmpc2_act(self.p, self.enc, None if self.enc_ws is None else self.enc_ws.data_ptr(),
-                                   C.byref(self.conv) if self.pixel else None, C.byref(a), self.scratch.data_ptr(), _stream())
+                                   C.byref(self.conv) if self.pixel else None, C.byref(a), self.scratch.data_ptr(), cuda_stream())
 
     def act(self, *args, **kw):
         _cabi.check(self.act_rc(*args, **kw))
         return self.action.clone(), self.prev_mean.clone()
-
-
-def draws(lib, p, state, d, eval_mode=False, pixel=False):
-    """tdmpc2_plan_draws of planner p at `state` -> (prior, qidx, expo, final, shift)."""
-    E, H, P, A, I, K = d.num_envs, d.horizon, d.num_pi_trajs, d.action_dim, d.iterations, d.num_elites
-    f32 = dict(device="cuda", dtype=torch.float32)
-    prior, qidx = torch.empty(E, H, P, A, **f32), torch.empty(I, E, 2, device="cuda", dtype=torch.int32)
-    expo, final = torch.empty(E, K, **f32), None if eval_mode else torch.empty(E, A, **f32)
-    shift = torch.empty(E, 2, **f32) if pixel else None
-    pt = lambda t: None if t is None or t.numel() == 0 else t.data_ptr()
-    _cabi.check(lib.tdmpc2_plan_draws(p, state.data_ptr(), int(eval_mode), pt(prior), qidx.data_ptr(), expo.data_ptr(), pt(final),
-                                      pt(shift), _stream()))
-    return prior, qidx, expo, final, shift
 
 
 def _inputs(cfg, E, steps, seed=3):
@@ -184,15 +168,8 @@ def test_discount_powers_follow_an_overridden_horizon(case, tmp_path):
 
 
 # ------------------------------------------------------------------------------------------------------------ draw laws
-def _draw_planner(num_q, E=65536, I=4):
-    """A planner whose draws are large: prior E x 16 x 16 normals, I E qidx rows, E x 16 exponentials, E x 16 finals."""
-    lib = _cabi.load()
-    d = _cabi.Dims(num_envs=E, num_samples=64, num_pi_trajs=16, num_elites=16, horizon=1, iterations=I, obs_dim=8, action_dim=16,
-                   latent_dim=64, mlp_dim=64, enc_dim=64, num_enc_layers=2, task_dim=0, num_tasks=1, num_q=num_q, num_bins=101,
-                   simnorm_dim=8, episodic=0, temperature=0.5, min_std=0.05, max_std=2.0, log_std_min=-10.0, log_std_dif=12.0)
-    p = C.c_void_p()
-    _cabi.check(lib.tdmpc2_planner_create(C.byref(d), C.byref(p)))
-    return lib, p, d
+# a planner whose draws are large: prior E x 16 x 16 normals, I E qidx rows, E x 16 exponentials, E x 16 finals
+LARGE_DRAWS = dict(E=65536, N=64, P=16, K=16, H=1, A=16)
 
 
 def _chi2_ok(counts):
@@ -203,26 +180,25 @@ def _chi2_ok(counts):
 
 
 def test_draw_laws_normals_and_exponentials():
-    lib, p, d = _draw_planner(5)
+    lib, p, d = draw_planner(I=4, num_q=5, **LARGE_DRAWS)
     st = torch.tensor([987654321, 17], dtype=torch.int64, device="cuda")
-    prior, qidx, expo, final, shift = draws(lib, p, st, d, pixel=True)
-    torch.cuda.synchronize()
-    for x in (prior.flatten().double().cpu(), final.flatten().double().cpu()):
+    prior, qidx, expo, final, shift = plan_draws(p, st, d, pixel=True)
+    for x in (prior.flatten().double(), final.flatten().double()):
         n = x.numel()
         assert n >= 1 << 20 and torch.isfinite(x).all()
         assert abs(float(x.mean())) < 5.0 / n ** 0.5 and abs(float(x.var()) - 1.0) < 0.01
         assert abs(float((x ** 4).mean()) - 3.0) < 0.05 and abs(float((x ** 3).mean())) < 0.02
         assert abs(float((x[:-1] * x[1:]).mean())) < 0.005
-    x = expo.flatten().double().cpu()
+    x = expo.flatten().double()
     assert x.numel() >= 1 << 20 and torch.isfinite(x).all() and bool((x >= 0).all())
     assert abs(float(x.mean()) - 1.0) < 5.0 / x.numel() ** 0.5 and abs(float(x.var()) - 1.0) < 0.02
-    s = shift.flatten().cpu()
+    s = shift.flatten()
     assert torch.equal(s, s.floor()) and int(s.min()) == 0 and int(s.max()) == 6
     ok, chi = _chi2_ok(torch.bincount(s.long(), minlength=7).numpy())
     assert ok, chi
     # deterministic for the same state; every kind changes with the counter
-    again = draws(lib, p, st, d, pixel=True)
-    other = draws(lib, p, torch.tensor([987654321, 18], dtype=torch.int64, device="cuda"), d, pixel=True)
+    again = plan_draws(p, st, d, pixel=True)
+    other = plan_draws(p, torch.tensor([987654321, 18], dtype=torch.int64, device="cuda"), d, pixel=True)
     for a, b, c in zip((prior, qidx, expo, final, shift), again, other):
         assert torch.equal(a, b) and not torch.equal(a, c)
     lib.tdmpc2_planner_destroy(p)
@@ -230,9 +206,9 @@ def test_draw_laws_normals_and_exponentials():
 
 @pytest.mark.parametrize("num_q", [5, 8])
 def test_draw_laws_qidx_is_an_ordered_pair_of_distinct_heads(num_q):
-    lib, p, d = _draw_planner(num_q, I=8)
+    lib, p, d = draw_planner(I=8, num_q=num_q, **LARGE_DRAWS)
     st = torch.tensor([42, 3], dtype=torch.int64, device="cuda")
-    q = draws(lib, p, st, d)[1].view(-1, 2).long().cpu()
+    q = plan_draws(p, st, d)[1].view(-1, 2).long()
     assert q.shape[0] >= 1 << 19
     assert bool((q >= 0).all()) and bool((q < num_q).all()) and bool((q[:, 0] != q[:, 1]).all())
     code = q[:, 0] * num_q + q[:, 1]
@@ -245,16 +221,15 @@ def test_draw_laws_qidx_is_an_ordered_pair_of_distinct_heads(num_q):
 
 
 def test_draw_streams_are_uncorrelated_with_each_other_and_the_iteration_streams():
-    lib, p, d = _draw_planner(5)
+    lib, p, d = draw_planner(I=4, num_q=5, **LARGE_DRAWS)
     st = torch.tensor([2024, 5], dtype=torch.int64, device="cuda")
-    prior, qidx, expo, final, shift = draws(lib, p, st, d, pixel=True)
+    prior, qidx, expo, final, shift = plan_draws(p, st, d, pixel=True)
     n = final.numel()
     it = []
     for s in (0, 1):                                                     # tdmpc2_plan_iter_rng's streams of iteration 0
         out = torch.empty(n, device="cuda")
-        _cabi.check(lib.tdmpc2_debug_rng(st.data_ptr(), s, 0, n // 4, out.data_ptr(), _stream()))
-        it.append(out)
-    torch.cuda.synchronize()
+        _cabi.check(lib.tdmpc2_debug_rng(st.data_ptr(), s, 0, n // 4, out.data_ptr(), cuda_stream()))
+        it.append(out.cpu())
     z = lambda t: (t.flatten()[:n].double() - t.flatten()[:n].double().mean()) / t.flatten()[:n].double().std()
     series = [z(prior), z(final), z(expo), z(qidx[..., 0].float()), z(shift), z(it[0]), z(it[1])]
     for i in range(len(series)):
@@ -276,16 +251,15 @@ def test_act_is_the_python_philox_plan_bit_for_bit(case, E, eval_mode, tmp_path)
     cfg, sd, path = _model(case, E, tmp_path, rng="philox", rng_seed=seed)
     m = CModel(path, seed=seed)
     assert m.E == E
-    pl = Planner(cfg, E, "cuda:0")
-    pl.pack(sd)
+    pl = planner_for(cfg, E, None, sd)
     assert pl.philox and int(pl.rng_state[0]) == seed
     obs, task = _inputs(cfg, E, 3)
     prev = torch.zeros(E, cfg.horizon, cfg.action_dim, device="cuda")
     for k in range(3):
         t0 = torch.full((E,), int(k == 0), dtype=torch.uint8, device="cuda")
         nz = alloc_noise(cfg, E, "cuda", eval_mode)
-        prior, qidx, expo, final, shift = draws(m.lib, m.p, torch.tensor([seed, k + 1], dtype=torch.int64, device="cuda"), m.d,
-                                                eval_mode, m.pixel)
+        prior, qidx, expo, final, shift = plan_draws(m.p, torch.tensor([seed, k + 1], dtype=torch.int64, device="cuda"), m.d,
+                                                     eval_mode, m.pixel)
         nz.prior.copy_(prior); nz.qidx.copy_(qidx); nz.expo.copy_(expo)
         if not eval_mode:
             nz.final.copy_(final)

@@ -7,6 +7,7 @@ import torch
 
 from tdmpc2_b200.config import workload
 from tdmpc2_b200.synth import synth_state_dict
+from helpers import planner_for, to_gpu_noise
 
 pytestmark = pytest.mark.gpu
 
@@ -14,7 +15,6 @@ pytestmark = pytest.mark.gpu
 @pytest.mark.parametrize("wl,engine", [("c1", "tcgen05"), ("tiny-mt", "tcgen05"), ("tiny-wide", "tcgen05")])
 def test_fast_mode_is_close_to_but_not_at_parity(wl, engine):
     from oracle.plan_oracle import draw_noise as oracle_noise, plan_oracle
-    from tdmpc2_b200.planner import Noise, Planner
     E = 2
     cfg = workload(wl, num_envs=E)
     sd = synth_state_dict(cfg, seed=13, perturb=True)
@@ -24,13 +24,12 @@ def test_fast_mode_is_close_to_but_not_at_parity(wl, engine):
     t0, task = [True, False], ([1, 3] if cfg.multitask else None)
     on = oracle_noise(cfg, 50, E)
     want = plan_oracle(cfg, sd, obs, task=task, t0=t0, prev_mean=prev, noise=on)
-    noise = Noise.from_env_major(on.prior, on.r, on.pi, on.qidx, on.expo, on.final, device="cuda")
+    noise = to_gpu_noise(on)
     taskv = None if task is None else torch.tensor(task, dtype=torch.int32).cuda()
     got = {}
     for passes in (3, 1, 3):                                   # parity, fast, parity again (the knob leaves no state behind)
-        pl = Planner(cfg.replace(passes=passes), E, "cuda:0", engine=engine)
+        pl = planner_for(cfg.replace(passes=passes), E, engine, sd)
         assert pl.passes == passes
-        pl.pack(sd)
         _, _, tr = pl.plan(obs.cuda(), taskv, torch.tensor(t0, dtype=torch.uint8).cuda(), prev.cuda(), noise, trace=True)
         torch.cuda.synchronize()
         got.setdefault(passes, []).append((tr["values"][:, 0].cpu(), tr["elite_idx"][:, 0].cpu()))

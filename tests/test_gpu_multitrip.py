@@ -14,16 +14,9 @@ import torch
 
 from tdmpc2_b200.config import workload
 from tdmpc2_b200.synth import synth_state_dict
-from helpers import mixed_noise, slice_noise, compare_with_oracle
+from helpers import compare_with_oracle, mixed_noise, planner_for, slice_noise
 
 pytestmark = pytest.mark.gpu
-
-
-def _planner(cfg, E, engine, sd):
-    from tdmpc2_b200.planner import Planner
-    pl = Planner(cfg, E, "cuda:0", engine=engine)
-    pl.pack(sd)
-    return pl
 
 
 def _inputs(cfg, E, seed):
@@ -62,7 +55,7 @@ def test_many_trip_batch_is_bit_identical_to_small_runs_and_matches_oracle(E, en
     oracle_envs = [0, E // 3, E // 2 + 1, E - 1]
     nz_a, on_a = mixed_noise(cfg, E, oracle_envs, 100)
     nz_b, on_b = mixed_noise(cfg, E, oracle_envs, 200)
-    pl = _planner(cfg, E, engine, sd)
+    pl = planner_for(cfg, E, engine, sd)
     big1, big2 = _two_plans(pl, obs, task, t0, prev, nz_a, nz_b)
     del pl
     # ---- bit-identity against single-trip 2-environment runs of the same environments
@@ -70,7 +63,7 @@ def test_many_trip_batch_is_bit_identical_to_small_runs_and_matches_oracle(E, en
     for envs in pairs:
         idx = list(envs)
         cfg2 = workload("c1", num_envs=2)
-        pl2 = _planner(cfg2, 2, engine, sd)
+        pl2 = planner_for(cfg2, 2, engine, sd)
         small1, small2 = _two_plans(pl2, obs[idx], None, t0[idx], prev[idx], slice_noise(nz_a, idx), slice_noise(nz_b, idx))
         for big, small, which in ((big1, small1, "first"), (big2, small2, "warm-started")):
             (ab, mb, trb), (as_, ms, trs) = big, small
@@ -106,7 +99,7 @@ def test_c5_planner_shape_on_5m_model():
     nz, on = mixed_noise(cfg, E, oracle_envs, 300)
     out = {}
     for engine in ("simt", "tcgen05"):
-        pl = _planner(cfg, E, engine, sd)
+        pl = planner_for(cfg, E, engine, sd)
         a, m, tr = pl.plan(obs.cuda(), None, t0.cuda(), prev.cuda(), nz, trace=True)
         torch.cuda.synchronize()
         out[engine] = (a, m, tr)
@@ -136,7 +129,7 @@ def test_wide_presets_multi_env(wl):
     obs, prev, t0, task = _inputs(cfg, E, 33)
     oracle_envs = [1]
     nz, on = mixed_noise(cfg, E, oracle_envs, 400)
-    pl = _planner(cfg, E, None, sd)
+    pl = planner_for(cfg, E, None, sd)
     taskv = None if task is None else task.to(torch.int32).cuda()
     a, m, tr = pl.plan(obs.cuda(), taskv, t0.cuda(), prev.cuda(), nz, trace=True)
     torch.cuda.synchronize()

@@ -11,21 +11,21 @@
 
 The tensor-core engine only: the SIMT engine refuses in-kernel noise (tests/test_gpu_c_act.py).  Run on an H100:
 pytest -m gpu tests/test_gpu_philox_plan.py -s (prints the ratio table and the generator's largest error)."""
-import ctypes as C
 import functools
 
 import numpy as np
 import pytest
 import torch
 
-from helpers import (DEV, FLOOR, OBSERVED, RATIO, boundary_separated, compare_plans, level_model, print_ratio_table,
-                     stable_positions, trained_obs, _top_k_plus_one)
+from helpers import (DEV, FLOOR, RATIO, SENTINEL, boundary_separated, compare_plans, cuda_stream, draw_planner, level_model,
+                     plan_draws, planner_for, stable_positions, trained_obs, _top_k_plus_one)
+from helpers import ratio_table  # noqa: F401 (autouse: this module's ratio table)
 from oracle import philox_oracle as ph
 from test_gpu_shape_envelope import CASES as ENVELOPE, shape
 from test_philox_oracle_cpu import PINNED, ZERO_EXPO
 from tdmpc2_b200 import _cabi
 from tdmpc2_b200.config import workload
-from tdmpc2_b200.planner import Planner, alloc_noise
+from tdmpc2_b200.planner import alloc_noise
 
 pytestmark = pytest.mark.gpu
 SEED_HI = 0x1D872B41C9A5F3E7            # a seed >= 2^32 (below 2^63: Planner keeps 63 bits)
@@ -34,19 +34,15 @@ GEN_ERR = {}                            # what -> largest |device - float64| in 
 
 
 @pytest.fixture(scope="module", autouse=True)
-def tables():
-    OBSERVED.clear()
+def generator_table():
+    """The generator's largest errors, printed after the ratio table (pytest sets up a module's autouse fixtures in
+    order of name, so this one before ratio_table, and tears them down in reverse)."""
     GEN_ERR.clear()
     yield
-    print_ratio_table()
     if GEN_ERR:
         print(f"\n{'normals':44s} {'max |dev - f64| / (2^-24 rho)':>30s}")
         for k, v in sorted(GEN_ERR.items()):
             print(f"{k:44s} {v:30.3f}")
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def _state(seed, plan):
@@ -58,7 +54,7 @@ def dump(state, stream, group0, ngroups):
     """tdmpc2_debug_rng: the normals of groups group0 .. group0 + ngroups - 1 -> float32 numpy [ngroups, 4]."""
     lib = _cabi.load()
     out = torch.empty(4 * ngroups, device=DEV, dtype=torch.float32)
-    _cabi.check(lib.tdmpc2_debug_rng(state.data_ptr(), stream, group0, ngroups, out.data_ptr(), _stream()))
+    _cabi.check(lib.tdmpc2_debug_rng(state.data_ptr(), stream, group0, ngroups, out.data_ptr(), cuda_stream()))
     torch.cuda.synchronize()
     return out.cpu().numpy().reshape(ngroups, 4)
 
@@ -106,37 +102,6 @@ def test_generator_extremes(name):
 
 
 # ------------------------------------------------------------------------------------------------ (b) tdmpc2_plan_draws
-def draw_planner(E, N, P, K, H, A, I, num_q):
-    lib = _cabi.load()
-    d = _cabi.Dims(num_envs=E, num_samples=N, num_pi_trajs=P, num_elites=K, horizon=H, iterations=I, obs_dim=8, action_dim=A,
-                   latent_dim=64, mlp_dim=64, enc_dim=64, num_enc_layers=2, task_dim=0, num_tasks=1, num_q=num_q, num_bins=101,
-                   simnorm_dim=8, episodic=0, temperature=0.5, min_std=0.05, max_std=2.0, log_std_min=-10.0, log_std_dif=12.0)
-    p = C.c_void_p()
-    _cabi.check(lib.tdmpc2_planner_create(C.byref(d), C.byref(p)))
-    return lib, p
-
-
-SENTINEL = 1234.5
-
-
-def device_draws(h, state, E, H, P, A, I, K, eval_mode, pixel, sentinel=False):
-    """tdmpc2_plan_draws of planner handle h -> (prior, qidx, expo, final, shift) on the host; with `sentinel` the buffers
-    the call must not write (prior when P = 0, final in eval mode) are passed filled with SENTINEL and returned too."""
-    lib = _cabi.load()
-    f32 = dict(device=DEV, dtype=torch.float32)
-    prior = torch.full((E, H, max(P, 1) if sentinel else P, A), SENTINEL, **f32)
-    final = torch.full((E, A), SENTINEL, **f32) if (sentinel or not eval_mode) else None
-    qidx = torch.full((I, E, 2), -7, device=DEV, dtype=torch.int32)
-    expo = torch.full((E, K), SENTINEL, **f32)
-    shift = torch.full((E, 2), SENTINEL, **f32) if pixel else None
-    pt = lambda t: None if t is None or t.numel() == 0 else t.data_ptr()
-    _cabi.check(lib.tdmpc2_plan_draws(h, state.data_ptr(), int(eval_mode), pt(prior), qidx.data_ptr(), expo.data_ptr(), pt(final),
-                                      pt(shift), _stream()))
-    torch.cuda.synchronize()
-    cpu = lambda t: None if t is None else t.cpu()
-    return cpu(prior), cpu(qidx), cpu(expo), cpu(final), cpu(shift)
-
-
 def check_expo(what, dev, want):
     """Exponentials within 2 ulp (fp32, at the float64 value) of float64; an exact 0 stays exact."""
     dev, want = np.asarray(dev, dtype=np.float64).reshape(-1), np.asarray(want, dtype=np.float64).reshape(-1)
@@ -154,10 +119,10 @@ DRAW_CASES = [(2, False, 7, True, (5, 1)), (3, True, 7, False, (SEED_HI, 3)), (4
                          ids=[f"q{c[0]}-{'eval' if c[1] else 'explore'}-P{c[2]}-{'pixel' if c[3] else 'state'}" for c in DRAW_CASES])
 def test_plan_draws_are_the_host_law(num_q, eval_mode, P, pixel, state):
     E, H, A, I, K, N = 3, 2, 5, 3, 9, 16
-    lib, p = draw_planner(E, N, P, K, H, A, I, num_q)
+    lib, p, d = draw_planner(E, N, P, K, H, A, I, num_q)
     seed, plan = state
     try:
-        prior, qidx, expo, final, shift = device_draws(p, _state(seed, plan), E, H, P, A, I, K, eval_mode, pixel, sentinel=True)
+        prior, qidx, expo, final, shift = plan_draws(p, _state(seed, plan), d, eval_mode, pixel, sentinel=True)
     finally:
         lib.tdmpc2_planner_destroy(p)
     want = ph.plan_draws(seed, plan, E, H, P, A, I, K, num_q, eval_mode, pixel)
@@ -180,9 +145,9 @@ def test_expo_extremes():
     (seed, plan, _, g0, c0), (_, _, _, g1, c1) = PINNED["expo=0"], PINNED["expo=24ln2"]
     E, K = 65536, 96
     assert 4 * max(g0, g1) + 3 < E * K
-    lib, p = draw_planner(E, K, 0, K, 1, 1, 1, 2)
+    lib, p, d = draw_planner(E, K, 0, K, 1, 1, 1, 2)
     try:
-        expo = device_draws(p, _state(seed, plan), E, 1, 0, 1, 1, K, True, False)[2].numpy().reshape(-1)
+        expo = plan_draws(p, _state(seed, plan), d, eval_mode=True)[2].numpy().reshape(-1)
     finally:
         lib.tdmpc2_planner_destroy(p)
     assert expo[4 * g0 + c0] == 0.0
@@ -273,15 +238,14 @@ def test_philox_plan_against_oracles(case):
     pixel = cfg.get("obs", "state") == "rgb"
     s = rgb_shape(cfg) if pixel else shape(cfg)
     assert check(s, cfg), f"{case} does not reach {what!r}: {s}"
-    pl = Planner(cfg, E, DEV)
-    pl.pack(sd)
+    pl = planner_for(cfg, E, None, sd)
     assert pl.philox and int(pl.rng_state[0]) == seed
     if state0 is not None:
         pl.rng_state[1] = state0[1]
     plan = int(pl.rng_state[1]) + 1                                    # plan() advances the counter first
     state = _state(seed, plan)
     nz = alloc_noise(cfg, E, DEV, eval_mode)
-    prior, qidx, expo, final, shift = device_draws(pl.h, state, E, H, P, A, I, K, eval_mode, pixel)
+    prior, qidx, expo, final, shift = plan_draws(pl.h, state, pl._dims, eval_mode, pixel)
     nz.qidx.copy_(qidx); nz.expo.copy_(expo)
     if P > 0:
         nz.prior.copy_(prior)
@@ -391,13 +355,12 @@ def test_pick_with_an_exact_zero_exponential():
     cfg = workload("tiny", rng="philox", rng_seed=seed)
     from tdmpc2_b200.synth import synth_state_dict
     sd = synth_state_dict(cfg, seed=7, perturb=True)
-    E, H, P, A, I, K = cfg.num_envs, cfg.horizon, cfg.num_pi_trajs, cfg.action_dim, cfg.iterations, cfg.num_elites
+    E, K = cfg.num_envs, cfg.num_elites
     assert (E, K) == (2, 16)
-    pl = Planner(cfg, E, DEV)
-    pl.pack(sd)
+    pl = planner_for(cfg, E, None, sd)
     assert int(pl.rng_state[1]) == plan - 1
     nz = alloc_noise(cfg, E, DEV)
-    prior, qidx, expo, final, _ = device_draws(pl.h, _state(seed, plan), E, H, P, A, I, K, False, False)
+    prior, qidx, expo, final, _ = plan_draws(pl.h, _state(seed, plan), pl._dims)
     assert float(expo.reshape(-1)[elem]) == 0.0
     nz.prior.copy_(prior); nz.qidx.copy_(qidx); nz.expo.copy_(expo); nz.final.copy_(final)
     obs, _, t0, prev = plan_inputs(cfg, E, 4)

@@ -5,6 +5,7 @@ prologue.  Run on an H100: pytest -m gpu."""
 import pytest
 import torch
 
+from helpers import agent_for
 from oracle.wm_rgb_oracle import RGB_CASES, load_rgb_case, rgb_case_model
 from tdmpc2_b200.config import workload
 from tdmpc2_b200.synth import synth_state_dict
@@ -13,13 +14,6 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda"
 Z_TOL = 1e-5                       # the bar of test_gpu_pixels.py: exact fp32 products, another summation order than ATen's
 TD_TOL = (5e-5, 1e-5)              # "value" tolerance of the world-model goldens (test_gpu_world_model.py)
-
-
-def agent_for(cfg, sd, engine="tcgen05"):
-    from tdmpc2_b200.tdmpc2 import TDMPC2
-    agent = TDMPC2(cfg, device=DEV, engine=engine)
-    agent.model.load_state_dict(sd)
-    return agent
 
 
 def model_for(cfg, sd):

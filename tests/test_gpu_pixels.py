@@ -7,6 +7,7 @@ import torch
 
 from tdmpc2_b200.config import workload
 from tdmpc2_b200.synth import synth_state_dict
+from helpers import compare_with_oracle, planner_for, to_gpu_noise
 
 pytestmark = pytest.mark.gpu
 
@@ -21,14 +22,12 @@ def test_encode_pixel_rows_matches_oracle(E):
     """z = encode(frames) for every shift pair the reference can draw on some environment: 1e-5 (the convolutions are exact
     fp32 products summed in a different order than ATen's; SimNorm outputs are <= 1)."""
     from oracle.plan_oracle import OracleModel
-    from tdmpc2_b200.planner import Planner
     cfg = workload("tiny-rgb", num_envs=E)
     sd = synth_state_dict(cfg, seed=14, perturb=True)
     frames = _frames(cfg, E, 3)
     shift = torch.tensor([[(3 * e) % 7, (5 * e + 6) % 7] for e in range(E)], dtype=torch.float32)
     want = OracleModel(cfg, sd).encode_rgb(frames, shift)
-    pl = Planner(cfg, E, "cuda:0")
-    pl.pack(sd)
+    pl = planner_for(cfg, E, None, sd)
     got = pl.encode_pixel_rows(frames.cuda(), shift.cuda(), out=pl.pix_z).cpu()
     torch.cuda.synchronize()
     assert got.shape == (E, cfg.latent_dim)
@@ -40,8 +39,6 @@ def test_pixel_plan_matches_oracle_and_act_shapes():
     """Full plan() on pixel observations, E = 2, explicit noise (ShiftAug's draw included) vs the oracle; then the
     reference's call shape act(obs[C, 64, 64] on the host) -> action[A] on the host through the CUDA-graph path."""
     from oracle.plan_oracle import draw_noise as oracle_noise, plan_oracle
-    from helpers import compare_with_oracle
-    from tdmpc2_b200.planner import Noise, Planner
     from tdmpc2_b200.tdmpc2 import TDMPC2
     E = 2
     cfg = workload("tiny-rgb", num_envs=E)
@@ -52,13 +49,13 @@ def test_pixel_plan_matches_oracle_and_act_shapes():
     t0 = [True, False]
     on = oracle_noise(cfg, 70, E)
     want = plan_oracle(cfg, sd, frames, t0=t0, prev_mean=prev, noise=on)
-    pl = Planner(cfg, E, "cuda:0")
-    pl.pack(sd)
-    noise = Noise.from_env_major(on.prior, on.r, on.pi, on.qidx, on.expo, on.final, device="cuda", shift=on.shift)
-    action, new_mean, tr = pl.plan(frames.cuda(), None, torch.tensor(t0, dtype=torch.uint8).cuda(), prev.cuda(), noise, trace=True)
+    pl = planner_for(cfg, E, None, sd)
+    action, new_mean, tr = pl.plan(frames.cuda(), None, torch.tensor(t0, dtype=torch.uint8).cuda(), prev.cuda(),
+                                   to_gpu_noise(on), trace=True)
     torch.cuda.synchronize()
     assert torch.allclose(tr["z"].cpu(), want.z, atol=1e-5, rtol=0)
-    n = compare_with_oracle(cfg, tr, action, new_mean, want, on, list(range(E)))
+    n = compare_with_oracle(cfg, tr, action, new_mean, want, on, range(E))
+    print(n)
     assert n["topk"] > 0 and n["values"] > 0, n
     # reference-shaped agent: one environment, host observation in, host action out (graph replay from the 2nd call)
     cfg1 = workload("tiny-rgb", num_envs=1)

@@ -13,7 +13,8 @@ import pytest
 import torch
 
 from helpers import (DEV, OBSERVED, compare_plans, fused_layer_ratio_rule, level_model, mixed_noise, plan_three_ways,
-                     print_ratio_table, row_mode_ratio_rule, slice_noise, trained_obs)
+                     planner_for, row_mode_ratio_rule, slice_noise, trained_obs)
+from helpers import ratio_table  # noqa: F401 (autouse: this module's ratio table)
 
 pytestmark = pytest.mark.gpu
 ENGINES = ["simt", "tcgen05"]
@@ -131,13 +132,6 @@ PRESET_PLAN_OVER = dict(num_samples=256, num_elites=32)
 SATURATED_POLICY = ("a97", "a128", "preset19")
 
 
-@pytest.fixture(scope="module", autouse=True)
-def ratio_table():
-    OBSERVED.clear()
-    yield
-    print_ratio_table()
-
-
 @functools.lru_cache(maxsize=1)
 def model(case, level, **extra):
     wl, over, _, _, _ = CASES[case]
@@ -225,7 +219,6 @@ def test_plan_prior_tile_boundary(engine):
     action of a one-iteration plan.  (A later iteration samples from each implementation's own refit, so its values
     carry that refit's allowed difference times the value's slope in the actions as well as the arithmetic error.)"""
     from oracle.plan_oracle import plan_oracle
-    from tdmpc2_b200.planner import Planner
     cfg, sd = model("pi1_e130", "mid")
     cfg = cfg.replace(**PLAN_OVER)
     reaches("pi1_e130", cfg)
@@ -235,13 +228,11 @@ def test_plan_prior_tile_boundary(engine):
     t0 = torch.tensor([i % 2 == 0 for i in range(E)], dtype=torch.uint8)
     prev = 0.3 * torch.randn(E, cfg.horizon, cfg.action_dim, generator=torch.Generator().manual_seed(5))
     nz, on = mixed_noise(cfg, E, envs, 500)
-    pl = Planner(cfg, E, DEV, engine=engine)
-    pl.pack(sd)
+    pl = planner_for(cfg, E, engine, sd)
     action, new_mean, tr = pl.plan(obs.to(DEV), None, t0.to(DEV), prev.to(DEV), nz, trace=True)
     torch.cuda.synchronize()
     for pair in ([0, 1], [126, 127], [127, 128], [128, 129]):
-        p2 = Planner(cfg.replace(num_envs=2), 2, DEV, engine=engine)
-        p2.pack(sd)
+        p2 = planner_for(cfg.replace(num_envs=2), 2, engine, sd)
         a2, m2, tr2 = p2.plan(obs[pair].to(DEV), None, t0[pair].to(DEV), prev[pair].to(DEV), slice_noise(nz, pair),
                               trace=True)
         torch.cuda.synchronize()
@@ -251,8 +242,7 @@ def test_plan_prior_tile_boundary(engine):
     del pl
     cfg = cfg.replace(iterations=1)
     nz, on = mixed_noise(cfg, E, envs, 500)
-    pl = Planner(cfg, E, DEV, engine=engine)
-    pl.pack(sd)
+    pl = planner_for(cfg, E, engine, sd)
     action, new_mean, tr = pl.plan(obs.to(DEV), None, t0.to(DEV), prev.to(DEV), nz, trace=True)
     torch.cuda.synchronize()
     sel = torch.tensor(envs)

@@ -11,18 +11,11 @@ import functools
 import pytest
 import torch
 
-from helpers import (OBSERVED, compare_plans, fused_layer_ratio_rule, level_model, plan_three_ways, print_ratio_table,
-                     row_mode_ratio_rule)
+from helpers import compare_plans, fused_layer_ratio_rule, level_model, plan_three_ways, row_mode_ratio_rule
+from helpers import ratio_table  # noqa: F401 (autouse: this module's ratio table)
 
 pytestmark = pytest.mark.gpu
 ENGINES = ["simt", "tcgen05"]
-
-
-@pytest.fixture(scope="module", autouse=True)
-def ratio_table():
-    OBSERVED.clear()
-    yield
-    print_ratio_table()
 
 
 # ------------------------------------------------------------------------------------------------- models

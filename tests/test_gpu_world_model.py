@@ -3,6 +3,7 @@ reference's own methods and against the CPU oracle (oracle/wm_oracle.py)."""
 import pytest
 import torch
 
+from helpers import agent_for
 from oracle.wm_oracle import CASES, WMOracle, case_model, load_case, with_target_blend
 
 pytestmark = pytest.mark.gpu
@@ -14,13 +15,6 @@ TOL = {"latent": (2e-6, 1e-5), "pi": (1e-5, 0.0), "value": (5e-5, 1e-5), "entrop
 KIND = {"z": "latent", "next": "latent", "reward": "value", "pi_action": "pi", "pi_mean": "pi", "pi_log_std": "pi",
         "pi_entropy": "entropy", "pi_scaled_entropy": "entropy", "q_all": "value", "qt_all": "value", "q_min": "value",
         "q_avg": "value", "qt_min": "value", "term": "value", "term_logit": "value", "td": "value"}
-
-
-def agent_for(cfg, sd, engine):
-    from tdmpc2_b200.tdmpc2 import TDMPC2
-    agent = TDMPC2(cfg, device=DEV, engine=engine)
-    agent.model.load_state_dict(sd)
-    return agent
 
 
 def check(name, got, want, worst):
